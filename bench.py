@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- mask-loss fwd+bwd ms/img (BoxInst R-50, 800x1024, batch 2/GPU) on N B200s.
+"""bench.py -- mask-loss fwd+bwd ms/img (BoxInst R-50, 800x1024, batch 2/GPU) on N H100s.
 
 Contract (driver): ``python bench.py --gpus N --steps K --warmup W`` prints ONE JSON line on
 rank 0.  N > 1 is launched by torchrun, one rank per GPU; the loss is per image so ranks are
@@ -13,7 +13,7 @@ loss of ONE batch -- 2 images of 3x800x1024, 8 GT boxes each, N=128 sampled inst
   e2e   : through the public head API with HOST (pinned) buffers: H2D of image, logits, boxes ->
           target building (LAB, similarity, rects) -> loss fwd+bwd -> D2H of the gradient + losses.
 L2 hygiene: the timed loop rotates over R input/gradient sets whose footprint (R x 52 MB) exceeds
-the 126 MB L2, so every step streams its logits from HBM.
+the 50 MB L2, so every step streams its logits from HBM.
 
 ``--impl reference`` times the reference's own CPU path (the oracle port, torch-on-CPU with all
 host threads) on a bounded sample: ONE image (64 instances) of the same workload per step.
@@ -29,6 +29,7 @@ ROOT = os.path.dirname(os.path.abspath(__file__))
 if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
 
+import numpy as np  # noqa: E402
 import torch  # noqa: E402
 
 METRIC = 'mask_loss_fwd_bwd_ms_per_img'
@@ -42,21 +43,11 @@ ALGO_BYTES = 3 * N_INST * H * W * 4 + 2 * B_IMG * K_NEIGH * H * W * 4     # SURV
 ROTATE = 8
 
 
-def ncu_traffic_bytes():
-    """DRAM bytes per step from the committed ncu --set full capture (None when the summary is absent)."""
-    path = os.path.join(os.path.dirname(os.path.abspath(__file__)), 'profiles', 'r2_traffic.json')
-    try:
-        with open(path) as f:
-            return float(json.load(f)['step_dram_bytes'])
-    except (OSError, KeyError, ValueError):
-        return None
-
-
 def measured_peak_gbs():
     p = os.path.join(ROOT, 'MEASURED_PEAKS.json')
     if os.path.exists(p):
         return float(json.load(open(p))['hbm_gbs']), 'measured (MEASURED_PEAKS.json hbm_gbs)'
-    return 6650.0, 'fallback (B200_PROFILING.md 6.65 TB/s)'
+    return 3350.0, 'fallback (H100 SXM data sheet: 3.35 TB/s HBM3)'
 
 
 class ClockSampler(threading.Thread):
@@ -92,29 +83,6 @@ class ClockSampler(threading.Thread):
         self.join(timeout=2)
         s = sorted(self.samples)
         return {'sm_mhz': s[len(s) // 2] if s else None, 'sm_max_mhz': self.max_mhz, 'reasons': sorted(self.reasons)}
-
-
-def pin_to_numa_node(local_rank, world=1):
-    """Keep this rank's host threads (launch loop, pinned-memory staging) on the CPU socket its GPU hangs off: the e2e
-    path moves 72 MB / step / rank over PCIe, and round 1's 8-rank e2e lost ~35 % to cross-socket traffic and launch
-    contention.  Topology of the 8 x B200 boxes of this pool (SCALE_r01.json): GPUs 0-3 <-> CPUs 0-31,64-95; GPUs 4-7 <->
-    CPUs 32-63,96-127.  Best effort: any failure leaves the affinity alone."""
-    try:
-        ncpu = os.cpu_count() or 0
-        if ncpu < 128 or not hasattr(os, 'sched_setaffinity'):
-            return None
-        half = ncpu // 4
-        node = 0 if local_rank < 4 else 1
-        cpus = set(range(node * half, (node + 1) * half)) | set(range(2 * half + node * half, 2 * half + (node + 1) * half))
-        # one slice of the node per rank so that the ranks of a socket do not fight for the same cores
-        per = min(4, max(1, (world + 1) // 2))          # ranks sharing this socket
-        mine = sorted(cpus)[(local_rank % 4 % per) * (len(cpus) // per):(local_rank % 4 % per + 1) * (len(cpus) // per)]
-        os.sched_setaffinity(0, mine)
-        if world > 1:
-            torch.set_num_threads(max(1, min(8, len(mine))))
-        return f'{mine[0]}-{mine[-1]} ({len(mine)} cpus, numa node {node})'
-    except Exception:  # noqa: BLE001
-        return None
 
 
 def ddp_allreduce_leg(dist, dev, world, loss_step, steps):
@@ -288,8 +256,44 @@ def run_gpu_reference(case, dev, iters=10, ours_grad=None):
             'loss_prj': float(prj.detach()), 'loss_pairwise': float(pair.detach())}
 
 
+DUMP_BUDGET = 64 << 20          # bytes of .npy data one --dump-outputs may write
+STEP_OUTPUTS = ('loss_prj', 'loss_pairwise', 'grad_logits')     # what one config-A step hands its caller
+
+
+def step_outputs(out, prefix=''):
+    """{name: tensor} of what a step returns to its caller (tensors nested in dicts / tuples / lists, in order)."""
+    if torch.is_tensor(out):
+        return {prefix or 'out': out}
+    items = out.items() if isinstance(out, dict) else enumerate(out) if isinstance(out, (list, tuple)) else ()
+    res = {}
+    for k, v in items:
+        res.update(step_outputs(v, f'{prefix}_{k}' if prefix else str(k)))
+    return res
+
+
+def dump_outputs(out_dir, named):
+    """Writes every output as out_dir/<name>.npy (float64 stays float64, everything else becomes float32).  When the
+    whole set exceeds DUMP_BUDGET, each output larger than its equal share keeps a fixed sample of its flattened entries
+    (randperm seeded with 0, sorted), so two builds given the same arguments write comparable files."""
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {k: v.detach().to('cpu', torch.float64 if v.dtype == torch.float64 else torch.float32) for k, v in named.items()}
+    total = sum(a.numel() * a.element_size() for a in arrays.values())
+    share = DUMP_BUDGET // max(len(arrays), 1)
+    written = {}
+    for k, a in arrays.items():
+        shape = list(a.shape)
+        if total > DUMP_BUDGET and a.numel() * a.element_size() > share:
+            keep = share // a.element_size()
+            idx = torch.randperm(a.numel(), generator=torch.Generator().manual_seed(0))[:keep].sort().values
+            a = a.flatten()[idx]
+        name = ''.join(c if c.isalnum() or c in '._-' else '_' for c in k)
+        np.save(os.path.join(out_dir, name + '.npy'), a.numpy())
+        written[name] = {'shape': shape, 'saved': list(a.shape), 'dtype': str(a.dtype).replace('torch.', '')}
+    return written
+
+
 # ------------------------------------------------------------------------------------------
-# B200 arm
+# CUDA arm
 # ------------------------------------------------------------------------------------------
 FWD_BYTES = N_INST * H * W * 4 + B_IMG * K_NEIGH * H * W * 4            # read logits + similarity      (29.5 MB)
 BWD_BYTES = 2 * N_INST * H * W * 4 + B_IMG * K_NEIGH * H * W * 4        # re-read logits, write gradient (55.7 MB)
@@ -303,7 +307,6 @@ def main_cuda(args, rank, world, local_rank):
     lib = L.lib()                                # fail loudly if the CUDA extension is missing
     dev = torch.device('cuda', local_rank)
     torch.cuda.set_device(dev)
-    pinned_cpus = pin_to_numa_node(local_rank, world)
     dist = None
     if world > 1:
         import torch.distributed as dist
@@ -343,7 +346,7 @@ def main_cuda(args, rank, world, local_rank):
         prj, pair = boxinst_mask_loss(x, targets, gt_inds32, it, plan=plan)
         torch.autograd.backward([prj, pair], [ones, ones])
         grad_ring[i % ROTATE], x.grad = x.grad, None
-        return prj, pair
+        return prj, pair, grad_ring[i % ROTATE]
 
     def barrier():
         if dist is not None:
@@ -364,6 +367,7 @@ def main_cuda(args, rank, world, local_rank):
     for i in range(warm):
         step(i)
     ms_eager = timed(step, args.steps)
+    last_outputs = dict(zip(STEP_OUTPUTS, step(args.steps - 1))) if args.dump_outputs else None   # eager: the last step again
 
     # ---- the same step (public autograd op, forward + backward) captured once per rotating input set
     #      into CUDA graphs: removes the ~0.2 ms/step of Python/autograd launch overhead ----
@@ -410,6 +414,8 @@ def main_cuda(args, rank, world, local_rank):
         ms_step = samples[REGIONS // 2] / args.steps
         ms_step_spread = (samples[0] / args.steps, samples[-1] / args.steps)
         steps_timed = args.steps
+        if args.dump_outputs:
+            last_outputs = dict(zip(STEP_OUTPUTS, graphs[-1]))     # the graph replayed last ends with the last captured step
         mode = f'cuda_graph ({ROTATE} steps per graph' + (f' + one tail graph of {tail}' if tail else '') + \
             f'); median of {REGIONS} timed regions of {args.steps} steps'
     except Exception as e:  # noqa: BLE001
@@ -544,21 +550,19 @@ def main_cuda(args, rank, world, local_rank):
         'steps': steps_timed, 'warmup': warm, 'ms_per_step': ms_step, 'higher_is_better': False, 'scaling': 'weak',
         'vs_baseline': None, 'dtype': 'f32', 'data': 'synthetic',
         'config': {'workload': WORKLOAD,
-                   'l2': f'inputs rotate over {ROTATE} logit/grad sets ({ROTATE * 52} MB > 126 MB L2)',
+                   'l2': f'inputs rotate over {ROTATE} logit/grad sets ({ROTATE * 52} MB > 50 MB L2)',
                    'launch': mode, 'eager_ms_per_step': ms_eager,
                    'e2e_mode': 'CondInstMaskHead.loss + backward from pinned host buffers, 2 steps in flight on 2 streams',
                    'parallelism': f'replicas x{world} (loss is per image; no data-path collective)',
                    'aggregate_img_per_s': world * B_IMG / (ms_step * 1e-3)},
         'roofline': {'bound': 'hbm', 'achieved': achieved, 'peak': peak, 'unit': 'GB/s', 'frac': achieved / peak,
-                     'traffic': ncu_traffic_bytes(),
-                     'traffic_source': 'profiles/r2_traffic.json (ncu --set full, dram read+write per launch, summed over the '
-                                       'kernels of one step)',
+                     'traffic': None,
                      'peak_source': peak_src,
                      'note': 'headline = the WHOLE step (wq_main + wq_finalize + onepass_backward kernels, CUDA-graph replay '
                              'through the public autograd op) against the 85.2 MB/step ALGORITHMIC figure of SURVEY 8d '
                              '(logits read in fwd and in bwd + gradient written + similarity read twice).  The single-pass '
                              'schedule moves 52.5 MB (logits once, gradient once, edge bytes): see kernels.*; the dominant '
-                             'kernel is wq_main_kernel (its share of the step: profiles/r2_launches_bench.csv)',
+                             'kernel is wq_main_kernel',
                      'kernels': {'single_pass_forward(wq_main+wq_finalize)': {
                                      'us': us_one_fwd, 'moved_mb': ONEPASS_BYTES / 1e6,
                                      'achieved_moved': ONEPASS_BYTES / (us_one_fwd * 1e-6) / 1e9,
@@ -579,9 +583,7 @@ def main_cuda(args, rank, world, local_rank):
     }
     if ddp is not None:
         line['ddp_allreduce'] = ddp
-    if pinned_cpus:
-        line['config']['cpu_affinity_rank0'] = pinned_cpus
-    # the B200 arm's own results on logit set 0 (the set the gpu_reference leg uses)
+    # the CUDA arm's own results on logit set 0 (the set the gpu_reference leg uses)
     x0 = logit_sets[0].detach().clone().requires_grad_(True)
     p0, q0 = boxinst_mask_loss(x0, targets, gt_inds32, it, plan=plan)
     (g0,) = torch.autograd.grad(p0 + q0, x0)
@@ -604,8 +606,10 @@ def main_cuda(args, rank, world, local_rank):
                     'rel_err_loss_prj': abs(line['losses']['loss_prj'] - rp) / abs(rp),
                     'rel_err_loss_pairwise': abs(line['losses']['loss_pairwise'] - rq) / abs(rq),
                     'rel_err_grad': ref_gpu.pop('_grad_rel_err', None),
-                    'what': 'B200 arm vs the restated reference loss around the reference CUDA pairwise op, same logits (set 0), '
+                    'what': 'CUDA arm vs the restated reference loss around the reference CUDA pairwise op, same logits (set 0), '
                             'same targets; bar: 1e-3 (BASELINE.json north_star)'}
+    if last_outputs is not None:
+        line['dumped_outputs'] = dump_outputs(args.dump_outputs, last_outputs)
     print(json.dumps(line), flush=True)
     if dist is not None:
         dist.destroy_process_group()
@@ -637,7 +641,7 @@ def main_config(args, rank, world, local_rank):
     sampler = ClockSampler(local_rank)
     sampler.start()
     cfg = args.config
-    # rotate over R independent input sets so that a step never finds its inputs in the 126 MB L2
+    # rotate over R independent input sets so that a step never finds its inputs in the 50 MB L2
     set_mb = dict(C=110, D=30, E=75)[cfg]
     R = max(2, -(-140 // set_mb))
     built = [bc.BUILDERS[cfg](dev, 1234 + rank + 100 * r) for r in range(R)]
@@ -663,9 +667,16 @@ def main_config(args, rank, world, local_rank):
     for i in range(max(warm, R)):
         steps_fn[i % R]()
     steps = max(args.steps, 1)
-    ms_eager = timed(lambda i: steps_fn[i % R](), steps)
+    last = []
+
+    def eager_step(i):
+        out = steps_fn[i % R]()
+        if i == steps - 1:
+            last[:] = [out]
+        return out
+    ms_eager = timed(eager_step, steps)
     mode, ms_step, steps_timed = 'eager', ms_eager, steps
-    try:                                          # the same steps as ONE CUDA graph of R consecutive steps
+    try:                                          # the same steps as CUDA graphs of R consecutive steps
         side = torch.cuda.Stream()
         side.wait_stream(torch.cuda.current_stream())
         with torch.cuda.stream(side):
@@ -673,16 +684,27 @@ def main_config(args, rank, world, local_rank):
                 steps_fn[r]()
         torch.cuda.current_stream().wait_stream(side)
         torch.cuda.synchronize()
-        g = torch.cuda.CUDAGraph()
-        keep = []
-        with torch.cuda.graph(g):
-            for r in range(R):
-                keep.append(steps_fn[r]())
-        g.replay()
-        reps = max(steps // R, 1)
-        ms_step = timed(lambda i: g.replay(), reps) / R
-        steps_timed = reps * R
-        mode = f'cuda_graph ({R} steps per graph)'
+
+        def capture(n):
+            gr, keep = torch.cuda.CUDAGraph(), []
+            with torch.cuda.graph(gr):
+                for r in range(n):
+                    keep.append(steps_fn[r]())
+            gr.replay()
+            return gr, keep
+        # EXACTLY `steps` timed steps: full graphs of R steps + one tail graph of steps % R
+        full, tail = steps // R, steps % R
+        g, keep = capture(R)
+        g_tail, keep_tail = capture(tail) if tail else (None, None)
+
+        def region(_i):
+            for _ in range(full):
+                g.replay()
+            if g_tail is not None:
+                g_tail.replay()
+        ms_step = timed(region, 1) / steps
+        last[:] = [keep_tail[-1] if tail else keep[-1]]
+        mode = f'cuda_graph ({R} steps per graph' + (f' + one tail graph of {tail}' if tail else '') + ')'
     except Exception as e:  # noqa: BLE001
         mode = f'eager (graph capture failed: {type(e).__name__}: {str(e)[:80]})'
     clocks = sampler.stop()
@@ -699,14 +721,14 @@ def main_config(args, rank, world, local_rank):
         'warmup': warm, 'ms_per_step': ms_step, 'higher_is_better': False, 'scaling': 'weak', 'vs_baseline': None,
         'dtype': 'f32', 'data': 'synthetic',
         'config': {'workload': info['workload'], 'gradients': info['grads'],
-                   'l2': f'inputs rotate over {R} independent sets (> 126 MB L2 in total)',
+                   'l2': f'inputs rotate over {R} independent sets (> 50 MB L2 in total)',
                    'launch': mode, 'eager_ms_per_step': ms_eager,
                    'parallelism': f'replicas x{world} (loss is per image; no data-path collective)'},
         'roofline': {'bound': 'hbm', 'achieved': achieved, 'peak': peak, 'unit': 'GB/s', 'frac': achieved / peak,
                      'traffic': None, 'peak_source': peak_src, 'algorithmic_bytes_per_step': info['algo_bytes'],
                      'algorithmic_bytes': info['algo'],
                      'note': 'whole step against the HBM lower bound of SURVEY 8d; the tree-filter / mean-field / LCM kernels are '
-                             'dependency-latency bound (levels / iterations), see profiles/r2_notes.md for the per-kernel ncu summaries'},
+                             'dependency-latency bound (levels / iterations)'},
         'e2e': {'value': ms_eager / (imgs * world), 'unit': 'ms/img', 'h2d_bytes_per_step': 0, 'd2h_bytes_per_step': 0,
                 'note': 'eager launch through the public head API (Python + autograd overhead included); inputs are feature maps '
                         'produced on the device by the network, so there is no host copy on this path'},
@@ -736,6 +758,8 @@ def main_config(args, rank, world, local_rank):
                     'loss_reference': float(rl[0].detach()) if hasattr(rl[0], 'detach') else float(rl[0]), 'loss_b200': float(ours_loss.detach()) if hasattr(ours_loss, 'detach') else float(ours_loss)}
         except Exception as e:  # noqa: BLE001
             line['gpu_reference'] = {'unavailable': f'{type(e).__name__}: {e}'[:300]}
+    if args.dump_outputs:
+        line['dumped_outputs'] = dump_outputs(args.dump_outputs, step_outputs(last[0]))
     print(json.dumps(line), flush=True)
     if dist is not None:
         dist.destroy_process_group()
@@ -748,6 +772,8 @@ def main():
     ap.add_argument('--warmup', type=int, default=5)
     ap.add_argument('--impl', default='b200', choices=['b200', 'reference'])
     ap.add_argument('--no-cpu-baseline', action='store_true')
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                    help='after the timed steps, write what the last timed step computed as DIR/<name>.npy')
     ap.add_argument('--config', default='A', choices=['A', 'C', 'D', 'E'],
                     help='A (default, the headline): BoxInst; C: DiscoBox; D: BoxLevelset; E: Box2Mask (BASELINE.json configs)')
     args = ap.parse_args()

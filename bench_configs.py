@@ -2,12 +2,12 @@
 (configs[2..4]) on the synthetic shapes of SURVEY.md section 8d.  Imported by bench.py; prints nothing itself.
 
   C  DiscoBox R-50 800x1024      mask_feat [2,256,200,256], 16 positive kernels / image -> per-image dynamic conv (a3,
-                                  tcgen05) -> MIL dice + mean-field teacher + dice (a6, a16, a17), fwd + bwd wrt mask_feat
+                                  wgmma) -> MIL dice + mean-field teacher + dice (a6, a16, a17), fwd + bwd wrt mask_feat
                                   and the kernels.                                   discobox_head.py:1206-1300
   D  BoxLevelset R-50 800x1024   5 levels x 16 instances (8 / image) at 200x256, 200x256, 100x128, 50x64, 50x64:
                                   projection + two level-set terms + two tree filters per level (a6, a9, a12-a15, a17),
                                   fwd + bwd wrt the mask logits and the level-set features.   box_solov2_head.py:334-367
-  E  Box2Mask 1024x1024, 1 img   mask_pred = einsum(100 queries, [256,256,256] feature) (a4, tcgen05), 8 matched queries,
+  E  Box2Mask 1024x1024, 1 img   mask_pred = einsum(100 queries, [256,256,256] feature) (a4, wgmma), 8 matched queries,
                                   10 decoder layers: projection + level-set + tree filter at 96x96 + LCM (a6, a9, a11-a15,
                                   a17, a18), fwd + bwd wrt the mask feature, the queries and the level-set feature.
                                                                                       box2mask_head.py:229-359

@@ -1,4 +1,4 @@
-"""boxinstseg_b200 -- B200-native (sm_100a) box-supervised mask-loss hot path of BoxInstSeg.
+"""boxinstseg_b200 -- H100 (sm_90a) box-supervised mask-loss hot path of BoxInstSeg.
 
 Layout mirrors the part of the reference it drops into:
   ops/pairwise, ops/tree_filter   <->  mmdet/ops/{pairwise,tree_filter}

@@ -1,4 +1,4 @@
-"""In-tree build of libboxseg_b200.so (sm_100a only) with nvcc; no torch involved.
+"""In-tree build of libboxseg_b200.so (sm_90a, H100) with nvcc; no torch involved.
 
     python -m boxinstseg_b200.build [--force] [--verbose]
 
@@ -17,7 +17,7 @@ LIBDIR = os.path.join(HERE, 'lib')
 LIB = os.path.join(LIBDIR, 'libboxseg_b200.so')
 INCLUDE = os.path.join(os.path.dirname(HERE), 'include')
 
-NVCC_FLAGS = ['-gencode', 'arch=compute_100a,code=sm_100a', '-O3', '-lineinfo', '-std=c++17',
+NVCC_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-O3', '-lineinfo', '-std=c++17',
               '-Xcompiler', '-fPIC', '--expt-relaxed-constexpr', '-I', INCLUDE]
 
 
@@ -58,7 +58,7 @@ def build(force=False, verbose=False):
             if verbose and log:
                 print(log)
     if jobs or force or not os.path.exists(LIB):
-        run([_nvcc(), '-shared', '-o', LIB] + objs + ['-gencode', 'arch=compute_100a,code=sm_100a'])
+        run([_nvcc(), '-shared', '-o', LIB] + objs + ['-gencode', 'arch=compute_90a,code=sm_90a'])
     return LIB
 
 

@@ -20,10 +20,10 @@ void set_last_error(cudaError_t e) {
 int sm_count() {
   static thread_local int cached_dev = -1, cached = 0;
   int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess) return 148;
+  if (cudaGetDevice(&dev) != cudaSuccess) return 132;
   if (dev != cached_dev) {
     cudaDeviceProp p;
-    if (cudaGetDeviceProperties(&p, dev) != cudaSuccess) return 148;
+    if (cudaGetDeviceProperties(&p, dev) != cudaSuccess) return 132;
     cached = p.multiProcessorCount;
     cached_dev = dev;
   }

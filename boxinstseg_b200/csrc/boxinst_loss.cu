@@ -2,7 +2,7 @@
 // backward.  Replaces the arithmetic of CondInstMaskHead.loss, condinst_head.py:1288-1343
 // (sigmoid -> compute_project_term :134-143 -> pairwise_nlog -> threshold weights -> reduction).
 //
-// B200-first design (DESIGN.md "BoxInst loss"):
+// Design (DESIGN.md "BoxInst loss"):
 //   * the [N,8,H,W] pairwise tensor, the [N,8,H,W] gathered similarity and the [N,1,H,W] gathered
 //     bitmask of the reference are never materialised.  The similarity enters as ONE BYTE per
 //     pixel per image (bit c = sim[c] >= thresh) and the box bitmask as 4 integers per GT.

@@ -4,7 +4,7 @@
 //
 // Why: the CTA-granular kernel (onepass_main_kernel) spent 31 % of its duration with SMs idle (per-CTA prologue of
 // 128 record loads + a block scan, a tail of CTA-wide pair items), its top stall was the CTA barrier around the strip
-// buffers, and its finalize kernel re-scaled the whole box span (profiles/r1_ncu_full_onepass.csv).  Here
+// buffers, and its finalize kernel re-scaled the whole box span.  Here
 //   * the work list is a PLAN built once per target set (wq_count_kernel + wq_build_kernel): instance records, every
 //     pair item as a 32-byte descriptor (long chains first) and the logit-independent weight total -- the main kernel
 //     has no prologue beyond one header load;

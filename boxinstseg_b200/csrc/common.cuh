@@ -1,12 +1,12 @@
-// Shared device/host helpers for the boxseg_b200 kernels (sm_100a only).
+// Shared device/host helpers for the boxseg_b200 kernels (sm_90a, H100).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
 
 #include "../../include/boxseg_b200.h"
 
-#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ < 1000)
-#error "boxseg_b200 is written for sm_100a (B200) only"
+#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ != 900)
+#error "boxseg_b200 is written for sm_90a (H100) only"
 #endif
 
 namespace bxs {

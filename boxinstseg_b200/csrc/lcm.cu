@@ -255,8 +255,8 @@ extern "C" int bxs_lcm_forward(const float* imgs, const float* phis, const float
   affinity_kernel<<<grid_for(total, 256), 256, 0, st>>>(imgs, aff, (int)C, (int)h, (int)w, dilation, total);
   const size_t sm = 2 * hw * sizeof(float);
   // One CTA per instance keeps phi in shared memory for all iterations, but it is ONE SM per instance: 8 instances of a
-  // 96x96 map ran on 8 of 148 SMs, issue-bound, 106 us forward / 324 us backward (config E: 16 % of the step).  Unless the
-  // instances fill the machine that way, run the iterations as grid-wide kernels (phi ping-pongs through L2; same arithmetic
+  // 96x96 map run on 8 of 132 SMs, issue-bound.
+  // Unless the instances fill the machine that way, run the iterations as grid-wide kernels (phi ping-pongs through L2; same arithmetic
   // per pixel, same results; the launches are graph-captured by the callers).
   if (sm <= kMaxFusedSmem && n >= 2 * (int64_t)sm_count()) {
     cudaFuncSetAttribute(lcm_fused_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMaxFusedSmem);

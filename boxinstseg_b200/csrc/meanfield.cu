@@ -209,8 +209,8 @@ extern "C" int bxs_meanfield_forward_inter(const float* K, const int32_t* obj_im
   const int64_t hw = h * w;
   const size_t sm = 2 * ((hw + 15) / 16) * 16;
   // One CTA per object keeps both bit maps in shared memory for all rounds, but it is ONE SM per object: a round of a
-  // 200x256 map is ~4500 instructions per thread, 1.6 ms for 10 rounds whatever the number of objects (r1: 16 objects on
-  // 16 of 148 SMs).  Unless there are enough objects to fill the machine that way, run the rounds as grid-wide
+  // 200x256 map is ~4500 instructions per thread, whatever the number of objects (16 objects run on 16 of 132 SMs).
+  // Unless there are enough objects to fill the machine that way, run the rounds as grid-wide
   // kernels over all objects' pixels (bit maps ping-pong through L2; the launches are graph-captured by the callers).
   const bool per_object = sm <= kMaxFusedSmem && (n >= 2 * (int64_t)sm_count() || !workspace);
   if (per_object) {

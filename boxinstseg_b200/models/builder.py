@@ -3,7 +3,7 @@
 The reference builds heads and losses from config dicts through mmcv registries
 (mmdet/models/builder.py:7-59: ``HEADS = LOSSES = MODELS``).  When the reference's ``mmdet`` is
 importable the classes of this package are registered INTO its registries with ``force=True``
-under the reference's own names, so ``configs/boxinst/*.py`` etc. build the B200 implementations
+under the reference's own names, so ``configs/boxinst/*.py`` etc. build the CUDA implementations
 unchanged after ``import boxinstseg_b200.models``.  Without mmcv/mmdet (this image) a minimal
 registry with the same ``register_module`` / ``build`` behaviour is used.
 """

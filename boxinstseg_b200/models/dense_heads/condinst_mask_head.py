@@ -3,7 +3,7 @@
 Same constructor kwargs, buffers (``sizes_of_interest``, ``_iter``), ``param_conv`` attribute and
 ``forward`` / ``loss`` / ``get_targets`` methods as the reference, so
 ``configs/boxinst/boxinst_r50_fpn_1x_coco.py`` builds it unchanged; the arithmetic runs in the
-sm_100a kernels of libboxseg_b200:
+sm_90a kernels of libboxseg_b200:
   forward      -> ops.condinst.dynamic_mask_head   (a1: rel-coords + 3 dynamic 1x1 convs + aligned x2)
   get_targets  -> ops.boxinst.boxinst_targets      (a5: no host round trip, no per-GT Python loop)
   loss         -> ops.boxinst.boxinst_mask_loss    (a6+a7+a8 fused; no [N,8,H,W] tensors)

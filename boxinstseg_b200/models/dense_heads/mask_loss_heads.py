@@ -191,7 +191,7 @@ class DiscoBoxSOLOv2Head(nn.Module):
                     use_ind_teacher=False, best=True, conv=None):
         """From the raw head outputs to the per-level lists of ``mask_loss`` / ``corr_loss_levels``: SOLO targets of every image
         (``best_target_single`` for corr_loss, ``solov2_target_single`` with ``best=False``), the dynamic kernels of the covered
-        cells gathered by ``grid_order``, one dynamic convolution per (level, image) with objects (a3: the tcgen05 kernel).
+        cells gathered by ``grid_order``, one dynamic convolution per (level, image) with objects (a3: the wgmma kernel).
         ``*_kernel_preds_raw``: per level [B,C,g,g]; ``*_ins_pred`` [B,C,H,W]; ``gt_mask_list``: per image uint8 [G,H',W'] device
         tensors.  Returns (s_ins_pred_list, t_ins_pred_list, img_ind_list, ins_labels, kernel_label_list) with None for a level
         without objects.  Plain torch around ``conv`` (default: ``self.dynamic_conv``)."""

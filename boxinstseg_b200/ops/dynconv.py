@@ -1,8 +1,8 @@
-"""a2/a3/a4: dense dynamic 1x1 convolution ``out[b,i] = sum_c kernel[b,i,c] * feat[b,c]`` on tcgen05.
+"""a2/a3/a4: dense dynamic 1x1 convolution ``out[b,i] = sum_c kernel[b,i,c] * feat[b,c]`` on Hopper wgmma.
 
-Forward is the hand-written TMA + tcgen05 (TF32, FP32 accumulate in TMEM) kernel of libboxseg_b200.
+Forward is the hand-written TMA + wgmma (TF32, FP32 accumulate in registers) kernel of libboxseg_b200.
 Backward is the same machinery (bxs_dynconv1x1_backward): d/d feat = kernel^T . g_out re-uses the forward kernel with
-the operand roles swapped, d/d kernel = g_out . feat^T is a split-K tcgen05 kernel over the pixels with an ordered
+the operand roles swapped, d/d kernel = g_out . feat^T is a split-K wgmma kernel over the pixels with an ordered
 (deterministic) reduction of the partials.  Only d/d feat with more than 256 kernels per image (outside every reference
 call site: the heads convolve the POSITIVE kernels of an image) goes through cuBLAS (torch.bmm).
 """

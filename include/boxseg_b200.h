@@ -1,5 +1,5 @@
 /*
- * boxseg_b200 -- C ABI of the B200-native (sm_100a) box-supervised mask-loss hot path.
+ * boxseg_b200 -- C ABI of the H100 (sm_90a) box-supervised mask-loss hot path.
  *
  * This is the drop-in boundary (SURVEY.md section 8b): every entry point takes raw DEVICE
  * pointers + sizes + the CUDA stream to launch on, allocates nothing, keeps no state and
@@ -308,7 +308,7 @@ int bxs_refine_backward_weight(const float* edge_weight, const int32_t* sorted_i
                                int64_t V, bxs_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------
- * a2/a3/a4  dense dynamic 1x1 convolution on the 5th-gen tensor cores (tcgen05 + TMEM, TMA fed)
+ * a2/a3/a4  dense dynamic 1x1 convolution on the Hopper tensor cores (wgmma, TMA fed)
  *     replaces F.conv2d(feature.view(1,B*C,h,w), kernel[B*S*S,C,1,1], groups=B)
  *       (mmdet/models/dense_heads/box_solov2_head.py:209-211),
  *     F.conv2d(mask_feat[1,C,h,w], kernels[I,C,1,1]) (mmdet/models/dense_heads/discobox_head.py:1219) and
@@ -320,8 +320,8 @@ int bxs_dynconv1x1_forward(const float* feat, const float* kernels, float* out, 
                            int64_t I, bxs_stream_t stream);
 
 /* Backward of the dynamic 1x1 convolution (autograd of the same call sites; the reference gets it from cuDNN / cuBLAS):
- *   g_feat    [B,C,P] = kernels^T . g_out   (tcgen05: the forward kernel with the operand roles swapped; I <= 256)
- *   g_kernels [B,I,C] = g_out . feat^T      (tcgen05 split-K over the pixels + an ordered reduction: deterministic)
+ *   g_feat    [B,C,P] = kernels^T . g_out   (wgmma: the forward kernel with the operand roles swapped; I <= 256)
+ *   g_kernels [B,I,C] = g_out . feat^T      (wgmma split-K over the pixels + an ordered reduction: deterministic)
  * Either output may be NULL (not needed).  TF32 inputs, FP32 accumulation.  workspace:
  * bxs_dynconv1x1_backward_workspace_bytes(B, C, P, I) bytes.  BXS_ERR_UNSUPPORTED: the forward's shape rules, or g_feat with
  * I > 256. */

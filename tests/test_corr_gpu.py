@@ -161,7 +161,7 @@ def test_corr_loss_levels_against_oracle():
 
 def test_head_corr_loss_with_the_reference_signature():
     """DiscoBoxSOLOv2Head.corr_loss (discobox_head.py:900-1139) from the raw head outputs: SOLO targets, kernel gathering, the
-    tcgen05 dynamic convolutions (against F.conv2d on the same tensors, TF32 tolerance), the colour features (align_corners=True
+    wgmma dynamic convolutions (against F.conv2d on the same tensors, TF32 tolerance), the colour features (align_corners=True
     resize), and two training steps of the level body on top of them (the first fills the bank): finite values, a gradient to the
     mask features, the kernels and the RoI feature map, the bank advancing."""
     import torch.nn.functional as F

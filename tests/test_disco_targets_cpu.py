@@ -64,7 +64,7 @@ def test_no_ground_truth_and_all_masks_empty(best):
 def test_head_inputs_from_raw_outputs_equal_reference_loops(best):
     """DiscoBoxSOLOv2Head.corr_inputs (discobox_head.py:917-1003 / 1161-1260): targets of every image, kernels gathered by
     grid_order, one dynamic convolution per (level, image) -- against the oracle's loop form, with F.conv2d standing in for the
-    tcgen05 kernel (the glue is plain torch; the kernel has its own GPU parity tests)."""
+    wgmma kernel (the glue is plain torch; the kernel has its own GPU parity tests)."""
     import torch.nn.functional as F
     from boxinstseg_b200.models import build_head
     from oracle import corr as oc

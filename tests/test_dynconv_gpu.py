@@ -1,4 +1,4 @@
-"""GPU parity of the tcgen05 dynamic 1x1 convolution (a2/a3/a4) against a float64 reference.
+"""GPU parity of the wgmma dynamic 1x1 convolution (a2/a3/a4) against a float64 reference.
 Tolerance 1e-3 of the output's scale: TF32 operands (10-bit mantissa), FP32 accumulation -> ~3e-4 at K = 256 (forward,
 d/d feat) and at K = 51 200 pixels (d/d kernel; the rounding errors are independent, the sum grows like sqrt(K) as
 the result does); the reference's own cuDNN conv2d runs in TF32 by default on Ampere and later GPUs.  Inputs that

@@ -1,4 +1,4 @@
-"""Per-operator timings on the GPU box at the shapes of SURVEY section 8d (configs C/D/E): dynamic conv (tcgen05, forward and
+"""Per-operator timings on the GPU box at the shapes of SURVEY section 8d (configs C/D/E): dynamic conv (wgmma, forward and
 both gradients, against cuBLAS TF32 and FP32), CondInst head, tree filter (MST / BFS / refine), level set (dense op and the
 fused assembly), projection, LCM, mean field, targets.  Every op is timed twice: eager (launch overhead included) and as a
 CUDA-graph replay (`*_graph_us`; device time only).  Prints one JSON object."""
@@ -12,7 +12,7 @@ import torch.nn.functional as F  # noqa: E402
 
 dev = torch.device('cuda:0')
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-PEAK = json.load(open(os.path.join(ROOT, 'MEASURED_PEAKS.json')))['hbm_gbs'] if os.path.exists(os.path.join(ROOT, 'MEASURED_PEAKS.json')) else 6567.7
+PEAK = json.load(open(os.path.join(ROOT, 'MEASURED_PEAKS.json')))['hbm_gbs'] if os.path.exists(os.path.join(ROOT, 'MEASURED_PEAKS.json')) else 3350.0   # H100 SXM data sheet
 
 
 def timeit(fn, reps=20, warm=3):

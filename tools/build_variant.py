@@ -23,5 +23,5 @@ for src in B.sources():
         objs.append(obj)
     else:
         objs.append(base)          # unchanged sources: reuse the main build's objects
-subprocess.run([B._nvcc(), '-shared', '-o', out] + objs + ['-gencode', 'arch=compute_100a,code=sm_100a'], check=True)
+subprocess.run([B._nvcc(), '-shared', '-o', out] + objs + ['-gencode', 'arch=compute_90a,code=sm_90a'], check=True)
 print(out)

@@ -14,7 +14,7 @@ if len(sys.argv) > 1 and sys.argv[1] == 'build':
         if 'onepass' in src or not os.path.exists(obj) or os.path.getmtime(obj) < max(os.path.getmtime(src), B._headers_mtime()):
             subprocess.run([B._nvcc()] + B.NVCC_FLAGS + ['-DBXS_OP_TRACE', '-c', src, '-o', obj], check=True)
         objs.append(obj)
-    subprocess.run([B._nvcc(), '-shared', '-o', TRACE_LIB] + objs + ['-gencode', 'arch=compute_100a,code=sm_100a'], check=True)
+    subprocess.run([B._nvcc(), '-shared', '-o', TRACE_LIB] + objs + ['-gencode', 'arch=compute_90a,code=sm_90a'], check=True)
     print(TRACE_LIB); sys.exit(0)
 import ctypes
 import numpy as np, torch
