@@ -49,9 +49,6 @@ SIGNATURES = {
     'bxs_projection_workspace_bytes': [c_i64] * 3,
     'bxs_projection_loss_forward': [c_p] * 4 + [c_i64] * 3 + [c_f, c_f, c_p],
     'bxs_projection_loss_backward': [c_p] * 3 + [c_i64] * 3 + [c_p],
-    'bxs_levelset_workspace_bytes': [c_i64],
-    'bxs_levelset_loss_forward': [c_p] * 5 + [c_i64] * 4 + [c_f, c_p],
-    'bxs_levelset_loss_backward': [c_p] * 7 + [c_i64] * 4 + [c_f, c_p],
     'bxs_length_reg_forward': [c_p] * 3 + [c_i64] * 4 + [c_p],
     'bxs_length_reg_backward': [c_p] * 3 + [c_i64] * 4 + [c_p],
     'bxs_lcm_workspace_bytes': [c_i64] * 3,
@@ -59,18 +56,13 @@ SIGNATURES = {
     'bxs_lcm_backward': [c_p] * 5 + [c_i64] * 3 + [c_int, c_int, c_p],
     'bxs_meanfield_kernel': [c_p, c_p] + [c_i64] * 4 + [c_int, c_f, c_f, c_f, c_p],
     'bxs_meanfield_workspace_bytes': [c_i64] * 3,
-    'bxs_meanfield_forward': [c_p] * 8 + [c_i64] * 3 + [c_int, c_int, c_p],
     'bxs_meanfield_forward_inter': [c_p] * 5 + [c_f] + [c_p] * 4 + [c_i64] * 3 + [c_int, c_int, c_p],
     'bxs_mst_workspace_bytes': [c_i64] * 3,
     'bxs_mst_forward': [c_p] * 4 + [c_i64] * 3 + [c_p],
     'bxs_bfs_workspace_bytes': [c_i64] * 2,
-    'bxs_bfs_forward': [c_p] * 7 + [c_i64] * 2 + [c_int, c_p],
     'bxs_bfs_forward_rooted': [c_p] * 7 + [c_i64] * 2 + [c_int, c_i64, c_p],
     'bxs_tree_levels': [c_p] * 4 + [c_i64] * 2 + [c_p],
     'bxs_refine_scratch_bytes': [c_i64] * 3,
-    'bxs_refine_forward': [c_p] * 13 + [c_i64] * 3 + [c_p],
-    'bxs_refine_backward_feature': [c_p] * 10 + [c_i64] * 3 + [c_p],
-    'bxs_refine_backward_weight': [c_p] * 14 + [c_i64] * 3 + [c_p],
     'bxs_refine_forward_grouped': [c_p] * 14 + [c_i64] * 4 + [c_p],
     'bxs_refine_backward_feature_grouped': [c_p] * 11 + [c_i64] * 4 + [c_p],
     'bxs_refine_backward_weight_grouped': [c_p] * 15 + [c_i64] * 4 + [c_p],
@@ -90,7 +82,7 @@ SIGNATURES = {
     'bxs_corr_transfer': [c_p] * 7 + [c_i64] * 5 + [c_p],
     'bxs_fcos_targets': [c_p] * 7 + [c_i64] * 2 + [c_p] * 5 + [c_int, c_int, c_i64, c_p],
 }
-_RESTYPE = {'bxs_mst_workspace_bytes': c_i64, 'bxs_bfs_workspace_bytes': c_i64, 'bxs_refine_scratch_bytes': c_i64, 'bxs_lcm_workspace_bytes': c_i64, 'bxs_meanfield_workspace_bytes': c_i64, 'bxs_projection_workspace_bytes': c_i64, 'bxs_levelset_workspace_bytes': c_i64, 'bxs_condinst_head_workspace_bytes': c_i64, 'bxs_last_error': ctypes.c_char_p, 'bxs_boxinst_loss_workspace_bytes': c_i64,
+_RESTYPE = {'bxs_mst_workspace_bytes': c_i64, 'bxs_bfs_workspace_bytes': c_i64, 'bxs_refine_scratch_bytes': c_i64, 'bxs_lcm_workspace_bytes': c_i64, 'bxs_meanfield_workspace_bytes': c_i64, 'bxs_projection_workspace_bytes': c_i64,'bxs_condinst_head_workspace_bytes': c_i64, 'bxs_last_error': ctypes.c_char_p, 'bxs_boxinst_loss_workspace_bytes': c_i64,
              'bxs_boxinst_loss_fused_workspace_bytes': c_i64, 'bxs_boxinst_loss_fused_sched_bytes': c_i64,
              'bxs_boxinst_loss_plan_bytes': c_i64, 'bxs_levelset_fused_workspace_bytes': c_i64,
              'bxs_dynconv1x1_backward_workspace_bytes': c_i64, 'bxs_corr_transfer_workspace_bytes': c_i64}

@@ -187,13 +187,6 @@ extern "C" int64_t bxs_meanfield_workspace_bytes(int64_t n, int64_t h, int64_t w
   return n <= 0 ? 0 : 2 * n * h * w + 64;
 }
 
-extern "C" int bxs_meanfield_forward(const float* K, const int32_t* obj_img, const float* x, const float* targets,
-                                     const float* neglog4_host, float* ret, float* valid, void* workspace, int64_t n,
-                                     int64_t h, int64_t w, int kernel_size, int num_iter, bxs_stream_t stream) {
-  return bxs_meanfield_forward_inter(K, obj_img, x, targets, nullptr, 0.f, neglog4_host, ret, valid, workspace, n, h, w,
-                                     kernel_size, num_iter, stream);
-}
-
 extern "C" int bxs_meanfield_forward_inter(const float* K, const int32_t* obj_img, const float* x, const float* targets,
                                            const float* inter_img_mask, float gamma, const float* neglog4_host, float* ret,
                                            float* valid, void* workspace, int64_t n, int64_t h, int64_t w, int kernel_size,

@@ -1,8 +1,8 @@
-// a6 (dense form), a9, a10: box-projection dice loss on arbitrary score/target maps, the Chan-Vese
-// region level-set energy and the (unused by the heads) length regulariser -- forward + backward.
+// a6 (dense form), a10: box-projection dice loss on arbitrary score/target maps and the (unused by the
+// heads) length regulariser -- forward + backward.  (The a9 region level-set energy is fused_assembly.cu.)
 // Replaces BoxProjectionLoss (mmdet/models/losses/box_projection_loss.py:11-42), mil_loss+dice_loss
-// (mmdet/models/dense_heads/discobox_head.py:542-562), LevelsetLoss / region_levelset /
-// length_regularization (mmdet/models/losses/levelset_loss.py:7-60).
+// (mmdet/models/dense_heads/discobox_head.py:542-562), length_regularization
+// (mmdet/models/losses/levelset_loss.py:47-60).
 //
 // These run on a few dozen instance maps (<= 20 MB, L2 resident): the design goal is ONE pass
 // per reduction with deterministic two-stage sums (per-CTA partials -> fixed-order finalize)
@@ -161,164 +161,6 @@ __global__ void __launch_bounds__(NT) prj_bwd_kernel(int64_t total, int h, int w
   }
 }
 
-// ---------------------------------------------------------------------------------------
-// level set
-// ---------------------------------------------------------------------------------------
-constexpr int MAXC = 8;
-constexpr float kClampEps = 1e-5f;       // levelset_loss.py:36-37
-
-struct LsStats {                          // per instance, after pass 1 / pass 2
-  float den[2];                           // max(sum S_k, eps)
-  float z[2];                             // sum S_k
-  float a[2][MAXC];                       // sum S_k T_c
-  float m[2][MAXC];                       // region means
-  float d[2][MAXC];                       // dE/dm = -(2/C)(A - m Z)
-  float energy;                           // E (already divided by C)
-};
-
-// pass 1 partials: [chunk][2 + 2C]  -> z0, z1, a0[c].., a1[c]..
-__global__ void __launch_bounds__(NT) ls_moments_kernel(const float* __restrict__ S, const float* __restrict__ T, int C,
-                                                        int64_t hw, int chunks, float* __restrict__ partial) {
-  __shared__ float s_red[NT / 32];
-  const int n = blockIdx.y, chunk = blockIdx.x;
-  const float* s0 = S + (int64_t)n * 2 * hw;
-  const float* s1 = s0 + hw;
-  const float* t = T + (int64_t)n * C * hw;
-  float acc[2 + 2 * MAXC];
-#pragma unroll
-  for (int i = 0; i < 2 + 2 * MAXC; ++i) acc[i] = 0.f;
-  for (int64_t p = chunk * (int64_t)NT + threadIdx.x; p < hw; p += (int64_t)chunks * NT) {
-    const float a = __ldg(s0 + p), b = __ldg(s1 + p);
-    acc[0] += a; acc[1] += b;
-#pragma unroll
-    for (int c = 0; c < MAXC; ++c)
-      if (c < C) {
-        const float tv = __ldg(t + c * hw + p);
-        acc[2 + c] = fmaf(a, tv, acc[2 + c]);
-        acc[2 + MAXC + c] = fmaf(b, tv, acc[2 + MAXC + c]);
-      }
-  }
-  float* out = partial + ((int64_t)n * chunks + chunk) * (2 + 2 * MAXC);
-#pragma unroll
-  for (int i = 0; i < 2 + 2 * MAXC; ++i) {
-    const float v = block_sum<float>(acc[i], s_red);
-    if (threadIdx.x == 0) out[i] = v;
-  }
-}
-
-__global__ void ls_stats1_kernel(const float* __restrict__ partial, int C, int chunks, LsStats* __restrict__ stats) {
-  const int n = blockIdx.x;
-  if (threadIdx.x != 0) return;
-  float acc[2 + 2 * MAXC];
-  for (int i = 0; i < 2 + 2 * MAXC; ++i) acc[i] = 0.f;
-  for (int k = 0; k < chunks; ++k)
-    for (int i = 0; i < 2 + 2 * MAXC; ++i) acc[i] += partial[((int64_t)n * chunks + k) * (2 + 2 * MAXC) + i];
-  LsStats st;
-  for (int k = 0; k < 2; ++k) {
-    st.z[k] = acc[k];
-    st.den[k] = fmaxf(acc[k], kClampEps);
-    for (int c = 0; c < MAXC; ++c) {
-      st.a[k][c] = c < C ? acc[2 + k * MAXC + c] : 0.f;
-      st.m[k][c] = st.a[k][c] / st.den[k];
-      st.d[k][c] = 0.f;
-    }
-  }
-  st.energy = 0.f;
-  stats[n] = st;
-}
-
-// pass 2 partials: [chunk][1 + 2C] -> energy*C, r0[c] = sum (T-m0)S0, r1[c]
-__global__ void __launch_bounds__(NT) ls_energy_kernel(const float* __restrict__ S, const float* __restrict__ T, int C,
-                                                       int64_t hw, int chunks, const LsStats* __restrict__ stats,
-                                                       float* __restrict__ partial) {
-  __shared__ float s_red[NT / 32];
-  __shared__ LsStats st;
-  const int n = blockIdx.y, chunk = blockIdx.x;
-  if (threadIdx.x == 0) st = stats[n];
-  __syncthreads();
-  const float* s0 = S + (int64_t)n * 2 * hw;
-  const float* s1 = s0 + hw;
-  const float* t = T + (int64_t)n * C * hw;
-  float acc[1 + 2 * MAXC];
-#pragma unroll
-  for (int i = 0; i < 1 + 2 * MAXC; ++i) acc[i] = 0.f;
-  for (int64_t p = chunk * (int64_t)NT + threadIdx.x; p < hw; p += (int64_t)chunks * NT) {
-    const float a = __ldg(s0 + p), b = __ldg(s1 + p);
-#pragma unroll
-    for (int c = 0; c < MAXC; ++c)
-      if (c < C) {
-        const float tv = __ldg(t + c * hw + p);
-        const float d0 = tv - st.m[0][c], d1 = tv - st.m[1][c];
-        acc[0] = fmaf(d0 * d0, a, acc[0]);
-        acc[0] = fmaf(d1 * d1, b, acc[0]);
-        acc[1 + c] = fmaf(d0, a, acc[1 + c]);
-        acc[1 + MAXC + c] = fmaf(d1, b, acc[1 + MAXC + c]);
-      }
-  }
-  float* out = partial + ((int64_t)n * chunks + chunk) * (1 + 2 * MAXC);
-#pragma unroll
-  for (int i = 0; i < 1 + 2 * MAXC; ++i) {
-    const float v = block_sum<float>(acc[i], s_red);
-    if (threadIdx.x == 0) out[i] = v;
-  }
-}
-
-__global__ void ls_stats2_kernel(const float* __restrict__ partial, int C, int chunks, const float* __restrict__ pixel_num,
-                                 float loss_weight, LsStats* __restrict__ stats, float* __restrict__ loss) {
-  const int n = blockIdx.x;
-  if (threadIdx.x != 0) return;
-  float acc[1 + 2 * MAXC];
-  for (int i = 0; i < 1 + 2 * MAXC; ++i) acc[i] = 0.f;
-  for (int k = 0; k < chunks; ++k)
-    for (int i = 0; i < 1 + 2 * MAXC; ++i) acc[i] += partial[((int64_t)n * chunks + k) * (1 + 2 * MAXC) + i];
-  LsStats st = stats[n];
-  st.energy = acc[0] / (float)C;
-  for (int k = 0; k < 2; ++k)
-    for (int c = 0; c < C; ++c) st.d[k][c] = -2.f / (float)C * acc[1 + k * MAXC + c];
-  stats[n] = st;
-  loss[n] = loss_weight * st.energy / pixel_num[n];
-}
-
-__global__ void __launch_bounds__(NT) ls_bwd_kernel(const float* __restrict__ S, const float* __restrict__ T, int C,
-                                                    int64_t hw, const LsStats* __restrict__ stats,
-                                                    const float* __restrict__ pixel_num, float loss_weight,
-                                                    const float* __restrict__ g_loss, float* __restrict__ gS,
-                                                    float* __restrict__ gT) {
-  __shared__ LsStats st;
-  const int n = blockIdx.y;
-  if (threadIdx.x == 0) st = stats[n];
-  __syncthreads();
-  const float scale = g_loss[n] * loss_weight / pixel_num[n];
-  const float inv_c = 1.f / (float)C;
-  const float* s0 = S + (int64_t)n * 2 * hw;
-  const float* s1 = s0 + hw;
-  const float* t = T + (int64_t)n * C * hw;
-  // d m_kc / d S_k(p) = T_c(p)/den_k - [Z_k > eps] A_kc / den_k^2   (clamp(min=eps) passes no gradient when active)
-  float off[2] = {0.f, 0.f};
-  for (int k = 0; k < 2; ++k)
-    if (st.z[k] > kClampEps)
-      for (int c = 0; c < C; ++c) off[k] -= st.d[k][c] * st.a[k][c] / (st.den[k] * st.den[k]);
-  for (int64_t p = blockIdx.x * (int64_t)NT + threadIdx.x; p < hw; p += (int64_t)gridDim.x * NT) {
-    const float a = __ldg(s0 + p), b = __ldg(s1 + p);
-    float g0 = off[0], g1 = off[1];
-#pragma unroll
-    for (int c = 0; c < MAXC; ++c)
-      if (c < C) {
-        const float tv = __ldg(t + c * hw + p);
-        const float d0 = tv - st.m[0][c], d1 = tv - st.m[1][c];
-        g0 += d0 * d0 * inv_c + st.d[0][c] * tv / st.den[0];
-        g1 += d1 * d1 * inv_c + st.d[1][c] * tv / st.den[1];
-        if (gT)
-          gT[((int64_t)n * C + c) * hw + p] =
-              scale * (2.f * inv_c * (d0 * a + d1 * b) + st.d[0][c] * a / st.den[0] + st.d[1][c] * b / st.den[1]);
-      }
-    if (gS) {
-      gS[(int64_t)n * 2 * hw + p] = scale * g0;
-      gS[(int64_t)n * 2 * hw + hw + p] = scale * g1;
-    }
-  }
-}
-
 // length regulariser: sum |dy| + sum |dx| per instance (all channels)
 __global__ void __launch_bounds__(NT) length_fwd_kernel(const float* __restrict__ s, int C, int h, int w, int chunks,
                                                         float* __restrict__ partial) {
@@ -406,44 +248,6 @@ extern "C" int bxs_projection_loss_backward(const void* workspace, const float* 
   const int64_t total = n * h * w;
   const int blocks = (int)std::min<int64_t>(ceil_div(total, NT), (int64_t)sm_count() * 16);
   prj_bwd_kernel<<<blocks, NT, 0, as_stream(stream)>>>(total, (int)h, (int)w, ws, g_loss, g_scores);
-  return check_launch();
-}
-
-extern "C" int64_t bxs_levelset_workspace_bytes(int64_t n) {
-  return n <= 0 ? 0 : (int64_t)(align_up(sizeof(LsStats) * n) + align_up(sizeof(float) * n * 64 * (2 + 2 * MAXC)));
-}
-
-extern "C" int bxs_levelset_loss_forward(const float* scores2, const float* targets, const float* pixel_num, float* loss,
-                                         void* workspace, int64_t n, int64_t C, int64_t h, int64_t w, float loss_weight,
-                                         bxs_stream_t stream) {
-  if (!scores2 || !targets || !pixel_num || !loss || !workspace || n <= 0 || n >= 65536 || h <= 0 || w <= 0)
-    return BXS_ERR_INVALID_ARG;
-  if (C < 1 || C > MAXC) return BXS_ERR_UNSUPPORTED;
-  cudaStream_t st = as_stream(stream);
-  LsStats* stats = (LsStats*)workspace;
-  float* partial = (float*)((char*)workspace + align_up(sizeof(LsStats) * n));
-  const int64_t hw = h * w;
-  const int chunks = pick_chunks(n, hw);
-  ls_moments_kernel<<<dim3(chunks, (unsigned)n), NT, 0, st>>>(scores2, targets, (int)C, hw, chunks, partial);
-  ls_stats1_kernel<<<(unsigned)n, 32, 0, st>>>(partial, (int)C, chunks, stats);
-  ls_energy_kernel<<<dim3(chunks, (unsigned)n), NT, 0, st>>>(scores2, targets, (int)C, hw, chunks, stats, partial);
-  ls_stats2_kernel<<<(unsigned)n, 32, 0, st>>>(partial, (int)C, chunks, pixel_num, loss_weight, stats, loss);
-  return check_launch();
-}
-
-extern "C" int bxs_levelset_loss_backward(const float* scores2, const float* targets, const float* pixel_num,
-                                          const void* workspace, const float* g_loss, float* g_scores2, float* g_targets,
-                                          int64_t n, int64_t C, int64_t h, int64_t w, float loss_weight,
-                                          bxs_stream_t stream) {
-  if (!scores2 || !targets || !pixel_num || !workspace || !g_loss || (!g_scores2 && !g_targets) || n <= 0 ||
-      n >= 65536 || h <= 0 || w <= 0)
-    return BXS_ERR_INVALID_ARG;
-  if (C < 1 || C > MAXC) return BXS_ERR_UNSUPPORTED;
-  const int64_t hw = h * w;
-  const int chunks = pick_chunks(n, hw);
-  ls_bwd_kernel<<<dim3(chunks, (unsigned)n), NT, 0, as_stream(stream)>>>(scores2, targets, (int)C, hw,
-                                                                         (const LsStats*)workspace, pixel_num,
-                                                                         loss_weight, g_loss, g_scores2, g_targets);
   return check_launch();
 }
 

@@ -872,7 +872,7 @@ __device__ __forceinline__ TreeView make_view(const float* w, const int32_t* idx
   return t;
 }
 
-// MODE 0: forward (channel c < C: feature; c == C: normaliser with input 1)
+// MODE 0: forward (feature CTAs, then one normaliser CTA with input 1 per tree)
 // MODE 1: backward wrt feature: input = g / Z
 template <int MODE, bool SMEM>
 __global__ void __launch_bounds__(RNT) refine_updown_kernel(const float* __restrict__ feature, const float* __restrict__ w,
@@ -886,13 +886,13 @@ __global__ void __launch_bounds__(RNT) refine_updown_kernel(const float* __restr
   // tree_of (may be null): the tree / edge weights / normaliser of batch entry b are those of group tree_of[b] -- the
   // instances of one image share one tree (box_solov2_head.py:300-305,353; box2mask_head.py:271-276), so the order,
   // the packed child weights and the normaliser Z exist once per image instead of once per instance.
-  // norm_from >= 0 (grouped forward): CTAs with blockIdx.x >= norm_from compute the normaliser of TREE blockIdx.x - norm_from
-  // (one per tree, blockIdx.y == 0 only) in the same launch as the feature CTAs -- the two are independent until the division,
-  // and as two launches on one stream they cost two level walks back to back.  norm_from < 0: the normaliser is channel C of
-  // every batch entry (grid.y == C + 1).
+  // norm_from = the instance count.  Forward: CTAs with blockIdx.x >= norm_from compute the normaliser of TREE
+  // blockIdx.x - norm_from (one per tree, blockIdx.y == 0 only) in the same launch as the feature CTAs -- the two are
+  // independent until the division, and as two launches on one stream they cost two level walks back to back.
+  // The backward launches exactly norm_from CTAs per channel.
   extern __shared__ float s_buf[];
   __shared__ RingSmem R;
-  const bool split_norm = norm_from >= 0 && (int)blockIdx.x >= norm_from;
+  const bool split_norm = (int)blockIdx.x >= norm_from;
   if (split_norm && blockIdx.y != 0) return;
   const int b = split_norm ? (int)blockIdx.x - norm_from : (int)blockIdx.x, c = split_norm ? C : (int)blockIdx.y;
   const int tb = (tree_of && !split_norm) ? __ldg(tree_of + b) : b;
@@ -1062,30 +1062,12 @@ extern "C" int64_t bxs_bfs_workspace_bytes(int64_t B, int64_t V) {
 
 // level_start [B, V+1] and num_levels [B] are extra outputs (may be NULL -> scratch inside the workspace is NOT
 // provided: pass real buffers whenever the result feeds bxs_refine_*).
-// bxs_bfs_forward roots every tree at vertex 0 like bfs.cu:100-135; bxs_bfs_forward_rooted takes the root vertex: the
-// tree filter's result does not depend on the root, but the number of dependent levels of every pass does (a 200x256
-// image MST is ~1900 levels deep from the corner, about half of that from the centre).
-static int bfs_forward_impl(const int32_t* tree_edges, int32_t* sorted_index, int32_t* sorted_parent, int32_t* sorted_child,
-                            int32_t* level_start, int32_t* num_levels, void* workspace, int64_t B, int64_t V, int max_adj,
-                            int64_t root, bxs_stream_t stream);
-
-extern "C" int bxs_bfs_forward(const int32_t* tree_edges, int32_t* sorted_index, int32_t* sorted_parent,
-                               int32_t* sorted_child, int32_t* level_start, int32_t* num_levels, void* workspace,
-                               int64_t B, int64_t V, int max_adj, bxs_stream_t stream) {
-  return bfs_forward_impl(tree_edges, sorted_index, sorted_parent, sorted_child, level_start, num_levels, workspace, B, V,
-                          max_adj, 0, stream);
-}
-
+// The reference roots every tree at vertex 0 (bfs.cu:100-135); here the caller picks the root: the tree filter's result
+// does not depend on it, but the number of dependent levels of every pass does (a 200x256 image MST is ~1900 levels deep
+// from the corner, about half of that from the centre).
 extern "C" int bxs_bfs_forward_rooted(const int32_t* tree_edges, int32_t* sorted_index, int32_t* sorted_parent,
                                       int32_t* sorted_child, int32_t* level_start, int32_t* num_levels, void* workspace,
                                       int64_t B, int64_t V, int max_adj, int64_t root, bxs_stream_t stream) {
-  return bfs_forward_impl(tree_edges, sorted_index, sorted_parent, sorted_child, level_start, num_levels, workspace, B, V,
-                          max_adj, root, stream);
-}
-
-static int bfs_forward_impl(const int32_t* tree_edges, int32_t* sorted_index, int32_t* sorted_parent, int32_t* sorted_child,
-                            int32_t* level_start, int32_t* num_levels, void* workspace, int64_t B, int64_t V, int max_adj,
-                            int64_t root, bxs_stream_t stream) {
   if (!tree_edges || !sorted_index || !sorted_parent || !sorted_child || !level_start || !num_levels || !workspace ||
       B <= 0 || B >= 65536 || V <= 1 || root < 0 || root >= V)
     return BXS_ERR_INVALID_ARG;
@@ -1157,94 +1139,9 @@ extern "C" int64_t bxs_refine_scratch_bytes(int64_t B, int64_t C, int64_t V) {
   return (B <= 0 || C <= 0 || V <= 0) ? 0 : (int64_t)carve_refine(nullptr, B, C, V).total_bytes;
 }
 
-extern "C" int bxs_refine_forward(const float* feature, const float* edge_weight, const int32_t* sorted_index,
-                                  const int32_t* sorted_parent, const int32_t* sorted_child, const int32_t* level_start,
-                                  const int32_t* num_levels, float* feature_out, float* aggr, float* aggr_up, float* wsum,
-                                  float* wsum_up, void* scratch, int64_t B, int64_t C, int64_t V, bxs_stream_t stream) {
-  if (!feature || !edge_weight || !sorted_index || !sorted_parent || !sorted_child || !level_start || !num_levels ||
-      !feature_out || !aggr || !aggr_up || !wsum || !wsum_up || !scratch || B <= 0 || B >= 65536 || C <= 0 ||
-      C >= 65535 || V <= 0 || V >= (int64_t(1) << 28))
-    return BXS_ERR_INVALID_ARG;
-  cudaStream_t st = as_stream(stream);
-  RefineScratch rs = carve_refine(scratch, B, C, V);
-  pack_tree(edge_weight, sorted_child, rs, B, V, st);
-  const size_t sm = (V + 4) * sizeof(float);
-  const dim3 grid((unsigned)B, (unsigned)(C + 1));
-  if (sm <= kMaxRefineSmem) {
-    cudaFuncSetAttribute(refine_updown_kernel<0, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMaxRefineSmem);
-    refine_updown_kernel<0, true><<<grid, RNT, sm, st>>>(feature, edge_weight, sorted_index, sorted_parent, rs.cinfo, rs.cw,
-                                                        level_start, num_levels, nullptr, aggr, aggr_up, wsum, wsum_up,
-                                                        nullptr, (int)C, (int)V, nullptr, -1);
-  } else {
-    refine_updown_kernel<0, false><<<grid, RNT, 0, st>>>(feature, edge_weight, sorted_index, sorted_parent, rs.cinfo, rs.cw,
-                                                        level_start, num_levels, nullptr, aggr, aggr_up, wsum, wsum_up,
-                                                        rs.bufs, (int)C, (int)V, nullptr, -1);
-  }
-  refine_div_kernel<<<grid_for(B * C * V, 256), 256, 0, st>>>(aggr, wsum, feature_out, (int)C, (int)V, B * C * V, nullptr);
-  return check_launch();
-}
-
-extern "C" int bxs_refine_backward_feature(const float* edge_weight, const int32_t* sorted_index,
-                                           const int32_t* sorted_parent, const int32_t* sorted_child,
-                                           const int32_t* level_start, const int32_t* num_levels, const float* wsum,
-                                           const float* grad_out, float* grad_feature, void* scratch, int64_t B, int64_t C,
-                                           int64_t V, bxs_stream_t stream) {
-  if (!edge_weight || !sorted_index || !sorted_parent || !sorted_child || !level_start || !num_levels || !wsum ||
-      !grad_out || !grad_feature || !scratch || B <= 0 || B >= 65536 || C <= 0 || C >= 65535 || V <= 0 ||
-      V >= (int64_t(1) << 28))
-    return BXS_ERR_INVALID_ARG;
-  cudaStream_t st = as_stream(stream);
-  RefineScratch rs = carve_refine(scratch, B, C, V);
-  pack_tree(edge_weight, sorted_child, rs, B, V, st);
-  const size_t sm = (V + 4) * sizeof(float);
-  const dim3 grid((unsigned)B, (unsigned)C);
-  if (sm <= kMaxRefineSmem) {
-    cudaFuncSetAttribute(refine_updown_kernel<1, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMaxRefineSmem);
-    refine_updown_kernel<1, true><<<grid, RNT, sm, st>>>(grad_out, edge_weight, sorted_index, sorted_parent, rs.cinfo, rs.cw,
-                                                        level_start, num_levels, wsum, grad_feature, nullptr, nullptr,
-                                                        nullptr, nullptr, (int)C, (int)V, nullptr, -1);
-  } else {
-    refine_updown_kernel<1, false><<<grid, RNT, 0, st>>>(grad_out, edge_weight, sorted_index, sorted_parent, rs.cinfo, rs.cw,
-                                                        level_start, num_levels, wsum, grad_feature, nullptr, nullptr,
-                                                        nullptr, rs.bufs, (int)C, (int)V, nullptr, -1);
-  }
-  return check_launch();
-}
-
-extern "C" int bxs_refine_backward_weight(const float* edge_weight, const int32_t* sorted_index,
-                                          const int32_t* sorted_parent, const int32_t* sorted_child,
-                                          const int32_t* level_start, const int32_t* num_levels, const float* feature_out,
-                                          const float* aggr, const float* aggr_up, const float* wsum, const float* wsum_up,
-                                          const float* grad_out, float* grad_weight, void* scratch, int64_t B, int64_t C,
-                                          int64_t V, bxs_stream_t stream) {
-  if (!edge_weight || !sorted_index || !sorted_parent || !sorted_child || !level_start || !num_levels || !feature_out ||
-      !aggr || !aggr_up || !wsum || !wsum_up || !grad_out || !grad_weight || !scratch || B <= 0 || B >= 65536 || C <= 0 ||
-      V <= 0 || V >= (int64_t(1) << 28))
-    return BXS_ERR_INVALID_ARG;
-  cudaStream_t st = as_stream(stream);
-  RefineScratch rs = carve_refine(scratch, B, C, V);
-  pack_tree(edge_weight, sorted_child, rs, B, V, st);
-  const size_t sm = (V + 4) * sizeof(float);
-  if (sm <= kMaxRefineSmem) {
-    cudaFuncSetAttribute(refine_bwd_weight_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMaxRefineSmem);
-    refine_bwd_weight_kernel<true><<<dim3((unsigned)B, 2), RNT, sm, st>>>(edge_weight, sorted_index, sorted_parent, rs.cinfo,
-                                                                         rs.cw, level_start, num_levels, feature_out, aggr,
-                                                                         aggr_up, wsum, wsum_up, grad_out, rs.gw2, nullptr,
-                                                                         rs.outd_par, (int)C, (int)V, nullptr);
-  } else {
-    refine_bwd_weight_kernel<false><<<dim3((unsigned)B, 2), RNT, 0, st>>>(edge_weight, sorted_index, sorted_parent, rs.cinfo,
-                                                                          rs.cw, level_start, num_levels, feature_out, aggr,
-                                                                          aggr_up, wsum, wsum_up, grad_out, rs.gw2, rs.bufs,
-                                                                          rs.outd_par, (int)C, (int)V, nullptr);
-  }
-  cudaMemcpyAsync(grad_weight, rs.gw2, sizeof(float) * B * V, cudaMemcpyDeviceToDevice, st);
-  refine_add_kernel<<<grid_for(B * V, 256), 256, 0, st>>>(grad_weight, rs.gw2 + B * V, B * V);
-  return check_launch();
-}
-
 // ---------------------------------------------------------------------------------------
-// Grouped forms: n instances share G trees (tree_of [n] -> group).  Order, packed child weights, edge weights and the
-// normaliser exist once per group; per-instance work is one CTA per (instance, channel).
+// n instances share G trees (tree_of [n] -> group; NULL: instance i uses tree i, n == G).  Order, packed child weights,
+// edge weights and the normaliser exist once per group; per-instance work is one CTA per (instance, channel).
 // ---------------------------------------------------------------------------------------
 extern "C" int bxs_refine_forward_grouped(const float* feature, const float* edge_weight, const int32_t* sorted_index,
                                           const int32_t* sorted_parent, const int32_t* sorted_child,
@@ -1252,8 +1149,8 @@ extern "C" int bxs_refine_forward_grouped(const float* feature, const float* edg
                                           float* feature_out, float* aggr, float* aggr_up, float* wsum, float* wsum_up,
                                           void* scratch, int64_t n, int64_t G, int64_t C, int64_t V, bxs_stream_t stream) {
   if (!feature || !edge_weight || !sorted_index || !sorted_parent || !sorted_child || !level_start || !num_levels ||
-      !tree_of || !feature_out || !aggr || !aggr_up || !wsum || !wsum_up || !scratch || n <= 0 || n >= 65536 || G <= 0 ||
-      G >= 65536 || C <= 0 || C >= 65535 || V <= 0 || V >= (int64_t(1) << 28))
+      !feature_out || !aggr || !aggr_up || !wsum || !wsum_up || !scratch || n <= 0 || n >= 65536 || G <= 0 ||
+      G >= 65536 || C <= 0 || C >= 65535 || V <= 0 || V >= (int64_t(1) << 28) || (!tree_of && n != G))
     return BXS_ERR_INVALID_ARG;
   cudaStream_t st = as_stream(stream);
   RefineScratch rs = carve_refine(scratch, std::max(n, G), C, V);
@@ -1279,9 +1176,9 @@ extern "C" int bxs_refine_backward_feature_grouped(const float* edge_weight, con
                                                    const int32_t* tree_of, const float* wsum, const float* grad_out,
                                                    float* grad_feature, void* scratch, int64_t n, int64_t G, int64_t C,
                                                    int64_t V, bxs_stream_t stream) {
-  if (!edge_weight || !sorted_index || !sorted_parent || !sorted_child || !level_start || !num_levels || !tree_of || !wsum ||
+  if (!edge_weight || !sorted_index || !sorted_parent || !sorted_child || !level_start || !num_levels || !wsum ||
       !grad_out || !grad_feature || !scratch || n <= 0 || n >= 65536 || G <= 0 || G >= 65536 || C <= 0 || C >= 65535 ||
-      V <= 0 || V >= (int64_t(1) << 28))
+      V <= 0 || V >= (int64_t(1) << 28) || (!tree_of && n != G))
     return BXS_ERR_INVALID_ARG;
   cudaStream_t st = as_stream(stream);
   RefineScratch rs = carve_refine(scratch, std::max(n, G), C, V);
@@ -1292,11 +1189,11 @@ extern "C" int bxs_refine_backward_feature_grouped(const float* edge_weight, con
     cudaFuncSetAttribute(refine_updown_kernel<1, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMaxRefineSmem);
     refine_updown_kernel<1, true><<<grid, RNT, sm, st>>>(grad_out, edge_weight, sorted_index, sorted_parent, rs.cinfo, rs.cw,
                                                         level_start, num_levels, wsum, grad_feature, nullptr, nullptr,
-                                                        nullptr, nullptr, (int)C, (int)V, tree_of, -1);
+                                                        nullptr, nullptr, (int)C, (int)V, tree_of, (int)n);
   } else {
     refine_updown_kernel<1, false><<<grid, RNT, 0, st>>>(grad_out, edge_weight, sorted_index, sorted_parent, rs.cinfo, rs.cw,
                                                         level_start, num_levels, wsum, grad_feature, nullptr, nullptr,
-                                                        nullptr, rs.bufs, (int)C, (int)V, tree_of, -1);
+                                                        nullptr, rs.bufs, (int)C, (int)V, tree_of, (int)n);
   }
   return check_launch();
 }
@@ -1309,9 +1206,9 @@ extern "C" int bxs_refine_backward_weight_grouped(const float* edge_weight, cons
                                                   const float* aggr_up, const float* wsum, const float* wsum_up,
                                                   const float* grad_out, float* grad_weight, void* scratch, int64_t n,
                                                   int64_t G, int64_t C, int64_t V, bxs_stream_t stream) {
-  if (!edge_weight || !sorted_index || !sorted_parent || !sorted_child || !level_start || !num_levels || !tree_of ||
-      !feature_out || !aggr || !aggr_up || !wsum || !wsum_up || !grad_out || !grad_weight || !scratch || n <= 0 ||
-      n >= 65536 || G <= 0 || G >= 65536 || C <= 0 || V <= 0 || V >= (int64_t(1) << 28))
+  if (!edge_weight || !sorted_index || !sorted_parent || !sorted_child || !level_start || !num_levels || !feature_out ||
+      !aggr || !aggr_up || !wsum || !wsum_up || !grad_out || !grad_weight || !scratch || n <= 0 || n >= 65536 || G <= 0 ||
+      G >= 65536 || C <= 0 || V <= 0 || V >= (int64_t(1) << 28) || (!tree_of && n != G))
     return BXS_ERR_INVALID_ARG;
   cudaStream_t st = as_stream(stream);
   RefineScratch rs = carve_refine(scratch, std::max(n, G), C, V);

@@ -1,6 +1,6 @@
 """``LevelsetLoss`` / ``region_levelset`` / ``length_regularization`` -- registry drop-ins for
-mmdet/models/losses/levelset_loss.py:7-60, computed by libboxseg_b200 (two-pass moments/energy
-kernels with an analytic backward; no [n,C,h,w] temporaries)."""
+mmdet/models/losses/levelset_loss.py:7-60, computed by libboxseg_b200 (the region energy: one cluster launch
+forward, one launch backward with an analytic gradient; no [n,C,h,w] temporaries)."""
 import torch
 import torch.nn as nn
 
@@ -8,48 +8,11 @@ from ... import _lib as L
 from ..builder import LOSSES, register
 
 
-class _LevelsetLoss(torch.autograd.Function):
-    @staticmethod
-    def forward(ctx, scores2, targets, pixel_num, loss_weight):
-        s = scores2.contiguous().float()
-        t = targets.contiguous().float()
-        p = pixel_num.contiguous().float()
-        L.require_cuda(s, t, p)
-        n, two, h, w = s.shape
-        assert two == 2 and t.shape[0] == n and t.shape[-2:] == (h, w)
-        C = t.shape[1]
-        lib = L.lib()
-        loss = torch.empty(n, dtype=torch.float32, device=s.device)
-        ws = torch.empty(max(lib.bxs_levelset_workspace_bytes(n), 1), dtype=torch.uint8, device=s.device)
-        if n:
-            with torch.cuda.device(s.device):
-                L.check(lib.bxs_levelset_loss_forward(L.ptr(s), L.ptr(t), L.ptr(p), L.ptr(loss), L.ptr(ws), n, C, h, w,
-                                                      float(loss_weight), L.stream()), 'levelset_loss_forward')
-        ctx.save_for_backward(s, t, p, ws)
-        ctx.loss_weight = float(loss_weight)
-        return loss
-
-    @staticmethod
-    def backward(ctx, g_loss):
-        s, t, p, ws = ctx.saved_tensors
-        n, _, h, w = s.shape
-        C = t.shape[1]
-        need_s, need_t = ctx.needs_input_grad[0], ctx.needs_input_grad[1]
-        gs = torch.empty_like(s) if need_s else None
-        gt = torch.empty_like(t) if need_t else None
-        if n and (need_s or need_t):
-            with torch.cuda.device(s.device):
-                L.check(L.lib().bxs_levelset_loss_backward(L.ptr(s), L.ptr(t), L.ptr(p), L.ptr(ws),
-                                                           L.ptr(g_loss.contiguous().float()), L.ptr(gs), L.ptr(gt),
-                                                           n, C, h, w, ctx.loss_weight, L.stream()),
-                        'levelset_loss_backward')
-        return gs, gt, None, None
-
-
 class _LevelsetFused(torch.autograd.Function):
     """One launch forward (a cluster of 8 CTAs per instance, the means -> energy dependency through distributed shared
     memory), one launch backward.  mode 1 = the whole assembly of box_solov2_head.py:341-360 / box2mask_head.py:305-327
-    from (logits, box mask, raw targets); mode 0 = LevelsetLoss.forward on dense (scores2, targets, pixel_num)."""
+    from (logits, box mask, raw targets); mode 0 = LevelsetLoss.forward / region_levelset on dense (scores2, targets,
+    pixel_num)."""
 
     @staticmethod
     def forward(ctx, x, y, targets, pixel_num, loss_weight, mode):
@@ -59,6 +22,7 @@ class _LevelsetFused(torch.autograd.Function):
         p = pixel_num.contiguous().float() if pixel_num is not None else None
         L.require_cuda(xs, ys, t, p)
         n, C, h, w = t.shape
+        assert mode != 0 or xs.shape == (n, 2, h, w)
         lib = L.lib()
         loss = torch.empty(n, dtype=torch.float32, device=t.device)
         ws = torch.empty(max(lib.bxs_levelset_fused_workspace_bytes(n), 1), dtype=torch.uint8, device=t.device)
@@ -126,7 +90,7 @@ class region_levelset(nn.Module):
 
     def forward(self, mask_score, lst_target):
         ones = torch.ones(mask_score.shape[0], dtype=torch.float32, device=mask_score.device)
-        return _LevelsetLoss.apply(mask_score, lst_target, ones, 1.0)
+        return _LevelsetFused.apply(mask_score, None, lst_target, ones, 1.0, 0)
 
 
 class length_regularization(nn.Module):
@@ -143,9 +107,7 @@ class LevelsetLoss(nn.Module):
         self.loss_weight = loss_weight
 
     def forward(self, mask_logits, targets, pixel_num):
-        if targets.shape[1] <= 8:
-            return _LevelsetFused.apply(mask_logits, None, targets, pixel_num, self.loss_weight, 0)
-        return _LevelsetLoss.apply(mask_logits, targets, pixel_num, self.loss_weight)
+        return _LevelsetFused.apply(mask_logits, None, targets, pixel_num, self.loss_weight, 0)
 
 
 class _LCM(torch.autograd.Function):

@@ -19,61 +19,34 @@ def _both(device, feature_fn, weight_fn):
 
 
 class _Refine(Function):
-    @staticmethod
-    def forward(ctx, feature_in, edge_weight, sorted_index, sorted_parent, sorted_child, low_tree):
-        levels = _C.levels_of(sorted_index, sorted_parent)
-        out, aggr, aggr_up, wsum, wsum_up = _C.refine_forward(feature_in, edge_weight, sorted_index, sorted_parent,
-                                                              sorted_child, levels)
-        ctx.save_for_backward(edge_weight, sorted_index, sorted_parent, sorted_child, out, aggr, aggr_up, wsum, wsum_up,
-                              *levels)
-        ctx.low_tree = low_tree
-        return out
-
-    @staticmethod
-    @once_differentiable
-    def backward(ctx, grad_output):
-        (edge_weight, sorted_index, sorted_parent, sorted_child, out, aggr, aggr_up, wsum, wsum_up, lvl,
-         nlv) = ctx.saved_tensors
-        args = (None, edge_weight, sorted_index, sorted_parent, sorted_child, out, aggr, aggr_up, wsum, wsum_up,
-                grad_output.contiguous())
-        if ctx.low_tree:
-            return _C.refine_backward_feature(*args, levels=(lvl, nlv)), None, None, None, None, None
-        grad_feature, grad_weight = _both(grad_output.device, lambda: _C.refine_backward_feature(*args, levels=(lvl, nlv)),
-                                          lambda: _C.refine_backward_weight(*args, levels=(lvl, nlv)))
-        return grad_feature, grad_weight, None, None, None, None
-
-
-refine = _Refine.apply
-
-
-class _RefineGrouped(Function):
-    """refine for n instances that share G trees (``tree_of`` [n] int32 -> group): the instances of one image share the
+    """``tree_of`` (optional, [n] int32 -> tree): n instances share the G trees given.  The instances of one image share the
     image's tree in both heads that use the filter (box_solov2_head.py:300-305,353; box2mask_head.py:271-276), so the
-    BFS order, the edge weights and the normaliser are computed once per image.  d/d edge_weight is summed over the
-    instances of a group."""
+    BFS order, the edge weights and the normaliser are computed once per image, and d/d edge_weight is summed over the
+    instances of a tree.  Without it instance i uses tree i, as in the reference.  An order that bfs_forward did not
+    produce is replaced by the equivalent canonical order of the same tree (tree_filter_cuda._resolve)."""
 
     @staticmethod
-    def forward(ctx, feature_in, edge_weight, sorted_index, sorted_parent, sorted_child, tree_of, low_tree):
-        levels = _C.levels_of(sorted_index, sorted_parent)
-        out, aggr, aggr_up, wsum, wsum_up = _C.refine_forward_grouped(feature_in, edge_weight, sorted_index, sorted_parent,
-                                                                      sorted_child, levels, tree_of)
-        ctx.save_for_backward(edge_weight, sorted_index, sorted_parent, sorted_child, tree_of, out, aggr, aggr_up, wsum,
-                              wsum_up, *levels)
+    def forward(ctx, feature_in, edge_weight, sorted_index, sorted_parent, sorted_child, low_tree, tree_of=None):
+        w, idx, par, chd, levels, perm = _C._resolve(edge_weight, sorted_index, sorted_parent, sorted_child)
+        out, aggr, aggr_up, wsum, wsum_up = _C.refine_forward_grouped(feature_in, w, idx, par, chd, levels, tree_of)
+        ctx.save_for_backward(w, idx, par, chd, *levels, tree_of, perm, out, aggr, aggr_up, wsum, wsum_up)
         ctx.low_tree = low_tree
         return out
 
     @staticmethod
     @once_differentiable
     def backward(ctx, grad_output):
-        (edge_weight, idx, par, chd, tree_of, out, aggr, aggr_up, wsum, wsum_up, lvl, nlv) = ctx.saved_tensors
+        (w, idx, par, chd, lvl, nlv, tree_of, perm, out, aggr, aggr_up, wsum, wsum_up) = ctx.saved_tensors
         g = grad_output.contiguous()
+
         def d_feature():
-            return _C.refine_backward_feature_grouped(edge_weight, idx, par, chd, (lvl, nlv), tree_of, wsum, g)
+            return _C.refine_backward_feature_grouped(w, idx, par, chd, (lvl, nlv), tree_of, wsum, g)
 
         def d_weight():
-            per_inst = _C.refine_backward_weight_grouped(edge_weight, idx, par, chd, (lvl, nlv), tree_of, out, aggr, aggr_up,
-                                                         wsum, wsum_up, g)
-            return torch.zeros_like(edge_weight).index_add_(0, tree_of.long(), per_inst)
+            gw = _C.refine_backward_weight_grouped(w, idx, par, chd, (lvl, nlv), tree_of, out, aggr, aggr_up, wsum, wsum_up, g)
+            if tree_of is not None:
+                gw = torch.zeros_like(w).index_add_(0, tree_of.long(), gw)
+            return _C._to_theirs(gw, perm)
 
         if ctx.low_tree:
             return d_feature(), None, None, None, None, None, None
@@ -81,4 +54,5 @@ class _RefineGrouped(Function):
         return grad_feature, grad_weight, None, None, None, None, None
 
 
-refine_grouped = _RefineGrouped.apply
+def refine(feature_in, edge_weight, sorted_index, sorted_parent, sorted_child, low_tree, tree_of=None):
+    return _Refine.apply(feature_in, edge_weight, sorted_index, sorted_parent, sorted_child, low_tree, tree_of)

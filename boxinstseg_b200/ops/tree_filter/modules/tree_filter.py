@@ -12,7 +12,7 @@ from .... import _lib as L
 
 from ..functions.bfs import bfs
 from ..functions.mst import mst
-from ..functions.refine import refine, refine_grouped
+from ..functions.refine import refine
 
 
 def _squared_distance(a, b):
@@ -159,8 +159,8 @@ class TreeFilter2D(nn.Module):
             edge_weight = self.build_edge_weight(embed_in, sorted_index, sorted_parent, low_tree, sorted_child)
             feat = feature_in.reshape(shape[0], shape[1], -1).contiguous()
             t_of = tree_of if tree_of.dtype == torch.int32 else tree_of.to(torch.int32)
-            return refine_grouped(feat, edge_weight, sorted_index, sorted_parent, sorted_child, t_of.contiguous(),
-                                  low_tree).reshape(shape)
+            return refine(feat, edge_weight, sorted_index, sorted_parent, sorted_child, low_tree,
+                          t_of.contiguous()).reshape(shape)
         shape = feature_in.shape
         sorted_index, sorted_parent, sorted_child = order if order is not None else bfs(tree, 4, self._root(shape))
         edge_weight = self.build_edge_weight(embed_in, sorted_index, sorted_parent, low_tree, sorted_child)

@@ -81,18 +81,15 @@ def _adopt(sorted_index, sorted_parent):
     return oidx, opar, ochd, _cached_levels(oidx), perm
 
 
-def _resolve(edge_weight, sorted_index, sorted_parent, sorted_child, levels):
+def _resolve(edge_weight, sorted_index, sorted_parent, sorted_child):
     """-> (w, idx, par, chd, levels, perm): the caller's order when it came from bfs_forward (perm None), else the
     adopted order with the per-position edge weights carried over by vertex."""
-    idx, par, chd = _i32(sorted_index), _i32(sorted_parent), _i32(sorted_child)
-    if levels is None:
-        levels = _cached_levels(sorted_index)
+    w, idx, par, chd = _f32(edge_weight), _i32(sorted_index), _i32(sorted_parent), _i32(sorted_child)
+    levels = _cached_levels(sorted_index)
     if levels is not None:
-        return edge_weight, idx, par, chd, levels, None
+        return w, idx, par, chd, levels, None
     oidx, opar, ochd, levels, perm = _adopt(idx, par)
-    w = torch.zeros_like(edge_weight)
-    w.scatter_(1, perm, edge_weight)
-    return w, oidx, opar, ochd, levels, perm
+    return torch.zeros_like(w).scatter_(1, perm, w), oidx, opar, ochd, levels, perm
 
 
 def _to_ours(t, perm):      # position-ordered [B,V] or [B,C,V] tensor: foreign order -> adopted order
@@ -113,55 +110,31 @@ def _scratch(B, C, V, dev):
     return torch.empty(max(L.lib().bxs_refine_scratch_bytes(B, C, V), 4), dtype=torch.uint8, device=dev)
 
 
-def refine_forward(feature_in, edge_weight, sorted_index, sorted_parent, sorted_child, levels=None):
-    f, w = _f32(feature_in), _f32(edge_weight)
-    L.require_cuda(f, w, sorted_index, sorted_parent, sorted_child)
-    w, idx, par, chd, (lvl, nlv), perm = _resolve(w, sorted_index, sorted_parent, sorted_child, levels)
-    B, C, V = f.shape
-    out, aggr, aggr_up = torch.empty_like(f), torch.empty_like(f), torch.empty_like(f)
-    wsum = torch.empty((B, V), dtype=torch.float32, device=f.device)
-    wsum_up = torch.empty_like(wsum)
-    with torch.cuda.device(f.device):
-        L.check(L.lib().bxs_refine_forward(L.ptr(f), L.ptr(w), L.ptr(idx), L.ptr(par), L.ptr(chd), L.ptr(lvl), L.ptr(nlv),
-                                           L.ptr(out), L.ptr(aggr), L.ptr(aggr_up), L.ptr(wsum), L.ptr(wsum_up),
-                                           L.ptr(_scratch(B, C, V, f.device)), B, C, V, L.stream()), 'refine_forward')
+def refine_forward(feature_in, edge_weight, sorted_index, sorted_parent, sorted_child):
+    w, idx, par, chd, levels, perm = _resolve(edge_weight, sorted_index, sorted_parent, sorted_child)
+    out, aggr, aggr_up, wsum, wsum_up = refine_forward_grouped(feature_in, w, idx, par, chd, levels, None)
     # out / aggr / wsum are vertex-ordered; the two *_up tensors are position-ordered (refine.cu:201-260)
     return out, aggr, _to_theirs(aggr_up, perm), wsum, _to_theirs(wsum_up, perm)
 
 
 def refine_backward_feature(feature_in, edge_weight, sorted_index, sorted_parent, sorted_child, feature_out,
-                            feature_aggr, feature_aggr_up, weight_sum, weight_sum_up, grad_out, levels=None):
-    w, g = _f32(edge_weight), _f32(grad_out)
-    w, idx, par, chd, (lvl, nlv), perm = _resolve(w, sorted_index, sorted_parent, sorted_child, levels)
-    B, C, V = g.shape
-    gf = torch.empty_like(g)
-    with torch.cuda.device(g.device):
-        L.check(L.lib().bxs_refine_backward_feature(L.ptr(w), L.ptr(idx), L.ptr(par), L.ptr(chd), L.ptr(lvl), L.ptr(nlv),
-                                                    L.ptr(_f32(weight_sum)), L.ptr(g), L.ptr(gf),
-                                                    L.ptr(_scratch(B, C, V, g.device)), B, C, V, L.stream()),
-                'refine_backward_feature')
-    return gf
+                            feature_aggr, feature_aggr_up, weight_sum, weight_sum_up, grad_out):
+    w, idx, par, chd, levels, _ = _resolve(edge_weight, sorted_index, sorted_parent, sorted_child)
+    return refine_backward_feature_grouped(w, idx, par, chd, levels, None, _f32(weight_sum), grad_out)
 
 
 def refine_backward_weight(feature_in, edge_weight, sorted_index, sorted_parent, sorted_child, feature_out,
-                           feature_aggr, feature_aggr_up, weight_sum, weight_sum_up, grad_out, levels=None):
-    w, g = _f32(edge_weight), _f32(grad_out)
-    w, idx, par, chd, (lvl, nlv), perm = _resolve(w, sorted_index, sorted_parent, sorted_child, levels)
-    feature_aggr_up, weight_sum_up = _to_ours(_f32(feature_aggr_up), perm), _to_ours(_f32(weight_sum_up), perm)
-    B, C, V = g.shape
-    gw = torch.empty((B, V), dtype=torch.float32, device=g.device)
-    with torch.cuda.device(g.device):
-        L.check(L.lib().bxs_refine_backward_weight(L.ptr(w), L.ptr(idx), L.ptr(par), L.ptr(chd), L.ptr(lvl), L.ptr(nlv),
-                                                   L.ptr(_f32(feature_out)), L.ptr(_f32(feature_aggr)),
-                                                   L.ptr(_f32(feature_aggr_up)), L.ptr(_f32(weight_sum)),
-                                                   L.ptr(_f32(weight_sum_up)), L.ptr(g), L.ptr(gw),
-                                                   L.ptr(_scratch(B, C, V, g.device)), B, C, V, L.stream()),
-                'refine_backward_weight')
+                           feature_aggr, feature_aggr_up, weight_sum, weight_sum_up, grad_out):
+    w, idx, par, chd, levels, perm = _resolve(edge_weight, sorted_index, sorted_parent, sorted_child)
+    gw = refine_backward_weight_grouped(w, idx, par, chd, levels, None, _f32(feature_out), _f32(feature_aggr),
+                                        _to_ours(_f32(feature_aggr_up), perm), _f32(weight_sum),
+                                        _to_ours(_f32(weight_sum_up), perm), grad_out)
     return _to_theirs(gw, perm)
 
 
 # ----------------------------------------------------------------------------------------------------------------
-# grouped forms (not part of the reference's pybind surface): n instances share G trees, tree_of [n] -> group
+# grouped forms (not part of the reference's pybind surface): n instances share G trees, tree_of [n] -> tree (None:
+# instance i uses tree i, n == G).  The order must come from bfs_forward (see _resolve); levels = its level table.
 # ----------------------------------------------------------------------------------------------------------------
 def refine_forward_grouped(feature_in, edge_weight, sorted_index, sorted_parent, sorted_child, levels, tree_of):
     f, w = _f32(feature_in), _f32(edge_weight)

@@ -201,21 +201,9 @@ int bxs_projection_loss_backward(const void* workspace, const float* g_loss, flo
                                  int64_t h, int64_t w, bxs_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------
- * a9  region level-set energy        replaces LevelsetLoss / region_levelset
- *     (mmdet/models/losses/levelset_loss.py:7-44).
- * scores2 [n,2,h,w], targets [n,C,h,w] (C <= 8), pixel_num [n] -> loss [n] = w * E / pixel_num.
- * backward writes g_scores2 and/or g_targets (either may be NULL).  workspace carries the
- * region means from forward to backward: bxs_levelset_workspace_bytes(n).
  * a10 length regulariser (levelset_loss.py:47-60): scores [n,C,h,w] -> out [n]; workspace n*64 floats.
+ *     (a9, the region level-set energy of LevelsetLoss / region_levelset, is bxs_levelset_fused_* mode 0.)
  * --------------------------------------------------------------------------------------- */
-int64_t bxs_levelset_workspace_bytes(int64_t n);
-int bxs_levelset_loss_forward(const float* scores2, const float* targets, const float* pixel_num, float* loss,
-                              void* workspace, int64_t n, int64_t C, int64_t h, int64_t w, float loss_weight,
-                              bxs_stream_t stream);
-int bxs_levelset_loss_backward(const float* scores2, const float* targets, const float* pixel_num,
-                               const void* workspace, const float* g_loss, float* g_scores2, float* g_targets,
-                               int64_t n, int64_t C, int64_t h, int64_t w, float loss_weight,
-                               bxs_stream_t stream);
 int bxs_length_reg_forward(const float* scores, float* out, void* workspace, int64_t n, int64_t C, int64_t h,
                            int64_t w, bxs_stream_t stream);
 int bxs_length_reg_backward(const float* scores, const float* g_out, float* g_scores, int64_t n, int64_t C,
@@ -240,20 +228,18 @@ int bxs_lcm_backward(const float* phis, const float* box, const void* workspace,
  * a16  DiscoBox mean-field CRF (forward only, as in the reference)     replaces MeanField
  *     (mmdet/models/dense_heads/discobox_head.py:585-651).
  * bxs_meanfield_kernel: feature [B,C,h,w] -> K [B,k*k,h,w] bilateral kernel (incl. centre tap).
- * bxs_meanfield_forward: x, targets [n,1,h,w]; obj_img [n] int32 (image of each object, may be NULL
+ * bxs_meanfield_forward_inter: x, targets [n,1,h,w]; obj_img [n] int32 (image of each object, may be NULL
  *   when B == 1); neglog4_host = {-log U_fg(bit0), -log U_fg(bit1), -log U_bg(bit0), -log U_bg(bit1)}
  *   (4 host floats computed by the caller with the reference's float32 arithmetic);
  *   ret [n,1,h,w] in {0,1}, valid [n].  workspace: bxs_meanfield_workspace_bytes (large maps only).
+ *   inter_img_mask f32 [n,2,h,w] (background, foreground) is the inter-image term of corr_loss
+ *   (discobox_head.py:616,643-644): f += inter_img_mask * gamma before the target product; NULL = no such term
+ *   (MeanField.forward without it).
  * --------------------------------------------------------------------------------------- */
 int bxs_meanfield_kernel(const float* feature, float* K, int64_t B, int64_t C, int64_t h, int64_t w,
                          int kernel_size, float two_theta0_sq, float two_theta1_sq, float alpha0,
                          bxs_stream_t stream);
 int64_t bxs_meanfield_workspace_bytes(int64_t n, int64_t h, int64_t w);
-int bxs_meanfield_forward(const float* K, const int32_t* obj_img, const float* x, const float* targets,
-                          const float* neglog4_host, float* ret, float* valid, void* workspace, int64_t n,
-                          int64_t h, int64_t w, int kernel_size, int num_iter, bxs_stream_t stream);
-/* same with the inter-image term of corr_loss (discobox_head.py:616,643-644): inter_img_mask f32 [n,2,h,w] (background,
- * foreground), f += inter_img_mask * gamma before the target product; NULL = the call above. */
 int bxs_meanfield_forward_inter(const float* K, const int32_t* obj_img, const float* x, const float* targets,
                                 const float* inter_img_mask, float gamma, const float* neglog4_host, float* ret,
                                 float* valid, void* workspace, int64_t n, int64_t h, int64_t w, int kernel_size,
@@ -267,45 +253,52 @@ int bxs_meanfield_forward_inter(const float* K, const int32_t* obj_img, const fl
  * bxs_mst_forward: edge_index int32 [B,E,2], edge_weight f32 [B,E] -> edge_out int32 [B,V-1,2]: the unique
  *   minimum spanning tree under the strict total order (weight, edge id) -- the same edge SET the reference's
  *   CPU Boruvka returns (src/mst/boruvka.cpp:74-80) -- emitted in ascending edge id.  Runs on the GPU.
- * bxs_bfs_forward: tree edges -> sorted_index [B,V] (position -> vertex), sorted_parent [B,V] (position of
+ * bxs_bfs_forward_rooted: tree edges -> sorted_index [B,V] (position -> vertex), sorted_parent [B,V] (position of
  *   the parent, root 0), sorted_child [B,V,4] (positions, 0 terminated) exactly as src/bfs/bfs.cu:46-98 defines
- *   them, plus level_start [B,V+1] / num_levels [B]: the order is level-contiguous and deterministic.
+ *   them, plus level_start [B,V+1] / num_levels [B]: the order is level-contiguous and deterministic.  The tree is
+ *   rooted at vertex `root` (the reference: always vertex 0).  The filter's result does not depend on the root; the
+ *   number of dependent levels of every pass does: about half from the centre of the map.
  * bxs_tree_levels: recovers level_start / num_levels from a level-contiguous sorted_parent (scratch 16*B*V bytes).
- * bxs_refine_forward: feature f32 [B,C,V] (vertex order), edge_weight f32 [B,V] (sorted order; entry 0 is
- *   ignored = 0 and NOT overwritten, unlike refine.cu:43-46) -> feature_out, aggr [B,C,V], aggr_up [B,C,V],
- *   wsum [B,V], wsum_up [B,V] (the five tensors of refine.cu:201-249).  scratch: bxs_refine_scratch_bytes.
- * bxs_refine_backward_feature / _weight: refine.cu:251-370.
+ * bxs_refine_forward_grouped: feature f32 [n,C,V] (vertex order), edge_weight f32 [G,V] (sorted order; entry 0 is
+ *   ignored = 0 and NOT overwritten, unlike refine.cu:43-46) -> feature_out, aggr [n,C,V], aggr_up [n,C,V],
+ *   wsum [G,V], wsum_up [G,V] (the five tensors of refine.cu:201-249).
+ * bxs_refine_backward_feature_grouped / _weight_grouped: refine.cu:251-370.
+ * The refine entry points take n instances that share G trees: tree_of [n] int32 -> tree.  The instances of one image
+ * share the image's tree in the heads (box_solov2_head.py:300-305,353; box2mask_head.py:271-276).  tree_of == NULL:
+ * instance i uses tree i (the reference's one tree per batch entry); n must equal G.  edge_weight / sorted_* /
+ * level_start / num_levels / wsum / wsum_up are per TREE ([G,...]); feature, feature_out, aggr, aggr_up, grad_* are
+ * per INSTANCE ([n,...]).  The normaliser is computed once per tree.  bxs_refine_backward_weight_grouped returns d/d
+ * edge_weight per instance [n,V]; with a tree_of table the caller sums the rows of a tree.
+ * scratch: bxs_refine_scratch_bytes(max(n, G), C, V).
  * --------------------------------------------------------------------------------------- */
 int64_t bxs_mst_workspace_bytes(int64_t B, int64_t E, int64_t V);
 int bxs_mst_forward(const int32_t* edge_index, const float* edge_weight, int32_t* edge_out, void* workspace,
                     int64_t B, int64_t E, int64_t V, bxs_stream_t stream);
 int64_t bxs_bfs_workspace_bytes(int64_t B, int64_t V);
-int bxs_bfs_forward(const int32_t* tree_edges, int32_t* sorted_index, int32_t* sorted_parent,
-                    int32_t* sorted_child, int32_t* level_start, int32_t* num_levels, void* workspace,
-                    int64_t B, int64_t V, int max_adj, bxs_stream_t stream);
-/* same, rooted at vertex `root` instead of vertex 0 (the filter's result does not depend on the root; the number of
- * dependent levels of every pass does: about half from the centre of the map) */
 int bxs_bfs_forward_rooted(const int32_t* tree_edges, int32_t* sorted_index, int32_t* sorted_parent,
                     int32_t* sorted_child, int32_t* level_start, int32_t* num_levels, void* workspace,
                     int64_t B, int64_t V, int max_adj, int64_t root, bxs_stream_t stream);
 int bxs_tree_levels(const int32_t* sorted_parent, int32_t* level_start, int32_t* num_levels, void* scratch,
                     int64_t B, int64_t V, bxs_stream_t stream);
 int64_t bxs_refine_scratch_bytes(int64_t B, int64_t C, int64_t V);
-int bxs_refine_forward(const float* feature, const float* edge_weight, const int32_t* sorted_index,
-                       const int32_t* sorted_parent, const int32_t* sorted_child, const int32_t* level_start,
-                       const int32_t* num_levels, float* feature_out, float* aggr, float* aggr_up, float* wsum,
-                       float* wsum_up, void* scratch, int64_t B, int64_t C, int64_t V, bxs_stream_t stream);
-int bxs_refine_backward_feature(const float* edge_weight, const int32_t* sorted_index,
-                                const int32_t* sorted_parent, const int32_t* sorted_child,
-                                const int32_t* level_start, const int32_t* num_levels, const float* wsum,
-                                const float* grad_out, float* grad_feature, void* scratch, int64_t B, int64_t C,
-                                int64_t V, bxs_stream_t stream);
-int bxs_refine_backward_weight(const float* edge_weight, const int32_t* sorted_index,
+int bxs_refine_forward_grouped(const float* feature, const float* edge_weight, const int32_t* sorted_index,
                                const int32_t* sorted_parent, const int32_t* sorted_child,
-                               const int32_t* level_start, const int32_t* num_levels, const float* feature_out,
-                               const float* aggr, const float* aggr_up, const float* wsum, const float* wsum_up,
-                               const float* grad_out, float* grad_weight, void* scratch, int64_t B, int64_t C,
-                               int64_t V, bxs_stream_t stream);
+                               const int32_t* level_start, const int32_t* num_levels, const int32_t* tree_of,
+                               float* feature_out, float* aggr, float* aggr_up, float* wsum, float* wsum_up,
+                               void* scratch, int64_t n, int64_t G, int64_t C, int64_t V, bxs_stream_t stream);
+int bxs_refine_backward_feature_grouped(const float* edge_weight, const int32_t* sorted_index,
+                                        const int32_t* sorted_parent, const int32_t* sorted_child,
+                                        const int32_t* level_start, const int32_t* num_levels,
+                                        const int32_t* tree_of, const float* wsum, const float* grad_out,
+                                        float* grad_feature, void* scratch, int64_t n, int64_t G, int64_t C,
+                                        int64_t V, bxs_stream_t stream);
+int bxs_refine_backward_weight_grouped(const float* edge_weight, const int32_t* sorted_index,
+                                       const int32_t* sorted_parent, const int32_t* sorted_child,
+                                       const int32_t* level_start, const int32_t* num_levels,
+                                       const int32_t* tree_of, const float* feature_out, const float* aggr,
+                                       const float* aggr_up, const float* wsum, const float* wsum_up,
+                                       const float* grad_out, float* grad_weight, void* scratch, int64_t n,
+                                       int64_t G, int64_t C, int64_t V, bxs_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------
  * a2/a3/a4  dense dynamic 1x1 convolution on the Hopper tensor cores (wgmma, TMA fed)
@@ -338,31 +331,6 @@ int bxs_dynconv1x1_backward(const float* feat, const float* kernels, const float
  * --------------------------------------------------------------------------------------- */
 int bxs_upsampled_rowcol_max(const float* x, float* row_prof, float* col_prof, void* workspace, int64_t n,
                              int64_t h, int64_t w, int64_t H, int64_t W, int sigmoid_act, bxs_stream_t stream);
-
-/* Grouped forms of the three refine entry points: n instances share G trees (tree_of [n] int32 -> group), as the
- * heads use them -- the instances of one image share the image's tree (box_solov2_head.py:300-305,353;
- * box2mask_head.py:271-276).  edge_weight / sorted_* / level_start / num_levels / wsum / wsum_up are per GROUP
- * ([G,...]); feature, feature_out, aggr, aggr_up, grad_* are per INSTANCE ([n,...]).  The normaliser is computed once
- * per group.  bxs_refine_backward_weight_grouped returns d/d edge_weight per instance [n,V]; the caller sums the
- * rows of a group.  scratch: bxs_refine_scratch_bytes(max(n, G), C, V). */
-int bxs_refine_forward_grouped(const float* feature, const float* edge_weight, const int32_t* sorted_index,
-                               const int32_t* sorted_parent, const int32_t* sorted_child,
-                               const int32_t* level_start, const int32_t* num_levels, const int32_t* tree_of,
-                               float* feature_out, float* aggr, float* aggr_up, float* wsum, float* wsum_up,
-                               void* scratch, int64_t n, int64_t G, int64_t C, int64_t V, bxs_stream_t stream);
-int bxs_refine_backward_feature_grouped(const float* edge_weight, const int32_t* sorted_index,
-                                        const int32_t* sorted_parent, const int32_t* sorted_child,
-                                        const int32_t* level_start, const int32_t* num_levels,
-                                        const int32_t* tree_of, const float* wsum, const float* grad_out,
-                                        float* grad_feature, void* scratch, int64_t n, int64_t G, int64_t C,
-                                        int64_t V, bxs_stream_t stream);
-int bxs_refine_backward_weight_grouped(const float* edge_weight, const int32_t* sorted_index,
-                                       const int32_t* sorted_parent, const int32_t* sorted_child,
-                                       const int32_t* level_start, const int32_t* num_levels,
-                                       const int32_t* tree_of, const float* feature_out, const float* aggr,
-                                       const float* aggr_up, const float* wsum, const float* wsum_up,
-                                       const float* grad_out, float* grad_weight, void* scratch, int64_t n,
-                                       int64_t G, int64_t C, int64_t V, bxs_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------
  * a18  bilinear resize      replaces F.interpolate(mode='bilinear') as the heads call it:

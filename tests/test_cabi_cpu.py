@@ -41,13 +41,17 @@ def test_identity_and_no_device(lib):
         assert h.bxs_device_sm_count() == -4          # BXS_ERR_NO_DEVICE, no crash
 
 
-def test_argument_validation_without_gpu(lib):
+def test_workspace_queries_and_argument_validation_without_gpu(lib):
     h = lib.lib()
     assert h.bxs_pairwise_nlog_forward(None, None, 1, 4, 4, 3, 2, 0, None) == -1      # null pointers
     assert h.bxs_boxinst_loss_workspace_bytes(128, 200, 256) > 0
     assert h.bxs_boxinst_loss_workspace_bytes(0, 200, 256) == 0
-    assert h.bxs_levelset_workspace_bytes(16) > 0 and h.bxs_lcm_workspace_bytes(8, 96, 96) > 0
+    assert h.bxs_levelset_fused_workspace_bytes(16) > 0 and h.bxs_lcm_workspace_bytes(8, 96, 96) > 0
     assert h.bxs_mst_workspace_bytes(2, 18240, 9216) > 0 and h.bxs_refine_scratch_bytes(2, 1, 9216) > 0
+    p = ctypes.cast((ctypes.c_float * 64)(), ctypes.c_void_p)
+    assert h.bxs_refine_forward_grouped(*[p] * 7, None, *[p] * 6, 2, 3, 1, 16, None) == -1    # no tree_of: n must equal G
+    assert h.bxs_refine_backward_feature_grouped(*[p] * 6, None, *[p] * 4, 2, 3, 1, 16, None) == -1
+    assert h.bxs_refine_backward_weight_grouped(*[p] * 6, None, *[p] * 8, 2, 3, 1, 16, None) == -1
 
 
 def test_ops_fail_loudly_on_cpu_tensors(lib):

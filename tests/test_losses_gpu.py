@@ -95,6 +95,26 @@ def test_levelset_vs_oracle(n, C, h, w):
     gs, gt = torch.autograd.grad((out * gl.to(DEV)).sum(), [sg, tg])
     assert torch.allclose(out.cpu().double(), ref.detach(), rtol=1e-4, atol=1e-7)
     assert rel_err(gs.cpu(), rs) < 1e-4 and rel_err(gt.cpu(), rt) < 1e-4
+    # region_levelset: the energy alone (pixel_num = 1, loss_weight = 1)
+    from boxinstseg_b200.models.losses import region_levelset
+    from oracle.levelset import region_levelset as oracle_region
+    ref = oracle_region(torch.cat([s64, 1 - s64], 1) * m.double(), t64 * m.double())
+    rs, rt = torch.autograd.grad((ref * gl.double()).sum(), [s64, t64])
+    out = region_levelset()(torch.cat([sg, 1 - sg], 1) * md, tg * md)
+    gs, gt = torch.autograd.grad((out * gl.to(DEV)).sum(), [sg, tg])
+    assert torch.allclose(out.cpu().double(), ref.detach(), rtol=1e-4, atol=1e-7)
+    assert rel_err(gs.cpu(), rs) < 1e-4 and rel_err(gt.cpu(), rt) < 1e-4
+
+
+def test_levelset_more_than_eight_channels_is_unsupported():
+    """The level-set kernels unroll at most 8 target channels: more is an error, never a silent fallback."""
+    from boxinstseg_b200._lib import BoxSegError
+    from boxinstseg_b200.models.losses import LevelsetLoss, region_levelset
+    s, t = torch.rand(2, 2, 8, 8, device=DEV), torch.rand(2, 9, 8, 8, device=DEV)
+    with pytest.raises(BoxSegError, match='unsupported shape'):
+        LevelsetLoss()(s, t, torch.ones(2, device=DEV))
+    with pytest.raises(BoxSegError, match='unsupported shape'):
+        region_levelset()(s, t)
 
 
 def test_length_regularization_grad():

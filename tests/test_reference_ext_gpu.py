@@ -146,8 +146,17 @@ def test_reference_bfs_order_is_accepted(ref):
     assert rel_err(gf, _stored(ref, 'bfs_gfeat')) <= 1e-5
     gw = ours.refine_backward_weight(feat, ew, ridx, rpar, rchd, o[0], o[1], o[2], o[3], o[4], gout)
     assert rel_err(gw[:, 1:], _stored(ref, 'bfs_gweight')[:, 1:]) <= 1e-4
-    # and the same tree through our own deterministic order gives the same filter output
+    # the same order through the grouped path (autograd, one tree per instance: tree_of = arange(B)) is adopted as well,
+    # never run with the level table of another order
+    from boxinstseg_b200.ops.tree_filter import refine
     B, V = ew.shape
+    f, w = feat.clone().requires_grad_(True), ew.clone().requires_grad_(True)
+    og = refine(f, w, ridx, rpar, rchd, False, torch.arange(B, dtype=torch.int32, device=DEV))
+    assert rel_err(og, _stored(ref, 'bfs_out0')) <= 1e-5
+    gfg, gwg = torch.autograd.grad((og * gout).sum(), [f, w])
+    assert rel_err(gfg, _stored(ref, 'bfs_gfeat')) <= 1e-5
+    assert rel_err(gwg[:, 1:], _stored(ref, 'bfs_gweight')[:, 1:]) <= 1e-4
+    # and the same tree through our own deterministic order gives the same filter output
     idx, par, chd = ours.bfs_forward(tree, 4)
     wv = torch.zeros(B, V, device=DEV).scatter_(1, ridx.long(), ew)   # weight of the edge (vertex -> parent), by vertex id
     o2 = ours.refine_forward(feat, torch.gather(wv, 1, idx.long()), idx, par, chd)[0]

@@ -1,7 +1,7 @@
 """Per-operator timings on the GPU box at the shapes of SURVEY section 8d (configs C/D/E): dynamic conv (wgmma, forward and
-both gradients, against cuBLAS TF32 and FP32), CondInst head, tree filter (MST / BFS / refine), level set (dense op and the
-fused assembly), projection, LCM, mean field, targets.  Every op is timed twice: eager (launch overhead included) and as a
-CUDA-graph replay (`*_graph_us`; device time only).  Prints one JSON object."""
+both gradients, against cuBLAS TF32 and FP32), CondInst head, tree filter (MST / BFS / refine), level set (LevelsetLoss on
+dense inputs and the fused assembly), projection, LCM, mean field, targets.  Every op is timed twice: eager (launch overhead
+included) and as a CUDA-graph replay (`*_graph_us`; device time only).  Prints one JSON object."""
 import json
 import os
 import sys
@@ -113,7 +113,7 @@ m = torch.zeros(16, 1, 200, 256, device=dev)
 m[:, :, 40:150, 60:200] = 1
 pix = m.sum((1, 2, 3))
 ls = LevelsetLoss()
-both(res, 'levelset_dense_fwd_bwd', lambda: torch.autograd.grad(ls(torch.cat([s, 1 - s], 1) * m, t * m, pix).sum(), s))
+both(res, 'levelset_loss_fwd_bwd', lambda: torch.autograd.grad(ls(torch.cat([s, 1 - s], 1) * m, t * m, pix).sum(), s))
 both(res, 'levelset_fused_fwd_bwd', lambda: torch.autograd.grad(levelset_assembly(logit, m, t).sum(), logit))
 both(res, 'projection_fwd_bwd', lambda: torch.autograd.grad(projection_losses(s, m).sum(), s))
 phi = torch.rand(8, 1, 96, 96, device=dev, generator=g).requires_grad_(True)

@@ -26,7 +26,8 @@ for (n, h, w) in [(2, 200, 256), (16, 200, 256), (2, 96, 96), (2, 50, 64)]:
     lvl = torch.empty((B, V + 1), dtype=torch.int32, device=dev); nlv = torch.empty(B, dtype=torch.int32, device=dev)
     nbytes = lib.bxs_bfs_workspace_bytes(B, V)
     ws = torch.zeros(nbytes, dtype=torch.uint8, device=dev)
-    rc = lib.bxs_bfs_forward(L.ptr(tree), L.ptr(idx), L.ptr(par), L.ptr(chd), L.ptr(lvl), L.ptr(nlv), L.ptr(ws), B, V, 4, L.stream())
+    rc = lib.bxs_bfs_forward_rooted(L.ptr(tree), L.ptr(idx), L.ptr(par), L.ptr(chd), L.ptr(lvl), L.ptr(nlv), L.ptr(ws), B, V, 4, 0,
+                                    L.stream())
     torch.cuda.synchronize()
     al = lambda v: (v + 255) // 256 * 256
     off = al(4 * B * V); off = al(off + 16 * B * V); off = al(off + 4 * B * V)
