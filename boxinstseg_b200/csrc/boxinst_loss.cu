@@ -49,34 +49,30 @@ struct Workspace {
   size_t total_bytes;
 };
 
-inline size_t align_up(size_t v, size_t a = 256) { return (v + a - 1) / a * a; }
-
 inline Workspace carve(void* base, int64_t N, int64_t H, int64_t W) {
   Workspace w{};
-  char* p = (char*)base;
-  size_t off = 0;
-  auto take = [&](size_t bytes) { char* r = p + off; off = align_up(off + bytes); return r; };
-  w.col_packed = (unsigned long long*)take(sizeof(unsigned long long) * N * W);
-  w.weight_sum = (unsigned long long*)take(sizeof(unsigned long long));
-  w.ticket = (unsigned int*)take(sizeof(unsigned int));
-  w.inst_ticket = (unsigned int*)take(sizeof(unsigned int) * N);
-  w.zero_bytes_fast = off;
-  w.row_packed = (unsigned long long*)take(sizeof(unsigned long long) * N * H);
-  w.zero_bytes = off;
-  w.coef_row = (float*)take(sizeof(float) * N * H);
-  w.coef_col = (float*)take(sizeof(float) * N * W);
-  w.row_arg = (int*)take(sizeof(int) * N * H);
-  w.col_arg = (int*)take(sizeof(int) * N * W);
-  w.tile_prefix = (int*)take(sizeof(int) * (N + 1));
+  Carver c(base);
+  w.col_packed = (unsigned long long*)c.take(sizeof(unsigned long long) * N * W);
+  w.weight_sum = (unsigned long long*)c.take(sizeof(unsigned long long));
+  w.ticket = (unsigned int*)c.take(sizeof(unsigned int));
+  w.inst_ticket = (unsigned int*)c.take(sizeof(unsigned int) * N);
+  w.zero_bytes_fast = c.off;
+  w.row_packed = (unsigned long long*)c.take(sizeof(unsigned long long) * N * H);
+  w.zero_bytes = c.off;
+  w.coef_row = (float*)c.take(sizeof(float) * N * H);
+  w.coef_col = (float*)c.take(sizeof(float) * N * W);
+  w.row_arg = (int*)c.take(sizeof(int) * N * H);
+  w.col_arg = (int*)c.take(sizeof(int) * N * W);
+  w.tile_prefix = (int*)c.take(sizeof(int) * (N + 1));
   const int64_t tiles_full = ceil_div(H, TH) * ceil_div(W, TW);
   const int64_t per_inst = std::max<int64_t>(tiles_full, 128);         // generic: tiles; fast: one per pair-role warp
-  w.pair_partial = (float*)take(sizeof(float) * N * per_inst);
-  w.den_partial = (int*)take(sizeof(int) * N * per_inst);
-  w.inst_prj = (float*)take(sizeof(float) * N);
-  w.inst_num = (float*)take(sizeof(float) * N);
-  w.scale_pair = (float*)take(sizeof(float));
-  w.inst_rec = (int*)take(sizeof(int) * 16 * N);
-  w.total_bytes = off;
+  w.pair_partial = (float*)c.take(sizeof(float) * N * per_inst);
+  w.den_partial = (int*)c.take(sizeof(int) * N * per_inst);
+  w.inst_prj = (float*)c.take(sizeof(float) * N);
+  w.inst_num = (float*)c.take(sizeof(float) * N);
+  w.scale_pair = (float*)c.take(sizeof(float));
+  w.inst_rec = (int*)c.take(sizeof(int) * 16 * N);
+  w.total_bytes = c.off;
   return w;
 }
 

@@ -51,8 +51,6 @@ struct OpWorkspace {
   size_t total_bytes;
 };
 
-inline size_t op_align(size_t v, size_t a = 256) { return (v + a - 1) / a * a; }
-
 #ifndef BXS_OP_LEN
 #define BXS_OP_LEN 12
 #endif
@@ -69,55 +67,23 @@ inline int64_t op_max_groups(int64_t H, int64_t W) {      // upper bound of ceil
 
 inline OpWorkspace op_carve(void* base, int64_t N, int64_t H, int64_t W) {
   OpWorkspace w{};
-  char* p = (char*)base;
-  size_t off = 0;
-  auto take = [&](size_t bytes) { char* r = p + off; off = op_align(off + bytes); return r; };
+  Carver c(base);
   const int64_t S = ceil_div(H, OP_R);
-  w.row_packed = (unsigned long long*)take(8 * N * H);
-  w.col_part = (unsigned long long*)take(8 * N * S * W);
+  w.row_packed = (unsigned long long*)c.take(8 * N * H);
+  w.col_part = (unsigned long long*)c.take(8 * N * S * W);
   const int64_t G = op_max_groups(H, W);
-  w.num_part = (float*)take(4 * N * G);
-  w.coef_row = (float*)take(4 * N * H);
-  w.coef_col = (float*)take(4 * N * W);
-  w.arg_row = (int*)take(4 * N * H);
-  w.arg_col = (int*)take(4 * N * W);
-  w.span = (int*)take(16 * N);
-  w.inst_prj = (float*)take(4 * N);
-  w.inst_num = (float*)take(4 * N);
-  w.sv_row = (float*)take(4 * N * H);
-  w.sv_col = (float*)take(4 * N * W);
-  w.total_bytes = off;
+  w.num_part = (float*)c.take(4 * N * G);
+  w.coef_row = (float*)c.take(4 * N * H);
+  w.coef_col = (float*)c.take(4 * N * W);
+  w.arg_row = (int*)c.take(4 * N * H);
+  w.arg_col = (int*)c.take(4 * N * W);
+  w.span = (int*)c.take(16 * N);
+  w.inst_prj = (float*)c.take(4 * N);
+  w.inst_num = (float*)c.take(4 * N);
+  w.sv_row = (float*)c.take(4 * N * H);
+  w.sv_col = (float*)c.take(4 * N * W);
+  w.total_bytes = c.off;
   return w;
-}
-
-// ---------------------------------------------------------------------------------------
-// PTX wrappers: mbarrier + 1-D bulk copy (TMA engine, no tensor map needed for a contiguous strip)
-// ---------------------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t op_smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void op_mbar_init(uint64_t* bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(op_smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void op_mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(op_smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void op_mbar_wait(uint64_t* bar, uint32_t parity) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred P1;\n\t"
-      "OP_WAIT:\n\t"
-      "mbarrier.try_wait.parity.shared::cta.b64 P1, [%0], %1;\n\t"
-      "@P1 bra OP_DONE;\n\t"
-      "bra OP_WAIT;\n\t"
-      "OP_DONE:\n\t"
-      "}" ::"r"(op_smem_u32(bar)),
-      "r"(parity)
-      : "memory");
-}
-__device__ __forceinline__ void op_bulk_g2s(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
-                   op_smem_u32(dst)),
-               "l"(src), "r"(bytes), "r"(op_smem_u32(bar))
-               : "memory");
 }
 
 // ---------------------------------------------------------------------------------------
@@ -393,16 +359,16 @@ onepass_main_kernel(const float* __restrict__ logits, const uint8_t* __restrict_
     info.c_lo = sp.c_lo; info.c_hi = sp.c_hi;
     s_info[stage] = info;
     const uint32_t bytes = (uint32_t)rows * (uint32_t)W * 4u;
-    op_mbar_expect_tx(&s_bar[stage], bytes);
-    op_bulk_g2s(xbuf + (size_t)stage * stage_floats, logits + ((int64_t)info.n * H + y0) * W, bytes, &s_bar[stage]);
+    mbar_expect_tx(&s_bar[stage], bytes);
+    bulk_g2s(xbuf + (size_t)stage * stage_floats, logits + ((int64_t)info.n * H + y0) * W, bytes, &s_bar[stage]);
   };
 
   unsigned fetched = 0;          // thread 0: next queue position (fetched one iteration ahead of its use)
   if (tid == 0) {
 #pragma unroll
-    for (int i = 0; i < OP_STAGES; ++i) op_mbar_init(&s_bar[i], 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+    for (int i = 0; i < OP_STAGES; ++i) mbar_init(&s_bar[i], 1);
+    fence_mbarrier_init();
+    fence_proxy_async_smem();
     fetched = gridDim.x + atomicAdd(&sched->next, 1u);
   }
   for (int n = tid; n < N; n += OP_NT) s_rec[n] = make_srec(rects, inst_gt, gt_img, n, H, W);
@@ -453,7 +419,7 @@ onepass_main_kernel(const float* __restrict__ logits, const uint8_t* __restrict_
       const int y0 = it.s * OP_R;
       const int rows = min(OP_R, H - y0);
       const int ya = it.ya, yb = it.yb;
-      op_mbar_wait(&s_bar[stage], (phases >> stage) & 1u);
+      mbar_wait(&s_bar[stage], (phases >> stage) & 1u);
       phases ^= 1u << stage;
       const float* xb = xbuf + (size_t)stage * stage_floats;       // strip row r at xb[r * W + col]
       // ---- row maxima (one warp per row, the warp's rows unrolled together) + zero stores outside the span ----
@@ -754,28 +720,9 @@ int op_launch_main(cudaStream_t st, const float* logits, const uint8_t* edge_bit
                    float* g_logits) {
   const size_t smem = op_smem_bytes(N, W);
   auto kern = onepass_main_kernel<NCHUNK, D, FULLW>;
-  constexpr int kMaxDev = 64;
-  static thread_local size_t configured[kMaxDev] = {};   // per instantiation and device: opted-in dynamic shared memory
-  static thread_local int occ_dev = -1, occ = 0;
-  static thread_local size_t occ_smem = 0;
-  int dev = 0;
-  cudaGetDevice(&dev);
-  const bool tracked = dev >= 0 && dev < kMaxDev;
-  if (!tracked || smem > configured[dev]) {
-    if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) {
-      set_last_error(cudaGetLastError());
-      return BXS_ERR_UNSUPPORTED;
-    }
-    if (tracked) configured[dev] = smem;
-  }
-  if (dev != occ_dev || smem != occ_smem) {
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, OP_NT, smem) != cudaSuccess || occ < 1) {
-      set_last_error(cudaGetLastError());
-      return BXS_ERR_UNSUPPORTED;
-    }
-    occ_dev = dev;
-    occ_smem = smem;
-  }
+  if (opt_in_smem(kern, smem) != BXS_OK) return BXS_ERR_UNSUPPORTED;
+  const int occ = max_active_ctas(kern, OP_NT, smem);
+  if (occ < 1) return BXS_ERR_UNSUPPORTED;
   const int S = (int)ceil_div(H, OP_R);
   const int64_t total = (int64_t)N * S;           // stream items alone; pair items come on top
   const int grid = (int)std::min<int64_t>(total, (int64_t)sm_count() * occ);
@@ -813,7 +760,7 @@ extern "C" int64_t bxs_boxinst_loss_fused_workspace_bytes(int64_t N, int64_t H, 
   if (N <= 0 || H <= 0 || W <= 0) return 0;
   size_t plan = 0;
   for (int d = 1; d <= 4; ++d) plan = std::max(plan, wq_plan_bytes(N, H, W, d));
-  return (int64_t)(op_align(op_carve(nullptr, N, H, W).total_bytes) + plan);
+  return (int64_t)(align_up(op_carve(nullptr, N, H, W).total_bytes) + plan);
 }
 
 extern "C" int64_t bxs_boxinst_loss_fused_sched_bytes(void) {
@@ -863,7 +810,7 @@ extern "C" int bxs_boxinst_loss_fused_forward(const float* logits, const uint8_t
   cudaStream_t st = as_stream(stream);
   OpWorkspace ws = op_carve(workspace, N, H, W);
   if (!op_use_cta_schedule()) {            // plan in the tail of the workspace, then the warp-granular kernel
-    unsigned char* plan = reinterpret_cast<unsigned char*>(workspace) + op_align(ws.total_bytes);
+    unsigned char* plan = reinterpret_cast<unsigned char*>(workspace) + align_up(ws.total_bytes);
     const int prc = wq_build_plan(st, edge_bits, rects, inst_gt, gt_img, plan, (int)N, (int)H, (int)W, dilation);
     if (prc != BXS_OK) return prc;
     return wq_forward(st, logits, edge_bits, plan, iter_ptr, warmup_iters, ws, reinterpret_cast<WqSched*>(sched_state),

@@ -177,12 +177,6 @@ __global__ void bitmask_kernel(const int32_t* __restrict__ rects, float* __restr
   }
 }
 
-inline int grid_for(int64_t total, int block = 256) {
-  int64_t g = (total + block - 1) / block;
-  int64_t cap = (int64_t)sm_count() * 8;
-  return (int)(g < cap ? (g > 0 ? g : 1) : cap);
-}
-
 }  // namespace
 }  // namespace bxs
 
@@ -225,7 +219,7 @@ extern "C" int bxs_boxinst_bitmasks(const int32_t* rects, float* bitmasks, int64
                                     bxs_stream_t stream) {
   if (G == 0) return BXS_OK;
   if (!rects || !bitmasks || G < 0 || H <= 0 || W <= 0) return BXS_ERR_INVALID_ARG;
-  bitmask_kernel<<<grid_for(G * H * W), 256, 0, as_stream(stream)>>>(rects, bitmasks, G, (int)H, (int)W);
+  bitmask_kernel<<<grid_for(G * H * W, 256), 256, 0, as_stream(stream)>>>(rects, bitmasks, G, (int)H, (int)W);
   return check_launch();
 }
 

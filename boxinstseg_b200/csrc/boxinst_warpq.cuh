@@ -1,6 +1,6 @@
 // a6 + a7 + a8, single pass, second schedule: ONE persistent kernel whose unit of work is a WARP item, plus a small
 // finalize kernel.  (Included by boxinst_onepass.cu inside namespace bxs::{anonymous}; shares SRec / op_span /
-// chain_geom / op_chain and the PTX wrappers with the CTA-granular schedule there.)
+// chain_geom / op_chain with the CTA-granular schedule there.)
 //
 // Why: the CTA-granular kernel (onepass_main_kernel) spent 31 % of its duration with SMs idle (per-CTA prologue of
 // 128 record loads + a block scan, a tail of CTA-wide pair items), its top stall was the CTA barrier around the strip
@@ -267,9 +267,9 @@ wq_main_kernel(const float* __restrict__ logits, const uint8_t* __restrict__ edg
   asm volatile("griddepcontrol.launch_dependents;");
   if (warp < WQ_STREAMERS && lane == 0) {
 #pragma unroll
-    for (int i = 0; i < WQ_RING; ++i) op_mbar_init(&s_bar[warp][i], 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+    for (int i = 0; i < WQ_RING; ++i) mbar_init(&s_bar[warp][i], 1);
+    fence_mbarrier_init();
+    fence_proxy_async_smem();
   }
   if (threadIdx.x == 0) s_exit = 0u;
   __syncthreads();                                         // the only CTA-wide barrier of this kernel
@@ -301,9 +301,9 @@ wq_main_kernel(const float* __restrict__ logits, const uint8_t* __restrict__ edg
       if (lane == 0) {
         const uint32_t bytes = (uint32_t)min(WQ_SUB, nrows - ik * WQ_SUB) * (uint32_t)W * 4u;
         uint64_t* bb = &bar[gi & (WQ_RING - 1)];
-        op_mbar_expect_tx(bb, bytes);
-        op_bulk_g2s(ring + (gi & (WQ_RING - 1)) * stage_floats, logits + ((size_t)n * H + row0) * W + (size_t)ik * stage_floats,
-                    bytes, bb);
+        mbar_expect_tx(bb, bytes);
+        bulk_g2s(ring + (gi & (WQ_RING - 1)) * stage_floats, logits + ((size_t)n * H + row0) * W + (size_t)ik * stage_floats,
+                 bytes, bb);
       }
       ++gi;
       if (++ik == (nrows + WQ_SUB - 1) / WQ_SUB) { ik = 0; ++iq; }
@@ -334,7 +334,7 @@ wq_main_kernel(const float* __restrict__ logits, const uint8_t* __restrict__ edg
       int y = row0;
       for (int k = 0; k < nsub; ++k) {
         const int st = gp & (WQ_RING - 1);
-        op_mbar_wait(&bar[st], (unsigned)(gp >> 2) & 1u);
+        mbar_wait(&bar[st], (unsigned)(gp >> 2) & 1u);
         const float* xb = ring + st * stage_floats + lane * 4;
         const int rows_here = min(WQ_SUB, nrows - k * WQ_SUB);
         float gm[NCHUNK][4];                 // column maxima of this 4-row group
@@ -494,7 +494,7 @@ wq_main_kernel(const float* __restrict__ logits, const uint8_t* __restrict__ edg
     // sequentially-consistent fence.  The other warps' stores reach the finalize CTAs by cumulativity: store -> release
     // (cta) -> acquire (cta) by the last warp -> release (gpu) -> acquire (gpu) by the poll.
     unsigned old;
-    asm volatile("atom.acq_rel.cta.shared::cta.add.u32 %0, [%1], 1;" : "=r"(old) : "r"((unsigned)__cvta_generic_to_shared(&s_exit)) : "memory");
+    asm volatile("atom.acq_rel.cta.shared::cta.add.u32 %0, [%1], 1;" : "=r"(old) : "r"(smem_u32(&s_exit)) : "memory");
     if (old == WQ_NW - 1)
       asm volatile("red.release.gpu.global.add.u32 [%0], %1;" ::"l"(&sched->done), "r"((unsigned)WQ_NW) : "memory");
 #endif
@@ -698,28 +698,9 @@ int wq_launch_main(cudaStream_t st, const float* logits, const uint8_t* edge_bit
                    float* g_logits) {
   const size_t smem = wq_smem_bytes(W);
   auto kern = wq_main_kernel<NCHUNK, D, FULLW>;
-  constexpr int kMaxDev = 64;
-  static thread_local size_t configured[kMaxDev] = {};   // per instantiation and device: opted-in dynamic shared memory
-  static thread_local int occ_dev = -1, occ = 0;
-  static thread_local size_t occ_smem = 0;
-  int dev = 0;
-  cudaGetDevice(&dev);
-  const bool tracked = dev >= 0 && dev < kMaxDev;
-  if (!tracked || smem > configured[dev]) {
-    if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) {
-      set_last_error(cudaGetLastError());
-      return BXS_ERR_UNSUPPORTED;
-    }
-    if (tracked) configured[dev] = smem;
-  }
-  if (dev != occ_dev || smem != occ_smem) {
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, WQ_NT, smem) != cudaSuccess || occ < 1) {
-      set_last_error(cudaGetLastError());
-      return BXS_ERR_UNSUPPORTED;
-    }
-    occ_dev = dev;
-    occ_smem = smem;
-  }
+  if (opt_in_smem(kern, smem) != BXS_OK) return BXS_ERR_UNSUPPORTED;
+  const int occ = max_active_ctas(kern, WQ_NT, smem);
+  if (occ < 1) return BXS_ERR_UNSUPPORTED;
   // the pair-item count lives in the plan (device memory): size the grid for the machine, bounded by the largest
   // possible queue; warps beyond the queues leave at once
   const int64_t max_items = (int64_t)N * (wq_strips(H) + wq_max_chains(H, W, D));

@@ -3,6 +3,10 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <algorithm>
+#include <map>
+#include <utility>
+
 #include "../../include/boxseg_b200.h"
 
 #if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ != 900)
@@ -30,6 +34,134 @@ inline cudaStream_t as_stream(bxs_stream_t s) { return reinterpret_cast<cudaStre
 inline int64_t ceil_div(int64_t a, int64_t b) { return (a + b - 1) / b; }
 
 int sm_count();
+
+// ---------------------------------------------------------------------------------------
+// launch configuration
+// ---------------------------------------------------------------------------------------
+namespace {    // one memo per source file, which launches only its own kernels; nothing exported from the library
+struct KernelState {
+  size_t smem_allowed = 0;             // dynamic shared memory opted in to
+  int occ_threads = -1, occ = 0;       // last occupancy query and its answer
+  size_t occ_smem = 0;
+};
+// Keyed by the kernel's address, not its type: instantiations with the same signature share a type.  Per thread, so
+// no lock; another thread repeats an opt-in or a query, which is harmless.
+inline KernelState& kernel_state(const void* kern) {
+  static thread_local std::map<std::pair<const void*, int>, KernelState> states;
+  int dev = 0;
+  cudaGetDevice(&dev);
+  return states[{kern, dev}];
+}
+
+// Lets `kern` use up to `smem` bytes of dynamic shared memory on the current device (a launch above 48 KB needs it).
+// Remembered per (kernel, device): a later call asking for no more skips the driver.  Returns BXS_OK, or
+// BXS_ERR_LAUNCH with bxs_last_error() set.
+inline int opt_in_smem(const void* kern, size_t smem) {
+  KernelState& s = kernel_state(kern);
+  if (smem <= s.smem_allowed) return BXS_OK;
+  const cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  if (e != cudaSuccess) {
+    cudaGetLastError();
+    set_last_error(e);
+    return BXS_ERR_LAUNCH;
+  }
+  s.smem_allowed = smem;
+  return BXS_OK;
+}
+
+// CTAs of `kern` resident per SM at `threads` threads and `smem` bytes of dynamic shared memory on the current device,
+// remembered per (kernel, device) for the last (threads, smem) asked.  0 when none fit or the query fails (then with
+// bxs_last_error() set).
+inline int max_active_ctas(const void* kern, int threads, size_t smem) {
+  KernelState& s = kernel_state(kern);
+  if (threads != s.occ_threads || smem != s.occ_smem) {
+    int occ = 0;
+    const cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, threads, smem);
+    if (e != cudaSuccess) {
+      cudaGetLastError();
+      set_last_error(e);
+      return 0;
+    }
+    s.occ_threads = threads;
+    s.occ_smem = smem;
+    s.occ = occ;
+  }
+  return s.occ;
+}
+
+template <typename... A>
+inline int opt_in_smem(void (*kern)(A...), size_t smem) {
+  return opt_in_smem(reinterpret_cast<const void*>(kern), smem);
+}
+template <typename... A>
+inline int max_active_ctas(void (*kern)(A...), int threads, size_t smem) {
+  return max_active_ctas(reinterpret_cast<const void*>(kern), threads, smem);
+}
+}  // namespace
+
+// 1-D grid of a grid-stride kernel: ceil(total / block) CTAs, at least 1, at most `ctas_per_sm` per SM
+inline int grid_for(int64_t total, int block, int ctas_per_sm = 8) {
+  const int64_t g = ceil_div(total, block), cap = (int64_t)sm_count() * ctas_per_sm;
+  return (int)std::max<int64_t>(1, std::min(g, cap));
+}
+
+// ---------------------------------------------------------------------------------------
+// workspaces
+// ---------------------------------------------------------------------------------------
+inline size_t align_up(size_t v, size_t a = 256) { return (v + a - 1) / a * a; }
+
+// Hands out consecutive pieces of a workspace, each starting 256-byte aligned.  With a null base it only measures:
+// `off` after the last piece is the size the workspace needs.
+struct Carver {
+  char* base;
+  size_t off = 0;
+  explicit Carver(void* b) : base(static_cast<char*>(b)) {}
+  char* take(size_t bytes) {
+    char* r = base + off;
+    off = align_up(off + bytes);
+    return r;
+  }
+};
+
+// ---------------------------------------------------------------------------------------
+// PTX: shared-memory addresses, mbarriers, 1-D bulk copy (TMA engine) and their fences
+// ---------------------------------------------------------------------------------------
+__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
+
+__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
+  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
+}
+__device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
+  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
+}
+__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
+  asm volatile(
+      "{\n\t"
+      ".reg .pred P1;\n\t"
+      "LAB_WAIT:\n\t"
+      "mbarrier.try_wait.parity.shared::cta.b64 P1, [%0], %1;\n\t"
+      "@P1 bra DONE;\n\t"
+      "bra LAB_WAIT;\n\t"
+      "DONE:\n\t"
+      "}" ::"r"(smem_u32(bar)),
+      "r"(parity)
+      : "memory");
+}
+// makes initialised mbarriers visible to the other threads and to the async proxy
+__device__ __forceinline__ void fence_mbarrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
+// orders this thread's generic-proxy shared-memory accesses before later async-proxy (bulk copy) ones
+__device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+
+// `bytes` contiguous bytes global -> shared, completing on `bar` (no tensor map needed)
+__device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {
+  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
+                   smem_u32(dst)),
+               "l"(src), "r"(bytes), "r"(smem_u32(bar))
+               : "memory");
+}
 
 // ---------------------------------------------------------------------------------------
 // numerics

@@ -456,8 +456,7 @@ extern "C" int bxs_condinst_head_backward(const float* feat, const float* params
   group_by_image<<<1, 256, (B + 1) * sizeof(int), st>>>(img_inds, (int)N, (int)B, order, start);
 #define BXS_LAUNCH_BWD(CM)                                                                                   \
   do {                                                                                                       \
-    cudaFuncSetAttribute(head_bwd_kernel<CM>, cudaFuncAttributeMaxDynamicSharedMemorySize,                   \
-                         (int)sizeof(SmemBwd<CM>));                                                          \
+    if (opt_in_smem(head_bwd_kernel<CM>, sizeof(SmemBwd<CM>)) != BXS_OK) return BXS_ERR_LAUNCH;              \
     head_bwd_kernel<CM><<<dim3(tiles, (unsigned)B, (unsigned)use_groups), NT, sizeof(SmemBwd<CM>), st>>>(    \
         feat, params, coors, soi, g_out, order, start, gf_target, partial, d, tiles, use_groups);            \
   } while (0)

@@ -75,11 +75,7 @@ extern "C" int bxs_corr_solve(const float* Cu, float* T, int64_t K, int64_t h, i
   const int64_t P = h * w;
   const int64_t smem = (2 * P * P + (1 + kCorrLanes) * P) * 4;
   if (smem > kMaxSmem || K > 65535) return BXS_ERR_UNSUPPORTED;
-  if (smem > 48 * 1024 &&
-      cudaFuncSetAttribute(corr_solve_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) {
-    set_last_error(cudaGetLastError());
-    return BXS_ERR_LAUNCH;
-  }
+  if (smem > 48 * 1024 && opt_in_smem(corr_solve_kernel, smem) != BXS_OK) return BXS_ERR_LAUNCH;
   corr_solve_kernel<<<(unsigned)K, NT_SOLVE, smem, as_stream(stream)>>>(Cu, T, (int)h, (int)w, dist_kernel, num_iter, num_smooth);
   return check_launch();
 }
@@ -97,11 +93,7 @@ extern "C" int bxs_corr_transfer(const float* T, const float* Cu, const float* m
   const int64_t P = h * w, M = Hm * Wm;
   const int64_t smem = (P * P + 2 * P + M + (int64_t)NT_XFER * P) * 4 + (Hm + Wm) * (int64_t)sizeof(CorrTap);
   if (smem > kMaxSmem || K > 65535 || M > (int64_t(1) << 24)) return BXS_ERR_UNSUPPORTED;
-  if (smem > 48 * 1024 &&
-      cudaFuncSetAttribute(corr_transfer_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) {
-    set_last_error(cudaGetLastError());
-    return BXS_ERR_LAUNCH;
-  }
+  if (smem > 48 * 1024 && opt_in_smem(corr_transfer_kernel, smem) != BXS_OK) return BXS_ERR_LAUNCH;
   float* partial = static_cast<float*>(workspace);
   const unsigned gx = (unsigned)ceil_div(M, NT_XFER);
   corr_transfer_kernel<<<dim3(gx, (unsigned)K), NT_XFER, smem, as_stream(stream)>>>(T, Cu, m0, m1, partial, (int)h, (int)w,

@@ -49,31 +49,6 @@ struct SmemLayout {
   uint64_t b_full;
 };
 
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
-__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred P1;\n\t"
-      "LAB_WAIT:\n\t"
-      "mbarrier.try_wait.parity.shared::cta.b64 P1, [%0], %1;\n\t"
-      "@P1 bra DONE;\n\t"
-      "bra LAB_WAIT;\n\t"
-      "DONE:\n\t"
-      "}" ::"r"(smem_u32(bar)),
-      "r"(parity)
-      : "memory");
-}
-
 __device__ __forceinline__ void tma_load_2d(const CUtensorMap* map, uint64_t* bar, void* dst, int x, int y) {
   asm volatile(
       "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];" ::"r"(
@@ -209,7 +184,7 @@ dynconv_tf32_kernel(const __grid_constant__ CUtensorMap tm_feat, const __grid_co
   if (threadIdx.x == 0) {
     for (int s = 0; s < STAGES; ++s) { mbar_init(&S.full[s], 1); mbar_init(&S.empty[s], CONSUMER_WARPS); }
     mbar_init(&S.b_full, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    fence_mbarrier_init();
   }
   __syncthreads();
   if (warp == CONSUMER_WARPS) {
@@ -370,7 +345,7 @@ dynconv_wgrad_kernel(const __grid_constant__ CUtensorMap tm_g, const __grid_cons
   const int kb0 = split * kb_per_split, kb1 = min(kb0 + kb_per_split, kb_total);
   if (threadIdx.x == 0) {
     for (int s = 0; s < WG_STAGES; ++s) { mbar_init(&S.full[s], 1); mbar_init(&S.empty[s], CONSUMER_WARPS); }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    fence_mbarrier_init();
   }
   __syncthreads();
   if (warp == CONSUMER_WARPS) {
@@ -436,7 +411,7 @@ int launch_forward(const CUtensorMap& tm_feat, const CUtensorMap& tm_kern, float
   const int tiles_m = (int)ceil_div(P, BLOCK_M);
   const int per_group = std::min((int)std::max<int64_t>(1, sm_count() / groups), tiles_m);
   const size_t smem = sizeof(SmemLayout) + 1024;
-  cudaFuncSetAttribute(dynconv_tf32_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  if (opt_in_smem(dynconv_tf32_kernel<BN>, smem) != BXS_OK) return BXS_ERR_LAUNCH;
   dynconv_tf32_kernel<BN><<<dim3(per_group, (unsigned)groups), NUM_THREADS, smem, st>>>(tm_feat, tm_kern, out, (int)C,
                                                                                         (int)P, (int)I, n_chunks);
   return check_launch();
@@ -496,7 +471,7 @@ template <int BN>
 int launch_wgrad(const CUtensorMap& tm_g, const CUtensorMap& tm_f, float* partial, int64_t B, int64_t C, int64_t P,
                  int64_t I, int chunks, int splits, int kb_per, cudaStream_t st) {
   const size_t smem = sizeof(WgSmem) + 1024;
-  cudaFuncSetAttribute(dynconv_wgrad_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  if (opt_in_smem(dynconv_wgrad_kernel<BN>, smem) != BXS_OK) return BXS_ERR_LAUNCH;
   dynconv_wgrad_kernel<BN><<<dim3((unsigned)splits, (unsigned)(B * chunks)), NUM_THREADS, smem, st>>>(
       tm_g, tm_f, partial, (int)C, (int)P, (int)I, chunks, splits, kb_per);
   return check_launch();

@@ -382,10 +382,6 @@ lsf_backward_kernel(const float* __restrict__ x, const float* __restrict__ y, co
   }
 }
 
-inline int blocks_for(int64_t total) {
-  return (int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(total, NT), (int64_t)sm_count() * 16));
-}
-
 }  // namespace
 }  // namespace bxs
 
@@ -395,8 +391,8 @@ extern "C" int bxs_bilinear_resize_forward(const float* in, float* out, int64_t 
                                            int align_corners, bxs_stream_t stream) {
   if (!in || !out || NC <= 0 || h <= 0 || w <= 0 || H <= 0 || W <= 0) return BXS_ERR_INVALID_ARG;
   if (h >= (1 << 24) || w >= (1 << 24) || H >= (1 << 24) || W >= (1 << 24)) return BXS_ERR_UNSUPPORTED;
-  resize_fwd_kernel<<<blocks_for(NC * H * W), NT, 0, as_stream(stream)>>>(in, out, NC, (int)h, (int)w, (int)H, (int)W,
-                                                                          align_corners != 0);
+  resize_fwd_kernel<<<grid_for(NC * H * W, NT, 16), NT, 0, as_stream(stream)>>>(in, out, NC, (int)h, (int)w, (int)H, (int)W,
+                                                                                  align_corners != 0);
   return check_launch();
 }
 
@@ -404,8 +400,8 @@ extern "C" int bxs_bilinear_resize_backward(const float* g_out, float* g_in, int
                                             int64_t W, int align_corners, bxs_stream_t stream) {
   if (!g_out || !g_in || NC <= 0 || h <= 0 || w <= 0 || H <= 0 || W <= 0) return BXS_ERR_INVALID_ARG;
   if (h >= (1 << 24) || w >= (1 << 24) || H >= (1 << 24) || W >= (1 << 24)) return BXS_ERR_UNSUPPORTED;
-  resize_bwd_kernel<<<blocks_for(NC * h * w), NT, 0, as_stream(stream)>>>(g_out, g_in, NC, (int)h, (int)w, (int)H, (int)W,
-                                                                          align_corners != 0);
+  resize_bwd_kernel<<<grid_for(NC * h * w, NT, 16), NT, 0, as_stream(stream)>>>(g_out, g_in, NC, (int)h, (int)w, (int)H,
+                                                                                  (int)W, align_corners != 0);
   return check_launch();
 }
 
@@ -415,8 +411,8 @@ extern "C" int bxs_tree_edge_weight_forward(const float* embed, const int32_t* s
   if (!embed || !sorted_index || !sorted_parent || !edge_weight || B <= 0 || groups <= 0 || C <= 0 || V <= 0 ||
       V >= (int64_t(1) << 31) || !(sigma > 0.f))
     return BXS_ERR_INVALID_ARG;
-  edge_weight_fwd_kernel<<<blocks_for(B * groups * V), NT, 0, as_stream(stream)>>>(embed, sorted_index, sorted_parent, edge_weight,
-                                                                                   B * groups, (int)groups, (int)C, (int)V, sigma);
+  edge_weight_fwd_kernel<<<grid_for(B * groups * V, NT, 16), NT, 0, as_stream(stream)>>>(
+      embed, sorted_index, sorted_parent, edge_weight, B * groups, (int)groups, (int)C, (int)V, sigma);
   return check_launch();
 }
 
@@ -427,7 +423,7 @@ extern "C" int bxs_tree_edge_weight_backward(const float* embed, const int32_t* 
   if (!embed || !sorted_index || !sorted_parent || !sorted_child || !edge_weight || !g_weight || !g_embed || B <= 0 ||
       groups <= 0 || C <= 0 || V <= 0 || V >= (int64_t(1) << 31) || !(sigma > 0.f))
     return BXS_ERR_INVALID_ARG;
-  edge_weight_bwd_kernel<<<blocks_for(B * groups * V), NT, 0, as_stream(stream)>>>(
+  edge_weight_bwd_kernel<<<grid_for(B * groups * V, NT, 16), NT, 0, as_stream(stream)>>>(
       embed, sorted_index, sorted_parent, sorted_child, edge_weight, g_weight, g_embed, B * groups, (int)groups, (int)C, (int)V,
       sigma);
   return check_launch();

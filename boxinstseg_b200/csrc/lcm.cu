@@ -220,11 +220,6 @@ __global__ void lcm_scale_kernel(const float* __restrict__ out, const float* __r
   if (threadIdx.x == 0 && blockIdx.x == 0) scale[0] = g_loss[0] * out[1];
 }
 
-inline int grid_for(int64_t total, int block) {
-  const int64_t g = ceil_div(total, block), cap = (int64_t)sm_count() * 8;
-  return (int)std::max<int64_t>(1, std::min(g, cap));
-}
-
 constexpr size_t kMaxFusedSmem = 200 * 1024;
 
 }  // namespace
@@ -259,7 +254,7 @@ extern "C" int bxs_lcm_forward(const float* imgs, const float* phis, const float
   // Unless the instances fill the machine that way, run the iterations as grid-wide kernels (phi ping-pongs through L2; same arithmetic
   // per pixel, same results; the launches are graph-captured by the callers).
   if (sm <= kMaxFusedSmem && n >= 2 * (int64_t)sm_count()) {
-    cudaFuncSetAttribute(lcm_fused_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMaxFusedSmem);
+    if (opt_in_smem(lcm_fused_kernel<0>, kMaxFusedSmem) != BXS_OK) return BXS_ERR_LAUNCH;
     lcm_fused_kernel<0><<<(unsigned)n, NT, sm, st>>>(aff, phis, box, phiT, inst, nullptr, nullptr, (int)h, (int)w,
                                                      dilation, num_iter);
   } else {
@@ -295,7 +290,7 @@ extern "C" int bxs_lcm_backward(const float* phis, const float* box, const void*
   lcm_scale_kernel<<<1, 32, 0, st>>>(out2, g_loss, scale);
   const size_t sm = 2 * hw * sizeof(float);
   if (sm <= kMaxFusedSmem && n >= 2 * (int64_t)sm_count()) {
-    cudaFuncSetAttribute(lcm_fused_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMaxFusedSmem);
+    if (opt_in_smem(lcm_fused_kernel<1>, kMaxFusedSmem) != BXS_OK) return BXS_ERR_LAUNCH;
     lcm_fused_kernel<1><<<(unsigned)n, NT, sm, st>>>(aff, phis, box, phiT, nullptr, scale, g_phis, (int)h, (int)w,
                                                      dilation, num_iter);
   } else {

@@ -158,10 +158,6 @@ __global__ void __launch_bounds__(256) mf_finish_global(const uint8_t* __restric
     valid[n] = ((double)cnt >= (double)hw * 0.05 && (double)cnt <= (double)hw * 0.95) ? 1.f : 0.f;
 }
 
-inline int grid_for(int64_t total, int block) {
-  const int64_t g = ceil_div(total, block), cap = (int64_t)sm_count() * 8;
-  return (int)std::max<int64_t>(1, std::min(g, cap));
-}
 constexpr size_t kMaxFusedSmem = 200 * 1024;
 
 }  // namespace
@@ -208,7 +204,7 @@ extern "C" int bxs_meanfield_forward_inter(const float* K, const int32_t* obj_im
   const bool per_object = sm <= kMaxFusedSmem && (n >= 2 * (int64_t)sm_count() || !workspace);
   if (per_object) {
     auto fused = kernel_size == 3 ? mf_fused_kernel<3> : mf_fused_kernel<0>;
-    cudaFuncSetAttribute(fused, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMaxFusedSmem);
+    if (opt_in_smem(fused, kMaxFusedSmem) != BXS_OK) return BXS_ERR_LAUNCH;
     fused<<<(unsigned)n, NT, sm, st>>>(K, obj_img, x, targets, mc, ret, valid, (int)h, (int)w, kernel_size, num_iter, iiu, gamma);
   } else {
     if (!workspace) return BXS_ERR_INVALID_ARG;

@@ -43,23 +43,19 @@ struct PrjWs {
   size_t total_bytes;
 };
 
-inline size_t align_up(size_t v, size_t a = 256) { return (v + a - 1) / a * a; }
-
 inline PrjWs carve_prj(void* base, int64_t n, int64_t h, int64_t w) {
   PrjWs p{};
-  char* b = (char*)base;
-  size_t off = 0;
-  auto take = [&](size_t bytes) { char* r = b + off; off = align_up(off + bytes); return r; };
-  p.col_s = (unsigned long long*)take(8 * n * w);
-  p.col_t = (unsigned*)take(4 * n * w);
-  p.zero_bytes = off;
-  p.row_s = (unsigned long long*)take(8 * n * h);
-  p.row_t = (float*)take(4 * n * h);
-  p.coef_row = (float*)take(4 * n * h);
-  p.coef_col = (float*)take(4 * n * w);
-  p.arg_row = (int*)take(4 * n * h);
-  p.arg_col = (int*)take(4 * n * w);
-  p.total_bytes = off;
+  Carver c(base);
+  p.col_s = (unsigned long long*)c.take(8 * n * w);
+  p.col_t = (unsigned*)c.take(4 * n * w);
+  p.zero_bytes = c.off;
+  p.row_s = (unsigned long long*)c.take(8 * n * h);
+  p.row_t = (float*)c.take(4 * n * h);
+  p.coef_row = (float*)c.take(4 * n * h);
+  p.coef_col = (float*)c.take(4 * n * w);
+  p.arg_row = (int*)c.take(4 * n * h);
+  p.arg_col = (int*)c.take(4 * n * w);
+  p.total_bytes = c.off;
   return p;
 }
 
@@ -362,7 +358,7 @@ extern "C" int bxs_upsampled_rowcol_max(const float* x, float* row_prof, float* 
   const int rows = (int)ceil_div(H, groups);
   groups = (int)ceil_div(H, rows);
   const size_t sm = (size_t)(NT / 32) * w * sizeof(float);
-  if (sm > 48 * 1024) cudaFuncSetAttribute(upsampled_rowcol_max_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm);
+  if (sm > 48 * 1024 && opt_in_smem(upsampled_rowcol_max_kernel, sm) != BXS_OK) return BXS_ERR_LAUNCH;
   upsampled_rowcol_max_kernel<<<dim3(groups, (unsigned)n), NT, sm, st>>>(x, (int)h, (int)w, (int)H, (int)W, rows,
                                                                          (float)h / (float)H, (float)w / (float)W, row_key,
                                                                          col_key);

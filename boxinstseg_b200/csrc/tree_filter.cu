@@ -41,18 +41,15 @@ struct MstWs {
   int* round_flags;           // [B*64] "this round hooked something"
   size_t total_bytes;
 };
-inline size_t align_up(size_t v, size_t a = 256) { return (v + a - 1) / a * a; }
 inline MstWs carve_mst(void* base, int64_t B, int64_t E, int64_t V) {
   MstWs w{};
-  char* p = (char*)base;
-  size_t off = 0;
-  auto take = [&](size_t bytes) { char* r = p + off; off = align_up(off + bytes); return r; };
-  w.best = (unsigned long long*)take(8 * B * V);
-  w.P = (int*)take(4 * B * V);
-  w.Q = (int*)take(4 * B * V);
-  w.in_tree = (uint8_t*)take(B * E);
-  w.round_flags = (int*)take(4 * B * 64);
-  w.total_bytes = off;
+  Carver c(base);
+  w.best = (unsigned long long*)c.take(8 * B * V);
+  w.P = (int*)c.take(4 * B * V);
+  w.Q = (int*)c.take(4 * B * V);
+  w.in_tree = (uint8_t*)c.take(B * E);
+  w.round_flags = (int*)c.take(4 * B * 64);
+  w.total_bytes = c.off;
   return w;
 }
 
@@ -265,14 +262,12 @@ struct BfsWs {
 };
 inline BfsWs carve_bfs(void* base, int64_t B, int64_t V) {
   BfsWs w{};
-  char* p = (char*)base;
-  size_t off = 0;
-  auto take = [&](size_t bytes) { char* r = p + off; off = align_up(off + bytes); return r; };
-  w.deg = (int*)take(4 * B * V);
-  w.adj = (int*)take(16 * B * V);
-  w.counts = (int*)take(4 * B * V);
-  w.flags = (int*)take(4 * B);
-  w.total_bytes = off;
+  Carver c(base);
+  w.deg = (int*)c.take(4 * B * V);
+  w.adj = (int*)c.take(16 * B * V);
+  w.counts = (int*)c.take(4 * B * V);
+  w.flags = (int*)c.take(4 * B);
+  w.total_bytes = c.off;
   return w;
 }
 
@@ -638,12 +633,11 @@ struct Rec { float4 q; int ia; float fa; };
 
 
 
-__device__ __forceinline__ uint32_t smem_addr(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void cpa4(void* dst, const void* src) {
-  asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(smem_addr(dst)), "l"(src) : "memory");
+  asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(smem_u32(dst)), "l"(src) : "memory");
 }
 __device__ __forceinline__ void cpa16(void* dst, const void* src) {
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_addr(dst)), "l"(src) : "memory");
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_u32(dst)), "l"(src) : "memory");
 }
 __device__ __forceinline__ void cp_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
 template <int N>
@@ -1008,10 +1002,6 @@ __global__ void refine_add_kernel(float* __restrict__ a, const float* __restrict
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) a[i] += b2[i];
 }
 
-inline int grid_for(int64_t total, int block) {
-  const int64_t g = ceil_div(total, block), cap = (int64_t)sm_count() * 8;
-  return (int)std::max<int64_t>(1, std::min(g, cap));
-}
 constexpr size_t kMaxTreeSmem = 220 * 1024;
 // refine kernels: the position-ordered values (dynamic) next to the copy ring + level window (static)
 constexpr size_t kMaxRefineSmem = 227 * 1024 - sizeof(RingSmem) - 64;
@@ -1082,7 +1072,7 @@ extern "C" int bxs_bfs_forward_rooted(const int32_t* tree_edges, int32_t* sorted
   const size_t grid_smem = ((size_t)(V + 3) / 4) * 4 + (size_t)BFS_BUFS * 2 * BFS_STRIDE * sizeof(int);
   const bool try_grid = grid_smem <= kMaxTreeSmem;
   if (try_grid) {
-    cudaFuncSetAttribute(bfs_grid_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMaxTreeSmem);
+    if (opt_in_smem(bfs_grid_kernel, kMaxTreeSmem) != BXS_OK) return BXS_ERR_LAUNCH;
     bfs_grid_kernel<<<(unsigned)B, NT, grid_smem, st>>>(tree_edges, (int)V, sorted_index, sorted_parent, sorted_child,
                                                         level_start, num_levels, flags, (int)root);
   } else {
@@ -1118,15 +1108,13 @@ struct RefineScratch {
 };
 inline RefineScratch carve_refine(void* base, int64_t B, int64_t C, int64_t V) {
   RefineScratch r{};
-  char* p = (char*)base;
-  size_t off = 0;
-  auto take = [&](size_t bytes) { char* q = p + off; off = align_up(off + bytes); return q; };
-  r.cw = (float4*)take(16 * B * V);
-  r.cinfo = (int32_t*)take(4 * B * V);
-  r.outd_par = (float*)take(2 * 4 * B * V);               // per d/d w term
-  r.gw2 = (float*)take(2 * 4 * B * V);                    // the two d/d w terms before they are summed
-  r.bufs = (float*)take(4 * B * (C + 2) * V);
-  r.total_bytes = off;
+  Carver c(base);
+  r.cw = (float4*)c.take(16 * B * V);
+  r.cinfo = (int32_t*)c.take(4 * B * V);
+  r.outd_par = (float*)c.take(2 * 4 * B * V);             // per d/d w term
+  r.gw2 = (float*)c.take(2 * 4 * B * V);                  // the two d/d w terms before they are summed
+  r.bufs = (float*)c.take(4 * B * (C + 2) * V);
+  r.total_bytes = c.off;
   return r;
 }
 inline void pack_tree(const float* w, const int32_t* chd, const RefineScratch& rs, int64_t B, int64_t V, cudaStream_t st) {
@@ -1157,7 +1145,7 @@ extern "C" int bxs_refine_forward_grouped(const float* feature, const float* edg
   pack_tree(edge_weight, sorted_child, rs, G, V, st);
   const size_t sm = (V + 4) * sizeof(float);
   if (sm <= kMaxRefineSmem) {
-    cudaFuncSetAttribute(refine_updown_kernel<0, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMaxRefineSmem);
+    if (opt_in_smem(refine_updown_kernel<0, true>, kMaxRefineSmem) != BXS_OK) return BXS_ERR_LAUNCH;
     refine_updown_kernel<0, true><<<dim3((unsigned)(n + G), (unsigned)C), RNT, sm, st>>>(
         feature, edge_weight, sorted_index, sorted_parent, rs.cinfo, rs.cw, level_start, num_levels, nullptr, aggr, aggr_up,
         wsum, wsum_up, nullptr, (int)C, (int)V, tree_of, (int)n);
@@ -1186,7 +1174,7 @@ extern "C" int bxs_refine_backward_feature_grouped(const float* edge_weight, con
   const size_t sm = (V + 4) * sizeof(float);
   const dim3 grid((unsigned)n, (unsigned)C);
   if (sm <= kMaxRefineSmem) {
-    cudaFuncSetAttribute(refine_updown_kernel<1, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMaxRefineSmem);
+    if (opt_in_smem(refine_updown_kernel<1, true>, kMaxRefineSmem) != BXS_OK) return BXS_ERR_LAUNCH;
     refine_updown_kernel<1, true><<<grid, RNT, sm, st>>>(grad_out, edge_weight, sorted_index, sorted_parent, rs.cinfo, rs.cw,
                                                         level_start, num_levels, wsum, grad_feature, nullptr, nullptr,
                                                         nullptr, nullptr, (int)C, (int)V, tree_of, (int)n);
@@ -1215,7 +1203,7 @@ extern "C" int bxs_refine_backward_weight_grouped(const float* edge_weight, cons
   pack_tree(edge_weight, sorted_child, rs, G, V, st);
   const size_t sm = (V + 4) * sizeof(float);
   if (sm <= kMaxRefineSmem) {
-    cudaFuncSetAttribute(refine_bwd_weight_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMaxRefineSmem);
+    if (opt_in_smem(refine_bwd_weight_kernel<true>, kMaxRefineSmem) != BXS_OK) return BXS_ERR_LAUNCH;
     refine_bwd_weight_kernel<true><<<dim3((unsigned)n, 2), RNT, sm, st>>>(edge_weight, sorted_index, sorted_parent, rs.cinfo,
                                                                          rs.cw, level_start, num_levels, feature_out, aggr,
                                                                          aggr_up, wsum, wsum_up, grad_out, rs.gw2, nullptr,
