@@ -23,12 +23,8 @@ SIGNATURES = {
     'bxs_version': [],
     'bxs_last_error': [],
     'bxs_device_sm_count': [],
-    'bxs_flush_l2': [c_p, c_i64, c_p],
     'bxs_pairwise_nlog_forward': [c_p, c_p, c_i64, c_i64, c_i64, c_int, c_int, c_int, c_p],
     'bxs_pairwise_nlog_backward': [c_p, c_p, c_p, c_i64, c_i64, c_i64, c_int, c_int, c_int, c_p],
-    'bxs_boxinst_lab': [c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_i64, c_i64, c_i64, c_int, c_p],
-    'bxs_boxinst_similarity': [c_p, c_p, c_p, c_p, c_i64, c_i64, c_i64, c_int, c_int, c_f, c_p],
-    'bxs_boxinst_rects': [c_p, c_p, c_i64, c_i64, c_i64, c_int, c_p],
     'bxs_boxinst_bitmasks': [c_p, c_p, c_i64, c_i64, c_i64, c_p],
     'bxs_boxinst_targets_forward': [c_p] * 13 + [c_i64] * 3 + [c_int] * 3 + [c_f, c_p],
     'bxs_rgb_u8_to_lab': [c_p, c_p, c_i64, c_p],
@@ -61,7 +57,6 @@ SIGNATURES = {
     'bxs_mst_forward': [c_p] * 4 + [c_i64] * 3 + [c_p],
     'bxs_bfs_workspace_bytes': [c_i64] * 2,
     'bxs_bfs_forward_rooted': [c_p] * 7 + [c_i64] * 2 + [c_int, c_i64, c_p],
-    'bxs_tree_levels': [c_p] * 4 + [c_i64] * 2 + [c_p],
     'bxs_refine_scratch_bytes': [c_i64] * 3,
     'bxs_refine_forward_grouped': [c_p] * 14 + [c_i64] * 4 + [c_p],
     'bxs_refine_backward_feature_grouped': [c_p] * 11 + [c_i64] * 4 + [c_p],

@@ -6,10 +6,6 @@
 namespace bxs {
 namespace {
 thread_local char g_err[256] = "";
-__global__ void fill_kernel(uint4* p, int64_t n, unsigned v) {
-  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
-    p[i] = make_uint4(v, v, v, v);
-}
 }  // namespace
 
 void set_last_error(cudaError_t e) {
@@ -38,11 +34,4 @@ extern "C" int bxs_device_sm_count(void) {
   int n = 0;
   if (cudaGetDeviceCount(&n) != cudaSuccess || n == 0) return BXS_ERR_NO_DEVICE;
   return bxs::sm_count();
-}
-
-extern "C" int bxs_flush_l2(void* scratch, int64_t bytes, bxs_stream_t stream) {
-  if (!scratch || bytes < 16) return BXS_ERR_INVALID_ARG;
-  static unsigned tick = 0;
-  bxs::fill_kernel<<<bxs::sm_count() * 8, 256, 0, bxs::as_stream(stream)>>>((uint4*)scratch, bytes / 16, ++tick);
-  return bxs::check_launch();
 }

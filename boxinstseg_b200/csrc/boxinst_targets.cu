@@ -79,21 +79,9 @@ __device__ __forceinline__ void lab_pixel(const float* __restrict__ img, const N
   valid[(int64_t)b * plane_sz + o] = (sy < ih - removed && sx < iw) ? 1 : 0;
 }
 
-__global__ void lab_kernel(const float* __restrict__ img, const int32_t* __restrict__ img_hw,
-                           const int32_t* __restrict__ removed_rows, Norm nm, float* __restrict__ lab,
-                           uint8_t* __restrict__ valid, int B, int Hp, int Wp, int s) {
-  const int H = Hp / s, W = Wp / s;
-  const int64_t total = (int64_t)B * H * W;
-  for (int64_t idx = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; idx < total;
-       idx += (int64_t)gridDim.x * blockDim.x) {
-    const int i = idx % W, j = (idx / W) % H, b = idx / ((int64_t)W * H);
-    lab_pixel(img, nm, img_hw[2 * b], img_hw[2 * b + 1], removed_rows[b], lab, valid, b, j, i, H, W, Hp, Wp, s);
-  }
-}
-
-// The per-image metadata of a batch travels BY VALUE in the kernel parameters (no host-to-device copy, nothing to keep
-// alive, capturable in a CUDA graph): image sizes, removed bottom rows, and the running GT count (gt_end[b] = number of
-// GT boxes of images 0..b).
+// The per-image metadata of up to kMaxMetaImages images travels BY VALUE in the kernel parameters (no host-to-device
+// copy, nothing to keep alive, capturable in a CUDA graph): image sizes, removed bottom rows, and the running GT count
+// (gt_end[b] = number of GT boxes of images 0..b).  Larger batches take one launch per chunk of that many images.
 constexpr int kMaxMetaImages = 64;
 struct TargetsMeta {
   int ih[kMaxMetaImages], iw[kMaxMetaImages], removed[kMaxMetaImages], gt_end[kMaxMetaImages];
@@ -101,10 +89,12 @@ struct TargetsMeta {
 };
 
 // lab + validity of every stride-s pixel; the tail of the grid also turns the GT boxes into grid rectangles and writes
-// the image index of every GT (get_bitmasks_from_boxes' per-image loop, condinst_head.py:1417-1448)
+// the image index of every GT (get_bitmasks_from_boxes' per-image loop, condinst_head.py:1417-1448).  All pointers and
+// counts are those of one chunk of images; b0, the chunk's first image, makes gt_img a batch-wide image index.
 __global__ void lab_rects_kernel(const float* __restrict__ img, const float* __restrict__ boxes,
                                  const __grid_constant__ TargetsMeta meta, float* __restrict__ lab, uint8_t* __restrict__ valid,
-                                 int32_t* __restrict__ rects, int32_t* __restrict__ gt_img, int B, int G, int Hp, int Wp, int s) {
+                                 int32_t* __restrict__ rects, int32_t* __restrict__ gt_img, int B, int b0, int G, int Hp, int Wp,
+                                 int s) {
   const int H = Hp / s, W = Wp / s;
   const int64_t total = (int64_t)B * H * W;
   const int64_t tid0 = blockIdx.x * (int64_t)blockDim.x + threadIdx.x, nth = (int64_t)gridDim.x * blockDim.x;
@@ -120,7 +110,7 @@ __global__ void lab_rects_kernel(const float* __restrict__ img, const float* __r
     *reinterpret_cast<int4*>(rects + 4 * g) = make_int4(j0, j1, i0, i1);
     int b = 0;
     while (b < B - 1 && g >= meta.gt_end[b]) ++b;
-    gt_img[g] = b;
+    gt_img[g] = b0 + b;
   }
 }
 
@@ -155,17 +145,6 @@ __global__ void similarity_kernel(const float* __restrict__ lab, const uint8_t* 
   }
 }
 
-__global__ void rects_kernel(const float* __restrict__ boxes, int32_t* __restrict__ rects, int G, int Hp, int Wp,
-                             int s) {
-  const int g = blockIdx.x * blockDim.x + threadIdx.x;
-  if (g >= G) return;
-  const float x1 = boxes[4 * g], y1 = boxes[4 * g + 1], x2 = boxes[4 * g + 2], y2 = boxes[4 * g + 3];
-  int j0, j1, i0, i1;
-  slice_range(y1, y2, Hp, s, j0, j1);
-  slice_range(x1, x2, Wp, s, i0, i1);
-  rects[4 * g + 0] = j0; rects[4 * g + 1] = j1; rects[4 * g + 2] = i0; rects[4 * g + 3] = i1;
-}
-
 __global__ void bitmask_kernel(const int32_t* __restrict__ rects, float* __restrict__ out, int64_t G, int H, int W) {
   const int64_t total = G * H * W;
   for (int64_t idx = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; idx < total;
@@ -182,39 +161,6 @@ __global__ void bitmask_kernel(const int32_t* __restrict__ rects, float* __restr
 
 using namespace bxs;
 
-extern "C" int bxs_boxinst_lab(const float* img, const int32_t* img_hw, const int32_t* removed_rows,
-                               const float* mean3_host, const float* std3_host, float* lab, uint8_t* valid,
-                               int64_t B, int64_t Hp, int64_t Wp, int stride, bxs_stream_t stream) {
-  if (!img || !img_hw || !removed_rows || !mean3_host || !std3_host || !lab || !valid || B <= 0 || Hp <= 0 ||
-      Wp <= 0 || stride <= 0 || stride > 256 || Hp % stride || Wp % stride)
-    return BXS_ERR_INVALID_ARG;
-  Norm nm;
-  for (int c = 0; c < 3; ++c) { nm.mean[c] = mean3_host[c]; nm.std[c] = std3_host[c]; }
-  const int64_t total = B * (Hp / stride) * (Wp / stride);
-  lab_kernel<<<grid_for(total, 128), 128, 0, as_stream(stream)>>>(img, img_hw, removed_rows, nm, lab, valid, (int)B,
-                                                                  (int)Hp, (int)Wp, stride);
-  return check_launch();
-}
-
-extern "C" int bxs_boxinst_similarity(const float* lab, const uint8_t* valid, float* sim, uint8_t* edge_bits,
-                                      int64_t B, int64_t H, int64_t W, int size, int dilation, float thresh,
-                                      bxs_stream_t stream) {
-  if (!lab || !valid || (!sim && !edge_bits) || B <= 0 || H <= 0 || W <= 0 || size < 3 || !(size & 1) ||
-      dilation < 1 || (edge_bits && size != 3))
-    return BXS_ERR_INVALID_ARG;
-  similarity_kernel<<<grid_for(B * H * W, 128), 128, 0, as_stream(stream)>>>(lab, valid, sim, edge_bits, (int)B, (int)H,
-                                                                             (int)W, size, dilation, thresh);
-  return check_launch();
-}
-
-extern "C" int bxs_boxinst_rects(const float* boxes, int32_t* rects, int64_t G, int64_t Hp, int64_t Wp, int stride,
-                                 bxs_stream_t stream) {
-  if (G == 0) return BXS_OK;
-  if (!boxes || !rects || G < 0 || Hp <= 0 || Wp <= 0 || stride <= 0) return BXS_ERR_INVALID_ARG;
-  rects_kernel<<<(unsigned)ceil_div(G, 128), 128, 0, as_stream(stream)>>>(boxes, rects, (int)G, (int)Hp, (int)Wp, stride);
-  return check_launch();
-}
-
 extern "C" int bxs_boxinst_bitmasks(const int32_t* rects, float* bitmasks, int64_t G, int64_t H, int64_t W,
                                     bxs_stream_t stream) {
   if (G == 0) return BXS_OK;
@@ -225,9 +171,9 @@ extern "C" int bxs_boxinst_bitmasks(const int32_t* rects, float* bitmasks, int64
 
 
 // ---------------------------------------------------------------------------------------
-// Whole target build of a batch in two launches, metadata by value (<= 64 images): LAB + validity + grid rectangles +
-// GT image index, then the colour similarity / edge bits.  Same results as bxs_boxinst_lab + bxs_boxinst_similarity +
-// bxs_boxinst_rects; no host-to-device copies, capturable in a CUDA graph.
+// Whole target build of a batch: LAB + validity + grid rectangles + GT image index, one launch per kMaxMetaImages
+// images with the metadata by value, then the colour similarity / edge bits in one launch.  No host-to-device copies,
+// capturable in a CUDA graph.
 // ---------------------------------------------------------------------------------------
 extern "C" int bxs_boxinst_targets_forward(const float* img, const float* boxes, const int32_t* img_hw_host,
                                            const int32_t* removed_rows_host, const int32_t* num_gts_host,
@@ -239,28 +185,36 @@ extern "C" int bxs_boxinst_targets_forward(const float* img, const float* boxes,
       (!sim && !edge_bits) || B <= 0 || Hp <= 0 || Wp <= 0 || stride <= 0 || stride > 256 || Hp % stride || Wp % stride ||
       size < 3 || !(size & 1) || dilation < 1 || (edge_bits && size != 3))
     return BXS_ERR_INVALID_ARG;
-  if (B > kMaxMetaImages) return BXS_ERR_UNSUPPORTED;
-  TargetsMeta meta;
   int64_t G = 0;
-  for (int b = 0; b < kMaxMetaImages; ++b) {
-    const bool in = b < B;
-    if (in && num_gts_host[b] < 0) return BXS_ERR_INVALID_ARG;
-    if (in) G += num_gts_host[b];
-    meta.ih[b] = in ? img_hw_host[2 * b] : 0;
-    meta.iw[b] = in ? img_hw_host[2 * b + 1] : 0;
-    meta.removed[b] = in ? removed_rows_host[b] : 0;
-    meta.gt_end[b] = (int)G;
+  for (int64_t b = 0; b < B; ++b) {
+    if (num_gts_host[b] < 0) return BXS_ERR_INVALID_ARG;
+    G += num_gts_host[b];
   }
   if (G > 0 && (!boxes || !rects || !gt_img)) return BXS_ERR_INVALID_ARG;
+  TargetsMeta meta;
   for (int c = 0; c < 3; ++c) { meta.nm.mean[c] = mean3_host[c]; meta.nm.std[c] = std3_host[c]; }
-  const int64_t H = Hp / stride, W = Wp / stride, total = B * H * W;
+  const int64_t H = Hp / stride, W = Wp / stride;
   cudaStream_t st = as_stream(stream);
-  lab_rects_kernel<<<(unsigned)std::max<int64_t>(ceil_div(total, 128), ceil_div(std::min<int64_t>(G, total), 128)), 128, 0, st>>>(
-      img, boxes, meta, lab, valid, rects, gt_img, (int)B, (int)G, (int)Hp, (int)Wp, stride);
-  int rc = check_launch();
-  if (rc != BXS_OK) return rc;
-  similarity_kernel<<<grid_for(total, 128), 128, 0, st>>>(lab, valid, sim, edge_bits, (int)B, (int)H, (int)W, size, dilation,
-                                                           thresh);
+  for (int64_t b0 = 0, g0 = 0; b0 < B; b0 += kMaxMetaImages) {
+    const int64_t nb = std::min<int64_t>(B - b0, kMaxMetaImages), total = nb * H * W;
+    int64_t gc = 0;
+    for (int b = 0; b < kMaxMetaImages; ++b) {
+      const bool in = b < nb;
+      if (in) gc += num_gts_host[b0 + b];
+      meta.ih[b] = in ? img_hw_host[2 * (b0 + b)] : 0;
+      meta.iw[b] = in ? img_hw_host[2 * (b0 + b) + 1] : 0;
+      meta.removed[b] = in ? removed_rows_host[b0 + b] : 0;
+      meta.gt_end[b] = (int)gc;
+    }
+    lab_rects_kernel<<<(unsigned)std::max<int64_t>(ceil_div(total, 128), ceil_div(std::min<int64_t>(gc, total), 128)), 128, 0,
+                       st>>>(img + b0 * 3 * Hp * Wp, boxes + 4 * g0, meta, lab + b0 * 3 * H * W, valid + b0 * H * W,
+                             rects + 4 * g0, gt_img + g0, (int)nb, (int)b0, (int)gc, (int)Hp, (int)Wp, stride);
+    const int rc = check_launch();
+    if (rc != BXS_OK) return rc;
+    g0 += gc;
+  }
+  similarity_kernel<<<grid_for(B * H * W, 128), 128, 0, st>>>(lab, valid, sim, edge_bits, (int)B, (int)H, (int)W, size,
+                                                               dilation, thresh);
   return check_launch();
 }
 

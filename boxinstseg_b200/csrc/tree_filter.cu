@@ -570,37 +570,6 @@ __global__ void __launch_bounds__(NT) bfs_grid_kernel(const int32_t* __restrict_
   }
 }
 
-// level boundaries from (level-contiguous) sorted_parent when they were not produced by bfs_block_kernel:
-// depth by pointer doubling, one CTA per tree, scratch in global memory
-__global__ void __launch_bounds__(NT) levels_from_parent_kernel(const int32_t* __restrict__ sorted_parent, int V,
-                                                                int* __restrict__ scratch,
-                                                                int32_t* __restrict__ level_start,
-                                                                int32_t* __restrict__ num_levels) {
-  const int b = blockIdx.x;
-  const int32_t* par = sorted_parent + (int64_t)b * V;
-  int* anc0 = scratch + (int64_t)b * 4 * V;
-  int* dep0 = anc0 + V;
-  int* anc1 = dep0 + V;
-  int* dep1 = anc1 + V;
-  int32_t* lvl = level_start + (int64_t)b * (V + 1);
-  for (int p = threadIdx.x; p < V; p += NT) { anc0[p] = p == 0 ? 0 : par[p]; dep0[p] = p == 0 ? 0 : 1; }
-  __syncthreads();
-  for (int step = 1; step < V; step <<= 1) {
-    for (int p = threadIdx.x; p < V; p += NT) {
-      const int a = anc0[p];
-      anc1[p] = anc0[a];
-      dep1[p] = dep0[p] + dep0[a];
-    }
-    __syncthreads();
-    int* t = anc0; anc0 = anc1; anc1 = t;
-    t = dep0; dep0 = dep1; dep1 = t;
-  }
-  for (int p = threadIdx.x; p < V; p += NT)
-    if (p == 0 || dep0[p] != dep0[p - 1]) lvl[dep0[p]] = p;
-  __syncthreads();
-  if (threadIdx.x == 0) { const int L = dep0[V - 1] + 1; lvl[L] = V; num_levels[b] = L; }
-}
-
 // ---------------------------------------------------------------------------------------
 // tree aggregation
 // ---------------------------------------------------------------------------------------
@@ -1050,8 +1019,7 @@ extern "C" int64_t bxs_bfs_workspace_bytes(int64_t B, int64_t V) {
   return (B <= 0 || V <= 0) ? 0 : (int64_t)carve_bfs(nullptr, B, V).total_bytes + 256;
 }
 
-// level_start [B, V+1] and num_levels [B] are extra outputs (may be NULL -> scratch inside the workspace is NOT
-// provided: pass real buffers whenever the result feeds bxs_refine_*).
+// level_start [B, V+1] and num_levels [B] are required outputs: the level table bxs_refine_* runs on.
 // The reference roots every tree at vertex 0 (bfs.cu:100-135); here the caller picks the root: the tree filter's result
 // does not depend on it, but the number of dependent levels of every pass does (a 200x256 image MST is ~1900 levels deep
 // from the corner, about half of that from the centre).
@@ -1084,14 +1052,6 @@ extern "C" int bxs_bfs_forward_rooted(const int32_t* tree_edges, int32_t* sorted
   bfs_sort_adj_kernel<<<grid_for(B * V, 256), 256, 0, st>>>(ws, B * V, (int)V, flags);
   bfs_block_kernel<<<(unsigned)B, NT, 0, st>>>(ws, (int)V, sorted_index, sorted_parent, sorted_child, level_start,
                                                num_levels, flags, (int)root);
-  return check_launch();
-}
-
-extern "C" int bxs_tree_levels(const int32_t* sorted_parent, int32_t* level_start, int32_t* num_levels, void* scratch,
-                               int64_t B, int64_t V, bxs_stream_t stream) {
-  if (!sorted_parent || !level_start || !num_levels || !scratch || B <= 0 || V <= 0) return BXS_ERR_INVALID_ARG;
-  levels_from_parent_kernel<<<(unsigned)B, NT, 0, as_stream(stream)>>>(sorted_parent, (int)V, (int*)scratch, level_start,
-                                                                       num_levels);
   return check_launch();
 }
 

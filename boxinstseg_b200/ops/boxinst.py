@@ -83,26 +83,14 @@ def boxinst_targets(img, img_metas, gt_bboxes, stride=4, pairwise_size=3, pairwi
     boxes = (torch.cat([b.reshape(-1, 4) for b in gt_bboxes]) if G else torch.zeros((0, 4), device=dev)).to(
         device=dev, dtype=torch.float32).contiguous()
     rects = torch.empty((G, 4), dtype=torch.int32, device=dev)
-    lib = L.lib()
+    gt_img = torch.empty(G, dtype=torch.int32, device=dev)
+    ng = np.asarray(num_gts, dtype=np.int32)
     with torch.cuda.device(dev):
-        if B <= 64:
-            # metadata by value: two launches, no host-to-device copies, capturable
-            gt_img = torch.empty(G, dtype=torch.int32, device=dev)
-            ng = np.asarray(num_gts, dtype=np.int32)
-            L.check(lib.bxs_boxinst_targets_forward(
-                L.ptr(img), L.ptr(boxes), hw.ctypes.data, removed.ctypes.data, ng.ctypes.data, mean.ctypes.data,
-                std.ctypes.data, L.ptr(lab), L.ptr(valid), L.ptr(sim), L.ptr(bits), L.ptr(rects), L.ptr(gt_img), B, Hp, Wp,
-                stride, pairwise_size, pairwise_dilation, float(pairwise_color_thresh), L.stream()), 'boxinst_targets')
-        else:
-            meta_dev = torch.from_numpy(np.concatenate([hw.reshape(-1), removed])).to(dev, non_blocking=True)
-            hw_dev, removed_dev = meta_dev[:2 * B], meta_dev[2 * B:]
-            L.check(lib.bxs_boxinst_lab(L.ptr(img), L.ptr(hw_dev), L.ptr(removed_dev), mean.ctypes.data, std.ctypes.data,
-                                        L.ptr(lab), L.ptr(valid), B, Hp, Wp, stride, L.stream()), 'boxinst_lab')
-            L.check(lib.bxs_boxinst_similarity(L.ptr(lab), L.ptr(valid), L.ptr(sim), L.ptr(bits), B, H, W, pairwise_size,
-                                               pairwise_dilation, float(pairwise_color_thresh), L.stream()),
-                    'boxinst_similarity')
-            L.check(lib.bxs_boxinst_rects(L.ptr(boxes), L.ptr(rects), G, Hp, Wp, stride, L.stream()), 'boxinst_rects')
-            gt_img = torch.from_numpy(np.repeat(np.arange(B, dtype=np.int32), num_gts)).to(dev, non_blocking=True)
+        # metadata by value: no host-to-device copies, capturable
+        L.check(L.lib().bxs_boxinst_targets_forward(
+            L.ptr(img), L.ptr(boxes), hw.ctypes.data, removed.ctypes.data, ng.ctypes.data, mean.ctypes.data,
+            std.ctypes.data, L.ptr(lab), L.ptr(valid), L.ptr(sim), L.ptr(bits), L.ptr(rects), L.ptr(gt_img), B, Hp, Wp,
+            stride, pairwise_size, pairwise_dilation, float(pairwise_color_thresh), L.stream()), 'boxinst_targets')
     return BoxInstTargets(bits, sim, rects, gt_img, num_gts, lab, valid)
 
 

@@ -33,7 +33,6 @@ typedef enum {
 int bxs_version(void);                       /* 10000*major + 100*minor + patch */
 const char* bxs_last_error(void);            /* text of the last CUDA error seen by this thread */
 int bxs_device_sm_count(void);               /* multiprocessor count of the current device */
-int bxs_flush_l2(void* scratch, int64_t bytes, bxs_stream_t stream); /* bench helper: overwrite scratch */
 
 /* ---------------------------------------------------------------------------------------
  * a7  pairwise -log P(same label)            replaces pairwise_ext.pairwise_nlog_forward /
@@ -54,34 +53,23 @@ int bxs_pairwise_nlog_backward(const void* logits, const void* g_out, void* g_lo
  *     (mmdet/models/dense_heads/condinst_head.py:170-246, 1345-1448) incl. the host round trips
  *     through mmcv.tensor2imgs and skimage.color.rgb2lab.
  *
- * bxs_boxinst_lab: img [B,3,Hp,Wp] normalised RGB -> lab [B,3,Hp/s,Wp/s] (float32) and
- *   valid [B,Hp/s,Wp/s] (uint8).  img_hw [B,2] int32 = (img_h, img_w) of each image,
- *   removed_rows [B] int32 = int(bottom_pixels_removed*img_h/ori_h) (host integers),
- *   mean/std: 3 floats each (host pointers, read at call time).
- * bxs_boxinst_similarity: lab, valid -> sim [B,k*k-1,H,W] float32 (may be NULL) and, for
- *   size==3, edge_bits [B,H,W] uint8 with bit c = (sim[c] >= thresh) (may be NULL).
- * bxs_boxinst_rects: boxes [G,4] float xyxy -> rects [G,4] int32 (j0,j1,i0,i1 inclusive grid
- *   ranges of the centre-sampled bitmask; empty when j0>j1 or i0>i1); Python slice semantics
- *   of condinst_head.py:1429-1432 are kept.
+ * bxs_boxinst_targets_forward: the whole target build of a batch.  img [B,3,Hp,Wp] normalised RGB ->
+ *   lab [B,3,H,W] float32 and valid [B,H,W] uint8 (H = Hp/s, W = Wp/s);
+ *   sim [B,k*k-1,H,W] float32 (may be NULL) and, for size==3, edge_bits [B,H,W] uint8 with
+ *   bit c = (sim[c] >= thresh) (may be NULL; not both);
+ *   boxes [G,4] float xyxy (device, image-major, G = sum num_gts) -> rects [G,4] int32 (j0,j1,i0,i1
+ *   inclusive grid ranges of the centre-sampled bitmask; empty when j0>j1 or i0>i1; Python slice
+ *   semantics of condinst_head.py:1429-1432) and gt_img [G] int32, the image of each GT
+ *   (boxes / rects / gt_img may be NULL when G == 0).
+ *   Host arrays, read at call time: img_hw_host [B,2] = (img_h, img_w) of img_shape,
+ *   removed_rows_host [B] = int(bottom_pixels_removed*img_h/ori_h), num_gts_host [B], mean/std:
+ *   3 floats each.  The per-image metadata is passed BY VALUE in the kernel parameters: no
+ *   host-to-device copies, capturable in a CUDA graph.  Two launches for up to 64 images, one
+ *   more per further 64.
  * bxs_boxinst_bitmasks: rects -> dense bitmasks [G,H,W] float32 (API parity only).
  * --------------------------------------------------------------------------------------- */
-int bxs_boxinst_lab(const float* img, const int32_t* img_hw, const int32_t* removed_rows,
-                    const float* mean3_host, const float* std3_host, float* lab, uint8_t* valid,
-                    int64_t B, int64_t Hp, int64_t Wp, int stride, bxs_stream_t stream);
-int bxs_boxinst_similarity(const float* lab, const uint8_t* valid, float* sim, uint8_t* edge_bits,
-                           int64_t B, int64_t H, int64_t W, int size, int dilation, float thresh,
-                           bxs_stream_t stream);
-int bxs_boxinst_rects(const float* boxes, int32_t* rects, int64_t G, int64_t Hp, int64_t Wp,
-                      int stride, bxs_stream_t stream);
 int bxs_boxinst_bitmasks(const int32_t* rects, float* bitmasks, int64_t G, int64_t H, int64_t W,
                          bxs_stream_t stream);
-
-/* The whole target build of a batch (bxs_boxinst_lab + bxs_boxinst_rects + the GT -> image index + bxs_boxinst_similarity) in
- * two launches, with the per-image metadata passed BY VALUE from host arrays (img_hw_host [B,2] = (h, w) of img_shape,
- * removed_rows_host [B], num_gts_host [B]; B <= 64, else BXS_ERR_UNSUPPORTED): no host-to-device copies, capturable in a CUDA
- * graph.  boxes [sum num_gts, 4] xyxy (device, image-major), rects [G,4] / gt_img [G] outputs (may be NULL when G == 0);
- * sim / edge_bits as in bxs_boxinst_similarity.  Replaces CondInstMaskHead.get_targets' host round trip
- * (condinst_head.py:170-246, 1345-1448). */
 int bxs_boxinst_targets_forward(const float* img, const float* boxes, const int32_t* img_hw_host,
                                 const int32_t* removed_rows_host, const int32_t* num_gts_host, const float* mean3_host,
                                 const float* std3_host, float* lab, uint8_t* valid, float* sim, uint8_t* edge_bits,
@@ -258,7 +246,6 @@ int bxs_meanfield_forward_inter(const float* K, const int32_t* obj_img, const fl
  *   them, plus level_start [B,V+1] / num_levels [B]: the order is level-contiguous and deterministic.  The tree is
  *   rooted at vertex `root` (the reference: always vertex 0).  The filter's result does not depend on the root; the
  *   number of dependent levels of every pass does: about half from the centre of the map.
- * bxs_tree_levels: recovers level_start / num_levels from a level-contiguous sorted_parent (scratch 16*B*V bytes).
  * bxs_refine_forward_grouped: feature f32 [n,C,V] (vertex order), edge_weight f32 [G,V] (sorted order; entry 0 is
  *   ignored = 0 and NOT overwritten, unlike refine.cu:43-46) -> feature_out, aggr [n,C,V], aggr_up [n,C,V],
  *   wsum [G,V], wsum_up [G,V] (the five tensors of refine.cu:201-249).
@@ -278,8 +265,6 @@ int64_t bxs_bfs_workspace_bytes(int64_t B, int64_t V);
 int bxs_bfs_forward_rooted(const int32_t* tree_edges, int32_t* sorted_index, int32_t* sorted_parent,
                     int32_t* sorted_child, int32_t* level_start, int32_t* num_levels, void* workspace,
                     int64_t B, int64_t V, int max_adj, int64_t root, bxs_stream_t stream);
-int bxs_tree_levels(const int32_t* sorted_parent, int32_t* level_start, int32_t* num_levels, void* scratch,
-                    int64_t B, int64_t V, bxs_stream_t stream);
 int64_t bxs_refine_scratch_bytes(int64_t B, int64_t C, int64_t V);
 int bxs_refine_forward_grouped(const float* feature, const float* edge_weight, const int32_t* sorted_index,
                                const int32_t* sorted_parent, const int32_t* sorted_child,

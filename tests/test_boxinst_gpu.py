@@ -100,52 +100,50 @@ def test_targets_vs_oracle(dev, ragged):
     assert mism == 0
 
 
-def test_targets_by_value_call_equals_separate_kernels(dev):
-    """bxs_boxinst_targets_forward (metadata by value, two launches) against the four separate entry points it fuses,
-    including images without GT boxes and a batch that ends with one."""
+def test_targets_forward_empty_images_and_chunks(dev):
+    """bxs_boxinst_targets_forward with images without GT boxes, including a batch that ends with one, against the
+    oracle; and a batch of more images than one launch carries the metadata of (64) against the same call on its two
+    halves, with images without GT boxes on both sides of the chunk boundary."""
     from boxinstseg_b200 import _lib as L
+    from oracle.boxinst import boxinst_targets as oracle_targets
     case = boxinst_case(5, B=4, hp=64, wp=96, gts_per_img=3, inst_per_gt=1, ragged=True)
     case['gt_bboxes'][1] = case['gt_bboxes'][1][:0]
     case['gt_bboxes'][3] = case['gt_bboxes'][3][:0]
     t = _targets(case, dev)
+    sim, bms = oracle_targets(case['img'], case['metas'], case['gt_bboxes'])
+    for got, want in zip(t.bitmasks(), bms):
+        assert torch.equal(got.cpu(), want)
+    assert torch.allclose(t.similarity.cpu(), sim, rtol=1e-5, atol=1e-7)
+    assert torch.equal(t.edge_bits.cpu(), sum(((sim[:, c] >= 0.3).to(torch.uint8) << c) for c in range(8)))
+    assert t.gt_img.cpu().tolist() == np.repeat(np.arange(4), [len(b) for b in case['gt_bboxes']]).tolist()
+
+    big = boxinst_case(6, B=70, hp=32, wp=48, gts_per_img=3, inst_per_gt=1, ragged=True)
+    num_gts = [0 if b in (3, 62, 63, 64, 66, 69) else b % 4 for b in range(70)]
+    big['gt_bboxes'] = [boxes[:n] for boxes, n in zip(big['gt_bboxes'], num_gts)]
+    whole = _targets(big, dev)
+    halves = [_targets(dict(img=big['img'][s], metas=big['metas'][s], gt_bboxes=big['gt_bboxes'][s]), dev)
+              for s in (slice(0, 64), slice(64, 70))]
+    for name in ('lab', 'valid', 'similarity', 'edge_bits', 'rects'):
+        assert torch.equal(getattr(whole, name), torch.cat([getattr(h, name) for h in halves])), name
+    assert whole.gt_img.cpu().tolist() == np.repeat(np.arange(70), num_gts).tolist()
+
+    # argument errors of the C entry point
     img = case['img'].to(dev).contiguous()
     B, _, Hp, Wp = img.shape
-    H, W = Hp // 4, Wp // 4
-    hw = torch.tensor([m['img_shape'][:2] for m in case['metas']], dtype=torch.int32)
-    rem = torch.tensor([int(10 * float(m['img_shape'][0]) / float(m['ori_shape'][0])) for m in case['metas']], dtype=torch.int32)
-    cfg = case['metas'][0]['img_norm_cfg']
-    mean = np.ascontiguousarray(np.asarray(cfg['mean'], np.float32))
-    std = np.ascontiguousarray(np.asarray(cfg['std'], np.float32))
-    lab = torch.empty(B, 3, H, W, device=dev)
-    valid = torch.empty(B, H, W, dtype=torch.uint8, device=dev)
-    sim = torch.empty(B, 8, H, W, device=dev)
-    bits = torch.empty(B, H, W, dtype=torch.uint8, device=dev)
-    lib = L.lib()
-    hw_d, rem_d = hw.to(dev), rem.to(dev)
-    assert lib.bxs_boxinst_lab(L.ptr(img), L.ptr(hw_d), L.ptr(rem_d), mean.ctypes.data, std.ctypes.data, L.ptr(lab),
-                               L.ptr(valid), B, Hp, Wp, 4, L.stream()) == 0
-    assert lib.bxs_boxinst_similarity(L.ptr(lab), L.ptr(valid), L.ptr(sim), L.ptr(bits), B, H, W, 3, 2, 0.3, L.stream()) == 0
     boxes = torch.cat(case['gt_bboxes']).float().to(dev).contiguous()
-    G = boxes.shape[0]
-    rects = torch.empty(G, 4, dtype=torch.int32, device=dev)
-    assert lib.bxs_boxinst_rects(L.ptr(boxes), L.ptr(rects), G, Hp, Wp, 4, L.stream()) == 0
-    torch.cuda.synchronize()
-    assert torch.equal(t.lab, lab) and torch.equal(t.valid, valid)
-    assert torch.equal(t.similarity, sim) and torch.equal(t.edge_bits, bits)
-    assert torch.equal(t.rects, rects)
-    want_img = np.repeat(np.arange(B), [b.shape[0] for b in case['gt_bboxes']])
-    assert t.gt_img.cpu().tolist() == want_img.tolist()
-    # argument errors of the C entry point
-    ng = np.asarray([b.shape[0] for b in case['gt_bboxes']], np.int32)
-    hw_h, rem_h = hw.numpy(), rem.numpy()
-    gi = torch.empty(G, dtype=torch.int32, device=dev)
+    ng = np.asarray([len(b) for b in case['gt_bboxes']], np.int32)
+    hw = np.asarray([m['img_shape'][:2] for m in case['metas']], np.int32)
+    rem = np.asarray([int(10 * float(m['img_shape'][0]) / float(m['ori_shape'][0])) for m in case['metas']], np.int32)
+    mean = np.ascontiguousarray(np.asarray(case['metas'][0]['img_norm_cfg']['mean'], np.float32))
+    std = np.ascontiguousarray(np.asarray(case['metas'][0]['img_norm_cfg']['std'], np.float32))
+    lib = L.lib()
 
-    def call(Bx, ngx=ng, lab_=lab):
-        return lib.bxs_boxinst_targets_forward(L.ptr(img), L.ptr(boxes), hw_h.ctypes.data, rem_h.ctypes.data, ngx.ctypes.data,
-                                               mean.ctypes.data, std.ctypes.data, L.ptr(lab_), L.ptr(valid), L.ptr(sim),
-                                               L.ptr(bits), L.ptr(rects), L.ptr(gi), Bx, Hp, Wp, 4, 3, 2, 0.3, L.stream())
+    def call(Bx, ngx=ng, lab_=t.lab):
+        return lib.bxs_boxinst_targets_forward(L.ptr(img), L.ptr(boxes), hw.ctypes.data, rem.ctypes.data, ngx.ctypes.data,
+                                               mean.ctypes.data, std.ctypes.data, L.ptr(lab_), L.ptr(t.valid),
+                                               L.ptr(t.similarity), L.ptr(t.edge_bits), L.ptr(t.rects), L.ptr(t.gt_img), Bx,
+                                               Hp, Wp, 4, 3, 2, 0.3, L.stream())
     assert call(B) == 0
-    assert call(65) == -3                                           # more images than the by-value metadata holds
     assert call(B, lab_=None) == -1
     assert call(B, ngx=np.asarray([1, -1, 0, 0], np.int32)) == -1
 
