@@ -64,6 +64,9 @@ SIGNATURES = {
     'bxs_dynconv1x1_forward': [c_p] * 3 + [c_i64] * 4 + [c_p],
     'bxs_dynconv1x1_backward_workspace_bytes': [c_i64] * 4,
     'bxs_dynconv1x1_backward': [c_p] * 6 + [c_i64] * 4 + [c_p],
+    'bxs_dynconv1x1_half_forward': [c_p] * 3 + [c_i64] * 4 + [c_int, c_p],
+    'bxs_dynconv1x1_half_backward_workspace_bytes': [c_i64] * 4 + [c_int],
+    'bxs_dynconv1x1_half_backward': [c_p] * 6 + [c_i64] * 4 + [c_int, c_p],
     'bxs_upsampled_rowcol_max': [c_p] * 4 + [c_i64] * 5 + [c_int, c_p],
     'bxs_bilinear_resize_forward': [c_p, c_p] + [c_i64] * 5 + [c_int, c_p],
     'bxs_bilinear_resize_backward': [c_p, c_p] + [c_i64] * 5 + [c_int, c_p],
@@ -80,7 +83,8 @@ SIGNATURES = {
 _RESTYPE = {'bxs_mst_workspace_bytes': c_i64, 'bxs_bfs_workspace_bytes': c_i64, 'bxs_refine_scratch_bytes': c_i64, 'bxs_lcm_workspace_bytes': c_i64, 'bxs_meanfield_workspace_bytes': c_i64, 'bxs_projection_workspace_bytes': c_i64,'bxs_condinst_head_workspace_bytes': c_i64, 'bxs_last_error': ctypes.c_char_p, 'bxs_boxinst_loss_workspace_bytes': c_i64,
              'bxs_boxinst_loss_fused_workspace_bytes': c_i64, 'bxs_boxinst_loss_fused_sched_bytes': c_i64,
              'bxs_boxinst_loss_plan_bytes': c_i64, 'bxs_levelset_fused_workspace_bytes': c_i64,
-             'bxs_dynconv1x1_backward_workspace_bytes': c_i64, 'bxs_corr_transfer_workspace_bytes': c_i64}
+             'bxs_dynconv1x1_backward_workspace_bytes': c_i64, 'bxs_corr_transfer_workspace_bytes': c_i64,
+             'bxs_dynconv1x1_half_backward_workspace_bytes': c_i64}
 
 _STATUS = {-1: 'invalid argument', -2: 'kernel launch failed', -3: 'unsupported shape', -4: 'no CUDA device'}
 

@@ -21,8 +21,11 @@
 //   warp 8   : TMA producer (B once, then a ring of 16 KB A stages)
 // synchronised with mbarriers only (full/empty per stage).
 #include <cuda.h>
+#include <cuda_bf16.h>
+#include <cuda_fp16.h>
 
 #include <algorithm>
+#include <type_traits>
 
 #include "common.cuh"
 
@@ -460,10 +463,10 @@ extern "C" int bxs_dynconv1x1_forward(const float* feat, const float* kernels, f
 // workspace: bxs_dynconv1x1_backward_workspace_bytes(B, C, P, I) bytes.
 // ---------------------------------------------------------------------------------------
 namespace {
-inline int wg_splits(int64_t B, int64_t P, int64_t I) {
-  const int64_t chunks = ceil_div(I, 128), kb_total = ceil_div(P, BLOCK_K);
+inline int wg_splits(int64_t B, int64_t P, int64_t I, int block_k = BLOCK_K) {
+  const int64_t chunks = ceil_div(I, 128), kb_total = ceil_div(P, block_k);
   int64_t s = std::max<int64_t>(1, (2 * (int64_t)sm_count()) / (B * chunks));
-  s = std::min<int64_t>(s, std::max<int64_t>(1, kb_total / 8));          // at least 8 k-blocks (256 pixels) per CTA
+  s = std::min<int64_t>(s, std::max<int64_t>(1, kb_total / (256 / block_k)));   // at least 256 pixels per CTA
   return (int)s;
 }
 
@@ -524,4 +527,474 @@ extern "C" int bxs_dynconv1x1_backward(const float* feat, const float* kernels, 
     if (rc != BXS_OK) return rc;
   }
   return BXS_OK;
+}
+
+
+// =====================================================================================================================
+// 16-bit operands (FP16 or BF16, chosen at compile time), FP32 accumulation in registers: the same three products for
+// callers that run in mixed precision (the reference's DiscoBox configs train under autocast), at half the bytes.
+//   forward / d/d feat: A = feat^T goes from TMA straight to a shared-memory descriptor.  wgmma transposes 16-bit
+//       operands itself (imm-trans-a), so A is read MN-major: [64 channels][64 pixels] boxes with the 128-byte swizzle
+//       are the canonical MN-major SW128 layout (64 pixels = 128 bytes per channel row, 8-row groups 1 KB apart).
+//       B = kernels, K-major [BN rows][64 channels] boxes, resident for the CTA's lifetime (<= 64 KB).  Each consumer
+//       warpgroup rounds its 64 pixels x BN kernels to the operand dtype into a [kernel][64 pixels] shared-memory tile
+//       and writes it out in 16-byte pieces, so every output row segment is whole 32-byte sectors.
+//   d/d kernel: both operands K-major over the pixels (64 per stage); split-K with FP32 partials, reduced in split
+//       order (deterministic) and rounded to the operand dtype only there.
+// =====================================================================================================================
+namespace bxs {
+namespace {
+
+constexpr int H_BLOCK_K = 64;                                // channels (or pixels) per stage: one 128-byte swizzle row
+constexpr int H_MMA_K = 16;
+constexpr int H_MAX_KBLOCKS = 4;                             // C <= 256
+constexpr int H_STAGES = 6;                                  // 96 KB of feat in flight per SM
+constexpr int H_BOX_BYTES = 64 * H_BLOCK_K * 2;              // [64 channels][64 pixels]: one warpgroup's A, 8 KB
+constexpr int H_A_STAGE_BYTES = BLOCK_M * H_BLOCK_K * 2;     // 16 KB
+constexpr int H_B_KBLOCK_BYTES = MAX_N * H_BLOCK_K * 2;      // 16 KB
+constexpr int H_OUT_BYTES = MAX_N * 64 * 2;                  // [BN <= 128 kernels][64 pixels] of one warpgroup
+
+struct HSmem {
+  alignas(1024) uint8_t a[H_STAGES][H_A_STAGE_BYTES];
+  alignas(1024) uint8_t b[H_MAX_KBLOCKS][H_B_KBLOCK_BYTES];
+  alignas(16) uint8_t out[2][H_OUT_BYTES];
+  alignas(8) uint64_t full[H_STAGES];
+  uint64_t empty[H_STAGES];
+  uint64_t b_full;
+};
+
+template <typename T>
+struct Half16;
+template <>
+struct Half16<__half> {
+  static constexpr CUtensorMapDataType tma = CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
+  static __device__ __forceinline__ __half round(float x) { return __float2half_rn(x); }
+};
+template <>
+struct Half16<__nv_bfloat16> {
+  static constexpr CUtensorMapDataType tma = CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
+  static __device__ __forceinline__ __nv_bfloat16 round(float x) { return __float2bfloat16_rn(x); }
+};
+
+// D[64 x 32] += A[64 x 16] * B[32 x 16]^T, both in shared memory, F16 in, FP32 accumulate; TA = 1: A is MN-major
+template <int TA>
+__device__ __forceinline__ void wgmma_f16_n32(float (&d)[16], uint64_t adesc, uint64_t bdesc) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %18, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, %19, 0;\n}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(adesc), "l"(bdesc), "r"(1), "n"(TA));
+}
+// D[64 x 64] += A[64 x 16] * B[64 x 16]^T, both in shared memory, F16 in, FP32 accumulate; TA = 1: A is MN-major
+template <int TA>
+__device__ __forceinline__ void wgmma_f16_n64(float (&d)[32], uint64_t adesc, uint64_t bdesc) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, %35, 0;\n}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(adesc), "l"(bdesc), "r"(1), "n"(TA));
+}
+// D[64 x 128] += A[64 x 16] * B[128 x 16]^T, both in shared memory, F16 in, FP32 accumulate; TA = 1: A is MN-major
+template <int TA>
+__device__ __forceinline__ void wgmma_f16_n128(float (&d)[64], uint64_t adesc, uint64_t bdesc) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, %67, 0;\n}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(adesc), "l"(bdesc), "r"(1), "n"(TA));
+}
+// D[64 x 256] += A[64 x 16] * B[256 x 16]^T, both in shared memory, F16 in, FP32 accumulate; TA = 1: A is MN-major
+template <int TA>
+__device__ __forceinline__ void wgmma_f16_n256(float (&d)[128], uint64_t adesc, uint64_t bdesc) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %130, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n256k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, %128, %129, p, 1, 1, %131, 0;\n}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]), "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]), "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]), "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]), "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+      : "l"(adesc), "l"(bdesc), "r"(1), "n"(TA));
+}
+// D[64 x 32] += A[64 x 16] * B[32 x 16]^T, both in shared memory, BF16 in, FP32 accumulate; TA = 1: A is MN-major
+template <int TA>
+__device__ __forceinline__ void wgmma_bf16_n32(float (&d)[16], uint64_t adesc, uint64_t bdesc) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %18, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, %19, 0;\n}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(adesc), "l"(bdesc), "r"(1), "n"(TA));
+}
+// D[64 x 64] += A[64 x 16] * B[64 x 16]^T, both in shared memory, BF16 in, FP32 accumulate; TA = 1: A is MN-major
+template <int TA>
+__device__ __forceinline__ void wgmma_bf16_n64(float (&d)[32], uint64_t adesc, uint64_t bdesc) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, %35, 0;\n}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(adesc), "l"(bdesc), "r"(1), "n"(TA));
+}
+// D[64 x 128] += A[64 x 16] * B[128 x 16]^T, both in shared memory, BF16 in, FP32 accumulate; TA = 1: A is MN-major
+template <int TA>
+__device__ __forceinline__ void wgmma_bf16_n128(float (&d)[64], uint64_t adesc, uint64_t bdesc) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, %67, 0;\n}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(adesc), "l"(bdesc), "r"(1), "n"(TA));
+}
+// D[64 x 256] += A[64 x 16] * B[256 x 16]^T, both in shared memory, BF16 in, FP32 accumulate; TA = 1: A is MN-major
+template <int TA>
+__device__ __forceinline__ void wgmma_bf16_n256(float (&d)[128], uint64_t adesc, uint64_t bdesc) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %130, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, %128, %129, p, 1, 1, %131, 0;\n}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]), "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]), "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]), "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]), "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+      : "l"(adesc), "l"(bdesc), "r"(1), "n"(TA));
+}
+
+template <typename T, int BN, int TA>
+__device__ __forceinline__ void wgmma16(float (&d)[BN / 2], uint64_t adesc, uint64_t bdesc) {
+  if constexpr (std::is_same_v<T, __half>) {
+    if constexpr (BN == 32) wgmma_f16_n32<TA>(d, adesc, bdesc);
+    else if constexpr (BN == 64) wgmma_f16_n64<TA>(d, adesc, bdesc);
+    else if constexpr (BN == 128) wgmma_f16_n128<TA>(d, adesc, bdesc);
+    else wgmma_f16_n256<TA>(d, adesc, bdesc);
+  } else {
+    if constexpr (BN == 32) wgmma_bf16_n32<TA>(d, adesc, bdesc);
+    else if constexpr (BN == 64) wgmma_bf16_n64<TA>(d, adesc, bdesc);
+    else if constexpr (BN == 128) wgmma_bf16_n128<TA>(d, adesc, bdesc);
+    else wgmma_bf16_n256<TA>(d, adesc, bdesc);
+  }
+}
+
+// wgmma shared-memory descriptor of an MN-major operand with the 128-byte swizzle (PTX ISA, canonical layouts of the
+// matrix descriptor): the layout is ((64 MN elements, m), (8 K rows, k)) with the MN index contiguous, a K row every
+// 128 bytes, SBO = the stride between groups of 8 K rows (1 KB here) and LBO = the stride between 64-element MN blocks.
+// An m64 A operand spans a single MN block, so LBO is never stepped; it is set to the 8 KB box pitch.  The k-th step of
+// 16 K rows starts 2 KB further, a whole number of swizzle atoms.
+__device__ __forceinline__ uint64_t make_desc_mn(uint32_t saddr) {
+  return (uint64_t)((saddr >> 4) & 0x3fff) | ((uint64_t)(H_BOX_BYTES >> 4) << 16) | ((uint64_t)(1024 >> 4) << 32) |
+         ((uint64_t)1 << 62);
+}
+
+// named barrier 1 + wg over the 128 threads of consumer warpgroup wg
+__device__ __forceinline__ void warpgroup_bar(int wg) {
+  if (wg == 0) asm volatile("bar.sync 1, 128;" ::: "memory");
+  else asm volatile("bar.sync 2, 128;" ::: "memory");
+}
+
+// the output tile of a warpgroup: row n (kernel) of 64 pixels = 128 bytes, its 16-byte chunks XOR-swizzled by n % 8 so
+// that the accumulator scatter (8 pixels x 4 kernels per warp instruction) and the row read-out are free of conflicts
+__device__ __forceinline__ int out_off(int n, int p) { return n * 128 + ((((p >> 3) ^ (n & 7))) << 4) + (p & 7) * 2; }
+
+// grid: (ctas_per_group, B * n_chunks), as dynconv_tf32_kernel
+template <typename T, int BN>
+__global__ void __launch_bounds__(NUM_THREADS, 1)
+dynconv_h_kernel(const __grid_constant__ CUtensorMap tm_feat, const __grid_constant__ CUtensorMap tm_kern,
+                 T* __restrict__ out, int C, int P, int I, int n_chunks) {
+  extern __shared__ uint8_t smem_raw[];
+  HSmem& S = *reinterpret_cast<HSmem*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int b = blockIdx.y / n_chunks, chunk = blockIdx.y % n_chunks;
+  const int kblocks = (C + H_BLOCK_K - 1) / H_BLOCK_K;   // channels beyond C are zero-filled by the 3-D tensor map
+  const int tiles_m = (P + BLOCK_M - 1) / BLOCK_M;
+
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < H_STAGES; ++s) { mbar_init(&S.full[s], 1); mbar_init(&S.empty[s], CONSUMER_WARPS); }
+    mbar_init(&S.b_full, 1);
+    fence_mbarrier_init();
+  }
+  __syncthreads();
+  if (warp == CONSUMER_WARPS) {
+    // ===================== TMA producer =====================
+    if (lane == 0) {
+      mbar_expect_tx(&S.b_full, (uint32_t)kblocks * BN * H_BLOCK_K * 2);
+      for (int kb = 0; kb < kblocks; ++kb)
+        tma_load_3d(&tm_kern, &S.b_full, S.b[kb], kb * H_BLOCK_K, b * I + chunk * BN, 0);
+      int stage = 0, phase = 0;
+      for (int mt = blockIdx.x; mt < tiles_m; mt += gridDim.x) {
+        for (int kb = 0; kb < kblocks; ++kb) {
+          mbar_wait(&S.empty[stage], phase ^ 1);
+          mbar_expect_tx(&S.full[stage], H_A_STAGE_BYTES);
+#pragma unroll
+          for (int g = 0; g < BLOCK_M / 64; ++g)
+            tma_load_3d(&tm_feat, &S.full[stage], S.a[stage] + g * H_BOX_BYTES, mt * BLOCK_M + g * 64, kb * H_BLOCK_K, b);
+          if (++stage == H_STAGES) { stage = 0; phase ^= 1; }
+        }
+      }
+    }
+  } else {
+    // ===================== consumers: wgmma (A MN-major, B K-major) -> shared tile -> global =====================
+    const int wg = warp >> 2, w = warp & 3, r = lane >> 2, c4 = lane & 3, t = threadIdx.x & 127;
+    uint8_t* tile = S.out[wg];
+    mbar_wait(&S.b_full, 0);
+    int stage = 0, phase = 0;
+    for (int mt = blockIdx.x; mt < tiles_m; mt += gridDim.x) {
+      float acc[BN / 2];
+#pragma unroll
+      for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+      for (int kb = 0; kb < kblocks; ++kb) {
+        mbar_wait(&S.full[stage], phase);
+        const uint32_t a_base = smem_u32(S.a[stage] + wg * H_BOX_BYTES), b_base = smem_u32(S.b[kb]);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < H_BLOCK_K / H_MMA_K; ++k)
+          wgmma16<T, BN, 1>(acc, make_desc_mn(a_base + k * (H_MMA_K * 128)), make_desc(b_base + k * (H_MMA_K * 2)));
+        wgmma_commit();
+        wgmma_wait_all();
+        fence_acc(acc);
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&S.empty[stage]);
+        if (++stage == H_STAGES) { stage = 0; phase ^= 1; }
+      }
+      // accumulator elements 4 j .. 4 j + 3: kernels n = 8 j + 2 c4 + {0, 1} of pixels 16 w + r and 16 w + r + 8
+      warpgroup_bar(wg);                       // the previous tile has been read out of `tile`
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j) {
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          const int n = 8 * j + 2 * c4 + (e & 1), p = 16 * w + r + ((e & 2) ? 8 : 0);
+          *reinterpret_cast<T*>(tile + out_off(n, p)) = Half16<T>::round(acc[4 * j + e]);
+        }
+      }
+      warpgroup_bar(wg);
+      const int pix = mt * BLOCK_M + wg * 64;
+#pragma unroll
+      for (int q = 0; q < BN / 16; ++q) {          // BN rows x 8 pieces of 16 bytes, 128 threads
+        const int n = 16 * q + (t >> 3), ch = t & 7, i = chunk * BN + n, p = pix + ch * 8;
+        if (i < I && p < P)
+          *reinterpret_cast<uint4*>(out + ((int64_t)b * I + i) * P + p) = *reinterpret_cast<const uint4*>(tile + out_off(n, ch * 8));
+      }
+    }
+  }
+}
+
+// kT[b, c, i] = kernels[b, i, c] for i < I, 0 for I <= i < Ipad; the bits are moved as they are (+0 is 0 in both dtypes)
+__global__ void transpose_pad_h_kernel(const uint16_t* __restrict__ k, uint16_t* __restrict__ kt, int I, int C, int Ipad,
+                                       int64_t total) {
+  for (int64_t idx = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; idx < total; idx += (int64_t)gridDim.x * blockDim.x) {
+    const int i = (int)(idx % Ipad);
+    const int c = (int)((idx / Ipad) % C);
+    const int64_t b = idx / ((int64_t)Ipad * C);
+    kt[idx] = i < I ? __ldg(k + (b * I + i) * C + c) : (uint16_t)0;
+  }
+}
+
+// d/d kernel, 16-bit operands: dynconv_wgrad_kernel with 64-pixel stages (A = g: 128 rows x 64 pixels, B = feat:
+// C rows x 64 pixels, both K-major; 4 stages of 48 KB)
+constexpr int HW_STAGES = 4;
+constexpr int HW_A_BYTES = 128 * H_BLOCK_K * 2;    // 16 KB
+constexpr int HW_B_BYTES = 256 * H_BLOCK_K * 2;    // 32 KB
+
+struct HWgSmem {
+  alignas(1024) uint8_t a[HW_STAGES][HW_A_BYTES];
+  alignas(1024) uint8_t b[HW_STAGES][HW_B_BYTES];
+  alignas(8) uint64_t full[HW_STAGES];
+  uint64_t empty[HW_STAGES];
+};
+
+template <typename T, int BN>
+__global__ void __launch_bounds__(NUM_THREADS, 1)
+dynconv_h_wgrad_kernel(const __grid_constant__ CUtensorMap tm_g, const __grid_constant__ CUtensorMap tm_feat,
+                       float* __restrict__ partial, int C, int P, int I, int chunks, int splits, int kb_per_split) {
+  extern __shared__ uint8_t smem_raw[];
+  HWgSmem& S = *reinterpret_cast<HWgSmem*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int split = blockIdx.x, b = blockIdx.y / chunks, chunk = blockIdx.y % chunks;
+  const int kb_total = (P + H_BLOCK_K - 1) / H_BLOCK_K;
+  const int kb0 = split * kb_per_split, kb1 = min(kb0 + kb_per_split, kb_total);
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < HW_STAGES; ++s) { mbar_init(&S.full[s], 1); mbar_init(&S.empty[s], CONSUMER_WARPS); }
+    fence_mbarrier_init();
+  }
+  __syncthreads();
+  if (warp == CONSUMER_WARPS) {
+    if (lane == 0) {
+      int stage = 0, phase = 0;
+      for (int kb = kb0; kb < kb1; ++kb) {
+        mbar_wait(&S.empty[stage], phase ^ 1);
+        mbar_expect_tx(&S.full[stage], HW_A_BYTES + (uint32_t)C * H_BLOCK_K * 2);
+        tma_load_3d(&tm_g, &S.full[stage], S.a[stage], kb * H_BLOCK_K, chunk * 128, b);     // rows >= I: zeros
+        tma_load_3d(&tm_feat, &S.full[stage], S.b[stage], kb * H_BLOCK_K, 0, b);
+        if (++stage == HW_STAGES) { stage = 0; phase ^= 1; }
+      }
+    }
+  } else {
+    const int wg = warp >> 2, w = warp & 3, r = lane >> 2, c4 = lane & 3;
+    float acc[BN / 2];
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+    int stage = 0, phase = 0;
+    for (int kb = kb0; kb < kb1; ++kb) {
+      mbar_wait(&S.full[stage], phase);
+      const uint32_t a_base = smem_u32(S.a[stage]) + wg * (64 * 128), b_base = smem_u32(S.b[stage]);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < H_BLOCK_K / H_MMA_K; ++k)
+        wgmma16<T, BN, 0>(acc, make_desc(a_base + k * (H_MMA_K * 2)), make_desc(b_base + k * (H_MMA_K * 2)));
+      wgmma_commit();
+      wgmma_wait_all();
+      fence_acc(acc);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&S.empty[stage]);
+      if (++stage == HW_STAGES) { stage = 0; phase ^= 1; }
+    }
+    // accumulator elements (i, i + 1), i even: row 16 w + r (+ 8 when i % 4 == 2), columns 8 (i / 4) + 2 c4 + {0, 1}
+    const int row0 = chunk * 128 + wg * 64 + w * 16 + r;
+    float* dst = partial + (((int64_t)b * splits + split) * I) * C;
+#pragma unroll
+    for (int i = 0; i < BN / 2; i += 2) {
+      const int row = row0 + ((i & 2) ? 8 : 0), n = 8 * (i >> 2) + 2 * c4;
+      if (row < I && n < C) *reinterpret_cast<float2*>(dst + (int64_t)row * C + n) = make_float2(acc[i], acc[i + 1]);
+    }
+  }
+}
+
+template <typename T>
+__global__ void dynconv_h_wgrad_reduce(const float* __restrict__ partial, T* __restrict__ out, int splits,
+                                       int64_t per_image, int64_t total) {
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t b = i / per_image, r = i - b * per_image;
+    const float* p = partial + b * splits * per_image + r;
+    float acc = 0.f;
+    for (int s = 0; s < splits; ++s) acc += p[(int64_t)s * per_image];          // split order: deterministic
+    out[i] = Half16<T>::round(acc);
+  }
+}
+
+// [batch, rows, cols] 16-bit tensor, box = [1, box_rows, 64 elements], 128-byte swizzle, zero fill out of bounds.  A
+// 2-D [rows, cols] matrix is the batch == 1 case.
+bool make_map3_h(CUtensorMap* map, CUtensorMapDataType dt, const void* base, int64_t batch, int64_t rows, int64_t cols,
+                 int box_rows) {
+  EncodeTiledFn fn = encode_fn();
+  if (!fn) return false;
+  cuuint64_t dims[3] = {(cuuint64_t)cols, (cuuint64_t)rows, (cuuint64_t)batch};
+  cuuint64_t strides[2] = {(cuuint64_t)cols * 2, (cuuint64_t)cols * (cuuint64_t)rows * 2};
+  cuuint32_t box[3] = {H_BLOCK_K, (cuuint32_t)box_rows, 1};
+  cuuint32_t estr[3] = {1, 1, 1};
+  return fn(map, dt, 3, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+            CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+}
+
+template <typename T, int BN>
+int launch_forward_h(const CUtensorMap& tm_feat, const CUtensorMap& tm_kern, T* out, int64_t B, int64_t C, int64_t P,
+                     int64_t I, cudaStream_t st) {
+  const int n_chunks = (int)ceil_div(I, BN);
+  const int64_t groups = B * n_chunks;
+  if (groups > 65535) return BXS_ERR_UNSUPPORTED;
+  const int tiles_m = (int)ceil_div(P, BLOCK_M);
+  const int per_group = std::min((int)std::max<int64_t>(1, sm_count() / groups), tiles_m);
+  const size_t smem = sizeof(HSmem) + 1024;
+  if (opt_in_smem(dynconv_h_kernel<T, BN>, smem) != BXS_OK) return BXS_ERR_LAUNCH;
+  dynconv_h_kernel<T, BN><<<dim3(per_group, (unsigned)groups), NUM_THREADS, smem, st>>>(tm_feat, tm_kern, out, (int)C,
+                                                                                       (int)P, (int)I, n_chunks);
+  return check_launch();
+}
+
+// out[b, i, p] = sum_c kern[b, i, c] * feat3[b, c, p] for c < C; rows c >= feat_rows of feat3 read as zeros
+template <typename T>
+int dynconv_forward_h(const T* feat3, int64_t feat_rows, const T* kern, T* out, int64_t B, int64_t C, int64_t P,
+                      int64_t I, cudaStream_t st) {
+  const int bn = forward_bn(I);
+  CUtensorMap tm_feat, tm_kern;
+  if (!make_map3_h(&tm_feat, Half16<T>::tma, feat3, B, feat_rows, P, H_BLOCK_K) ||
+      !make_map3_h(&tm_kern, Half16<T>::tma, kern, 1, B * I, C, bn)) {
+    set_last_error(cudaErrorNotSupported);
+    return BXS_ERR_LAUNCH;
+  }
+  if (bn == 32) return launch_forward_h<T, 32>(tm_feat, tm_kern, out, B, C, P, I, st);
+  if (bn == 64) return launch_forward_h<T, 64>(tm_feat, tm_kern, out, B, C, P, I, st);
+  return launch_forward_h<T, 128>(tm_feat, tm_kern, out, B, C, P, I, st);
+}
+
+template <typename T, int BN>
+int launch_wgrad_h(const CUtensorMap& tm_g, const CUtensorMap& tm_f, float* partial, int64_t B, int64_t C, int64_t P,
+                   int64_t I, int chunks, int splits, int kb_per, cudaStream_t st) {
+  const size_t smem = sizeof(HWgSmem) + 1024;
+  if (opt_in_smem(dynconv_h_wgrad_kernel<T, BN>, smem) != BXS_OK) return BXS_ERR_LAUNCH;
+  dynconv_h_wgrad_kernel<T, BN><<<dim3((unsigned)splits, (unsigned)(B * chunks)), NUM_THREADS, smem, st>>>(
+      tm_g, tm_f, partial, (int)C, (int)P, (int)I, chunks, splits, kb_per);
+  return check_launch();
+}
+
+template <typename T>
+int dynconv_backward_h(const T* feat, const T* kernels, const T* g_out, T* g_feat, T* g_kernels, void* workspace,
+                       int64_t B, int64_t C, int64_t P, int64_t I, cudaStream_t st) {
+  const int64_t ipad = ceil_div(I, 32) * 32;
+  T* kt = reinterpret_cast<T*>((reinterpret_cast<uintptr_t>(workspace) + 1023) & ~uintptr_t(1023));
+  float* partial = reinterpret_cast<float*>((reinterpret_cast<uintptr_t>(kt + B * C * ipad) + 1023) & ~uintptr_t(1023));
+  if (g_feat) {
+    const int64_t total = B * C * ipad;
+    transpose_pad_h_kernel<<<(unsigned)std::min<int64_t>(ceil_div(total, 256), 1024), 256, 0, st>>>(
+        reinterpret_cast<const uint16_t*>(kernels), reinterpret_cast<uint16_t*>(kt), (int)I, (int)C, (int)ipad, total);
+    // out[b, c, p] = sum_i kT[b, c, i] * g[b, i, p]: "C" := I (zero-filled up to the k-block), "I" := C
+    int rc = dynconv_forward_h<T>(g_out, I, kt, g_feat, B, ipad, P, C, st);
+    if (rc != BXS_OK) return rc;
+  }
+  if (g_kernels) {
+    const int chunks = (int)ceil_div(I, 128), splits = wg_splits(B, P, I, H_BLOCK_K);
+    const int kb_total = (int)ceil_div(P, H_BLOCK_K), kb_per = (int)ceil_div(kb_total, splits);
+    CUtensorMap tm_g, tm_f;
+    if (!make_map3_h(&tm_g, Half16<T>::tma, g_out, B, I, P, 128) || !make_map3_h(&tm_f, Half16<T>::tma, feat, B, C, P, (int)C)) {
+      set_last_error(cudaErrorNotSupported);
+      return BXS_ERR_LAUNCH;
+    }
+    int rc = C <= 32    ? launch_wgrad_h<T, 32>(tm_g, tm_f, partial, B, C, P, I, chunks, splits, kb_per, st)
+             : C <= 64  ? launch_wgrad_h<T, 64>(tm_g, tm_f, partial, B, C, P, I, chunks, splits, kb_per, st)
+             : C <= 128 ? launch_wgrad_h<T, 128>(tm_g, tm_f, partial, B, C, P, I, chunks, splits, kb_per, st)
+                        : launch_wgrad_h<T, 256>(tm_g, tm_f, partial, B, C, P, I, chunks, splits, kb_per, st);
+    if (rc != BXS_OK) return rc;
+    const int64_t total = B * I * C;
+    dynconv_h_wgrad_reduce<T><<<(unsigned)std::min<int64_t>(ceil_div(total, 256), 1024), 256, 0, st>>>(
+        partial, g_kernels, splits, I * C, total);
+    rc = check_launch();
+    if (rc != BXS_OK) return rc;
+  }
+  return BXS_OK;
+}
+
+inline bool misaligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) != 0; }
+inline bool known_half(int dtype) { return dtype == BXS_F16 || dtype == BXS_BF16; }
+// the envelope of the 16-bit kernels: TMA needs 16-byte row strides (P % 8) and bases; the output tile is written in
+// 16-byte pieces
+inline bool half_shape_ok(int64_t B, int64_t C, int64_t P, int64_t I) {
+  return C % 32 == 0 && C <= H_BLOCK_K * H_MAX_KBLOCKS && P % 8 == 0 && B * C < (int64_t(1) << 31) &&
+         B * I < (int64_t(1) << 31);
+}
+}  // namespace
+}  // namespace bxs
+
+extern "C" int bxs_dynconv1x1_half_forward(const void* feat, const void* kernels, void* out, int64_t B, int64_t C,
+                                           int64_t P, int64_t I, int dtype, bxs_stream_t stream) {
+  if (!feat || !kernels || !out || B <= 0 || C <= 0 || P <= 0 || I <= 0 || !known_half(dtype)) return BXS_ERR_INVALID_ARG;
+  if (!half_shape_ok(B, C, P, I) || misaligned16(feat) || misaligned16(kernels) || misaligned16(out))
+    return BXS_ERR_UNSUPPORTED;
+  cudaStream_t st = as_stream(stream);
+  if (dtype == BXS_F16)
+    return dynconv_forward_h(static_cast<const __half*>(feat), C, static_cast<const __half*>(kernels),
+                             static_cast<__half*>(out), B, C, P, I, st);
+  return dynconv_forward_h(static_cast<const __nv_bfloat16*>(feat), C, static_cast<const __nv_bfloat16*>(kernels),
+                           static_cast<__nv_bfloat16*>(out), B, C, P, I, st);
+}
+
+extern "C" int64_t bxs_dynconv1x1_half_backward_workspace_bytes(int64_t B, int64_t C, int64_t P, int64_t I, int dtype) {
+  if (B <= 0 || C <= 0 || P <= 0 || I <= 0 || !known_half(dtype)) return 0;
+  const int64_t ipad = ceil_div(I, 32) * 32;
+  return 2 * B * C * ipad + 1024 + 4 * B * (int64_t)wg_splits(B, P, I, H_BLOCK_K) * I * C + 1024;
+}
+
+extern "C" int bxs_dynconv1x1_half_backward(const void* feat, const void* kernels, const void* g_out, void* g_feat,
+                                            void* g_kernels, void* workspace, int64_t B, int64_t C, int64_t P, int64_t I,
+                                            int dtype, bxs_stream_t stream) {
+  if (!feat || !kernels || !g_out || (!g_feat && !g_kernels) || !workspace || B <= 0 || C <= 0 || P <= 0 || I <= 0 ||
+      !known_half(dtype))
+    return BXS_ERR_INVALID_ARG;
+  if (!half_shape_ok(B, C, P, I) || (g_feat && I > 256) || misaligned16(feat) || misaligned16(kernels) ||
+      misaligned16(g_out) || misaligned16(g_feat))
+    return BXS_ERR_UNSUPPORTED;
+  cudaStream_t st = as_stream(stream);
+  if (dtype == BXS_F16)
+    return dynconv_backward_h(static_cast<const __half*>(feat), static_cast<const __half*>(kernels),
+                              static_cast<const __half*>(g_out), static_cast<__half*>(g_feat),
+                              static_cast<__half*>(g_kernels), workspace, B, C, P, I, st);
+  return dynconv_backward_h(static_cast<const __nv_bfloat16*>(feat), static_cast<const __nv_bfloat16*>(kernels),
+                            static_cast<const __nv_bfloat16*>(g_out), static_cast<__nv_bfloat16*>(g_feat),
+                            static_cast<__nv_bfloat16*>(g_kernels), workspace, B, C, P, I, st);
 }

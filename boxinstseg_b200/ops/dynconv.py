@@ -5,28 +5,80 @@ Backward is the same machinery (bxs_dynconv1x1_backward): d/d feat = kernel^T . 
 the operand roles swapped, d/d kernel = g_out . feat^T is a split-K wgmma kernel over the pixels with an ordered
 (deterministic) reduction of the partials.  Only d/d feat with more than 256 kernels per image (outside every reference
 call site: the heads convolve the POSITIVE kernels of an image) goes through cuBLAS (torch.bmm).
+
+FP16 / BF16 operands run the 16-bit kernels (bxs_dynconv1x1_half_*: FP32 accumulation, result and gradients in the
+operand dtype), and under ``torch.autocast('cuda')`` both operands are cast to the autocast dtype first, as autocast does
+for the ``F.conv2d`` this op replaces.
 """
 import torch
 
 from .. import _lib as L
 
+_HALF = {torch.float16: 0, torch.bfloat16: 1}          # bxs_half_t
+_AUTOCAST_ELIGIBLE = (torch.float32, torch.float16, torch.bfloat16)
+
+
+def _half_native(*tensors):
+    """Inside the envelope of the 16-bit kernels: C % 32 == 0, C <= 256, h*w % 8 == 0, 16-byte aligned bases."""
+    B, C, h, w = tensors[0].shape
+    return C % 32 == 0 and C <= 256 and (h * w) % 8 == 0 and all(t.data_ptr() % 16 == 0 for t in tensors)
+
+
+def _forward(f, k):
+    B, C, h, w = f.shape
+    I = k.shape[1]
+    out = torch.empty((B, I, h, w), dtype=f.dtype, device=f.device)
+    if B and I:
+        with torch.cuda.device(f.device):
+            if f.dtype == torch.float32:
+                L.check(L.lib().bxs_dynconv1x1_forward(L.ptr(f), L.ptr(k), L.ptr(out), B, C, h * w, I, L.stream()),
+                        'dynconv1x1_forward')
+            else:
+                L.check(L.lib().bxs_dynconv1x1_half_forward(L.ptr(f), L.ptr(k), L.ptr(out), B, C, h * w, I, _HALF[f.dtype],
+                                                            L.stream()), 'dynconv1x1_half_forward')
+    return out
+
+
+def _backward(f, k, g, need_f, need_k):
+    B, C, h, w = f.shape
+    I = k.shape[1]
+    gf = gk = None
+    native_f = need_f and I <= 256
+    if need_f and not native_f:
+        gf = torch.bmm(k.transpose(1, 2), g.flatten(2)).view(B, C, h, w)
+    if native_f or need_k:
+        gf = torch.empty_like(f) if native_f else gf
+        gk = torch.empty_like(k) if need_k else None
+        with torch.cuda.device(f.device):
+            if f.dtype == torch.float32:
+                ws = torch.empty(L.lib().bxs_dynconv1x1_backward_workspace_bytes(B, C, h * w, I), dtype=torch.uint8,
+                                 device=f.device)
+                L.check(L.lib().bxs_dynconv1x1_backward(L.ptr(f), L.ptr(k), L.ptr(g), L.ptr(gf) if native_f else None,
+                                                        L.ptr(gk), L.ptr(ws), B, C, h * w, I, L.stream()),
+                        'dynconv1x1_backward')
+            else:
+                dt = _HALF[f.dtype]
+                ws = torch.empty(L.lib().bxs_dynconv1x1_half_backward_workspace_bytes(B, C, h * w, I, dt),
+                                 dtype=torch.uint8, device=f.device)
+                L.check(L.lib().bxs_dynconv1x1_half_backward(L.ptr(f), L.ptr(k), L.ptr(g),
+                                                             L.ptr(gf) if native_f else None, L.ptr(gk), L.ptr(ws), B, C,
+                                                             h * w, I, dt, L.stream()), 'dynconv1x1_half_backward')
+    return gf, gk
+
 
 class _DynConv1x1(torch.autograd.Function):
     @staticmethod
     def forward(ctx, feat, kernels):
-        f = feat.contiguous().float()
-        k = kernels.contiguous().float()
+        half = feat.dtype == kernels.dtype and feat.dtype in _HALF
+        f = feat.contiguous() if half else feat.contiguous().float()
+        k = kernels.contiguous() if half else kernels.contiguous().float()
         L.require_cuda(f, k)
         B, C, h, w = f.shape
         assert k.dim() == 3 and k.shape[0] == B and k.shape[2] == C, 'kernels must be [B,I,C]'
-        I = k.shape[1]
-        out = torch.empty((B, I, h, w), dtype=torch.float32, device=f.device)
-        if B and I:
-            with torch.cuda.device(f.device):
-                L.check(L.lib().bxs_dynconv1x1_forward(L.ptr(f), L.ptr(k), L.ptr(out), B, C, h * w, I, L.stream()),
-                        'dynconv1x1_forward')
         ctx.save_for_backward(f, k)
-        return out
+        if half and not _half_native(f, k):             # outside the 16-bit envelope: the FP32 kernels on promoted copies
+            return _forward(f.float(), k.float()).to(f.dtype)
+        return _forward(f, k)
 
     @staticmethod
     def backward(ctx, g_out):
@@ -36,25 +88,29 @@ class _DynConv1x1(torch.autograd.Function):
         need_f, need_k = ctx.needs_input_grad[0], ctx.needs_input_grad[1]
         if not (B and I) or not (need_f or need_k):
             return (torch.zeros_like(f) if need_f else None), (torch.zeros_like(k) if need_k else None)
-        g = g_out.contiguous().float()
-        gf = gk = None
-        native_f = need_f and I <= 256
-        if need_f and not native_f:
-            gf = torch.bmm(k.transpose(1, 2), g.flatten(2)).view(B, C, h, w)
-        if native_f or need_k:
-            gf = torch.empty_like(f) if native_f else gf
-            gk = torch.empty_like(k) if need_k else None
-            with torch.cuda.device(f.device):
-                ws = torch.empty(L.lib().bxs_dynconv1x1_backward_workspace_bytes(B, C, h * w, I), dtype=torch.uint8,
-                                 device=f.device)
-                L.check(L.lib().bxs_dynconv1x1_backward(L.ptr(f), L.ptr(k), L.ptr(g), L.ptr(gf) if native_f else None,
-                                                        L.ptr(gk), L.ptr(ws), B, C, h * w, I, L.stream()),
-                        'dynconv1x1_backward')
-        return gf, gk
+        g = g_out.contiguous().to(f.dtype)
+        if f.dtype != torch.float32 and not _half_native(f, k, g):
+            gf, gk = _backward(f.float(), k.float(), g.float(), need_f, need_k)
+            return (None if gf is None else gf.to(f.dtype)), (None if gk is None else gk.to(f.dtype))
+        return _backward(f, k, g, need_f, need_k)
 
 
 def dynconv1x1(feat, kernels):
-    """feat [B,C,h,w], kernels [B,I,C] -> [B,I,h,w]   (C % 32 == 0, C <= 256, h*w % 4 == 0)."""
+    """feat [B,C,h,w], kernels [B,I,C] -> [B,I,h,w]   (C % 32 == 0, C <= 256, h*w % 4 == 0).
+
+    The dtype rules of the ``F.conv2d`` / ``einsum`` it replaces:
+      * both operands float32: TF32 kernels, float32 result and gradients;
+      * both float16 or both bfloat16: 16-bit kernels (FP32 accumulation), result and gradients in that dtype
+        (outside their envelope -- h*w % 8 != 0 -- the float32 kernels on promoted copies, rounded back);
+      * inside ``torch.autocast('cuda')``: both operands are cast to the autocast dtype first, then the above; gradients
+        reach float32 leaves in float32 through autograd's cast;
+      * any other mix: both promoted to float32.
+    """
+    if torch.is_autocast_enabled('cuda'):
+        dt = torch.get_autocast_dtype('cuda')
+        cast = lambda t: t.to(dt) if t.is_cuda and t.dtype in _AUTOCAST_ELIGIBLE else t    # noqa: E731
+        with torch.autocast('cuda', enabled=False):
+            return _DynConv1x1.apply(cast(feat), cast(kernels))
     return _DynConv1x1.apply(feat, kernels)
 
 

@@ -307,6 +307,24 @@ int64_t bxs_dynconv1x1_backward_workspace_bytes(int64_t B, int64_t C, int64_t P,
 int bxs_dynconv1x1_backward(const float* feat, const float* kernels, const float* g_out, float* g_feat, float* g_kernels,
                             void* workspace, int64_t B, int64_t C, int64_t P, int64_t I, bxs_stream_t stream);
 
+/* The same three products with 16-bit operands, for callers that run under torch.autocast (the reference's DiscoBox
+ * configs train in FP16): feat, kernels, out, g_out, g_feat and g_kernels are all of the type `dtype` names, and the
+ * tensor cores accumulate in FP32.  Each result is rounded to `dtype` once, at the end; d/d kernel keeps FP32 split-K
+ * partials in the workspace and rounds only after their ordered (deterministic) reduction.  No TF32 step: the operands
+ * are multiplied exactly.
+ * BXS_ERR_INVALID_ARG: a NULL pointer (both gradient outputs NULL in the backward), a non-positive size or an unknown
+ * dtype.  BXS_ERR_UNSUPPORTED: C % 32 != 0, C > 256, P % 8 != 0 (the tensor maps need 16-byte row strides), a base
+ * that is not 16-byte aligned, or g_feat with I > 256.  All checks run before any device call.
+ * workspace: bxs_dynconv1x1_half_backward_workspace_bytes(B, C, P, I, dtype) bytes (0 for an empty shape or an unknown
+ * dtype). */
+typedef enum { BXS_F16 = 0, BXS_BF16 = 1 } bxs_half_t;
+int bxs_dynconv1x1_half_forward(const void* feat, const void* kernels, void* out, int64_t B, int64_t C, int64_t P,
+                                int64_t I, int dtype, bxs_stream_t stream);
+int64_t bxs_dynconv1x1_half_backward_workspace_bytes(int64_t B, int64_t C, int64_t P, int64_t I, int dtype);
+int bxs_dynconv1x1_half_backward(const void* feat, const void* kernels, const void* g_out, void* g_feat, void* g_kernels,
+                                 void* workspace, int64_t B, int64_t C, int64_t P, int64_t I, int dtype,
+                                 bxs_stream_t stream);
+
 /* ---------------------------------------------------------------------------------------
  * (SURVEY 8f rank 1)  projection profiles of a bilinearly resized map, never materialised.
  *     replaces, for BoxMatchingCost (mmdet/core/bbox/match_costs/match_cost.py:400-425), the F.interpolate of
