@@ -79,12 +79,14 @@ SIGNATURES = {
     'bxs_corr_transfer_workspace_bytes': [c_i64] * 3,
     'bxs_corr_transfer': [c_p] * 7 + [c_i64] * 5 + [c_p],
     'bxs_fcos_targets': [c_p] * 7 + [c_i64] * 2 + [c_p] * 5 + [c_int, c_int, c_i64, c_p],
+    'bxs_lsap_workspace_bytes': [c_p, c_p, c_i64],
+    'bxs_lsap_solve': [c_p] * 4 + [c_i64, c_int] + [c_p] * 4,
 }
 _RESTYPE = {'bxs_mst_workspace_bytes': c_i64, 'bxs_bfs_workspace_bytes': c_i64, 'bxs_refine_scratch_bytes': c_i64, 'bxs_lcm_workspace_bytes': c_i64, 'bxs_meanfield_workspace_bytes': c_i64, 'bxs_projection_workspace_bytes': c_i64,'bxs_condinst_head_workspace_bytes': c_i64, 'bxs_last_error': ctypes.c_char_p, 'bxs_boxinst_loss_workspace_bytes': c_i64,
              'bxs_boxinst_loss_fused_workspace_bytes': c_i64, 'bxs_boxinst_loss_fused_sched_bytes': c_i64,
              'bxs_boxinst_loss_plan_bytes': c_i64, 'bxs_levelset_fused_workspace_bytes': c_i64,
              'bxs_dynconv1x1_backward_workspace_bytes': c_i64, 'bxs_corr_transfer_workspace_bytes': c_i64,
-             'bxs_dynconv1x1_half_backward_workspace_bytes': c_i64}
+             'bxs_dynconv1x1_half_backward_workspace_bytes': c_i64, 'bxs_lsap_workspace_bytes': c_i64}
 
 _STATUS = {-1: 'invalid argument', -2: 'kernel launch failed', -3: 'unsupported shape', -4: 'no CUDA device'}
 

@@ -6,20 +6,18 @@ resolution ([100,1,1024,1024] per image per decoder layer, 420 MB x 10) only so 
 maxima of it.  ``assign(..., lowres=True)`` hands the LOW-resolution prediction to BoxMatchingCost.cost_from_lowres instead:
 the fused bilinear-upsample -> sigmoid -> projection kernel (bxs_upsampled_rowcol_max) never builds that tensor.
 
-Step 3, the Hungarian matching itself, is scipy.optimize.linear_sum_assignment on the host exactly as in the reference
-(:119); the cost matrix ([100, G] floats) is all that crosses PCIe.
+Step 3, the Hungarian matching (the reference's scipy.optimize.linear_sum_assignment on the host, :113-123), is the LSAP
+kernel of ops.lsap: scipy's algorithm and tie rules in float64, so the matching is scipy's bit for bit, and the cost matrix
+stays on the device.  ``assign`` reads one 4-byte status to raise scipy's errors; Box2MaskHead.get_targets matches a whole
+decoder layer in one launch without reading anything back.
 """
 from collections import namedtuple
 
 import torch
 
 from ..models.builder import MATCH_COST, register
+from ..ops.lsap import raise_for_status, solve_batched
 from .match_cost import BoxMatchingCost
-
-try:
-    from scipy.optimize import linear_sum_assignment
-except ImportError:                                  # pragma: no cover
-    linear_sum_assignment = None
 
 AssignResult = namedtuple('AssignResult', ['num_gts', 'gt_inds', 'max_overlaps', 'labels'])   # assign_result.py fields
 
@@ -83,13 +81,9 @@ class MaskHungarianAssigner:
             if num_gt == 0:
                 assigned_gt_inds[:] = 0
             return AssignResult(num_gt, assigned_gt_inds, None, assigned_labels)
-        cost = self.cost_matrix(cls_pred, mask_pred, gt_labels, gt_mask, lowres).detach().cpu()
-        if linear_sum_assignment is None:
-            raise ImportError('Please run "pip install scipy" to install scipy first.')
-        rows, cols = linear_sum_assignment(cost)
-        rows = torch.from_numpy(rows).to(mask_pred.device)
-        cols = torch.from_numpy(cols).to(mask_pred.device)
-        assigned_gt_inds[:] = 0
-        assigned_gt_inds[rows] = cols + 1
-        assigned_labels[rows] = gt_labels[cols]
-        return AssignResult(num_gt, assigned_gt_inds, None, assigned_labels)
+        cost = self.cost_matrix(cls_pred, mask_pred, gt_labels, gt_mask, lowres)
+        (match,), status = solve_batched([cost])
+        raise_for_status(int(status[0]))
+        m = match.long()                     # matched ground truth per query or -1 -> gt_inds 0 = background (:125-132)
+        labels = torch.where(m >= 0, gt_labels[m.clamp(min=0)].long(), -1)
+        return AssignResult(num_gt, m + 1, None, labels)

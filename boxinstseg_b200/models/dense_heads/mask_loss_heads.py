@@ -17,6 +17,7 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 from ...ops.dynconv import box2mask_mask_pred, dynconv1x1, solo_dynamic_conv
+from ...ops.lsap import solve_batched
 from ...ops.resize import bilinear_resize, scale_target as _scale_target   # a18: F.interpolate / _scale_target as kernels
 from ...ops._streams import Forked, run_concurrently
 from ...ops.tree_filter import MinimumSpanningTree, TreeFilter2D
@@ -289,14 +290,68 @@ class Box2MaskHead(nn.Module):
     """Box2Mask head: mask-loss path only."""
 
     def __init__(self, in_channels=None, feat_channels=256, out_channels=256, num_things_classes=80, num_stuff_classes=0,
-                 num_queries=100, loss_box=None, loss_mask=None, **cfg):
+                 num_queries=100, loss_box=None, loss_mask=None, train_cfg=None, **cfg):
         super().__init__()
         self.num_queries = num_queries
+        self.num_classes = num_things_classes + num_stuff_classes
+        self.train_cfg = train_cfg
         self.cfg = cfg
         self.loss_box = build_loss(loss_box or dict(type='BoxProjectionLoss', loss_weight=5.0))
         self.loss_mask = build_loss(loss_mask or dict(type='LevelsetLoss', loss_weight=1.0))
         self.mst = MinimumSpanningTree(TreeFilter2D.norm2_distance)
         self.tree_filter = TreeFilter2D()
+        self._bxs_post_init()
+
+    def _bxs_post_init(self):
+        """Also runs after the REFERENCE class's ``__init__`` when mmdet is importable: the matcher of ``get_targets`` is
+        this package's MaskHungarianAssigner, built from the same ``train_cfg['assigner']`` (box2mask_head.py:95-97)."""
+        from ...core.assigner import MaskHungarianAssigner      # core imports models.builder: not at module level
+        cfg = (getattr(self, 'train_cfg', None) or {}).get('assigner')
+        self.hungarian = MaskHungarianAssigner(**{k: v for k, v in cfg.items() if k != 'type'}) if cfg else None
+        self.lsap_status = None
+
+    # f1 -- box2mask_head.py:135-189 (get_targets + _get_target_single with MaskPseudoSampler), the reference's signature
+    @torch.no_grad()
+    def get_targets(self, cls_scores_list, mask_preds_list, gt_labels_list, gt_masks_list, img_metas):
+        """Classification and mask targets of one decoder layer for all images: (labels_list, label_weights_list,
+        mask_targets_list, mask_weights_list, num_total_pos, num_total_neg), as the reference returns them.
+        cls_scores_list[b] [Q,C+1], mask_preds_list[b] [Q,h,w] (low resolution: the assigner's BoxMatchingCost upsamples it
+        virtually to the ground truths' size), gt_labels_list[b] [G_b], gt_masks_list[b] [G_b,H,W].
+        The cost matrices of all images are matched in ONE launch and nothing is read back to the host: the call runs under
+        torch.cuda.set_sync_debug_mode('error') and can be captured in a CUDA graph.  Every size comes from the shapes:
+        min(Q, G_b) positives per image, in ascending query order, pos_assigned_gt_inds = match[pos_inds].
+        An image whose cost matrix holds a NaN (NaN predictions) cannot raise without a synchronisation: its queries come
+        back as background (labels = num_classes, mask_weights = 0), its min(Q, G_b) mask_targets rows are placeholders,
+        and ``self.lsap_status`` (int32 [B] on the device, 1 for such an image, else 0) keeps the per-image status."""
+        if self.hungarian is None:
+            raise RuntimeError('Box2MaskHead.get_targets needs train_cfg with an assigner')
+        Q = self.num_queries
+        costs = []
+        for cls_score, mask_pred, gt_labels, gt_masks in zip(cls_scores_list, mask_preds_list, gt_labels_list, gt_masks_list):
+            if gt_labels.shape[0] and mask_pred.shape[0]:
+                costs.append(self.hungarian.cost_matrix(cls_score, mask_pred, gt_labels, gt_masks, lowres=True))
+            else:
+                costs.append(mask_pred.new_zeros((mask_pred.shape[0], gt_labels.shape[0])))
+        matches, self.lsap_status = solve_batched(costs)
+        labels_list, label_weights_list, mask_targets_list, mask_weights_list = [], [], [], []
+        num_total_pos = num_total_neg = 0
+        for match, mask_pred, gt_labels, gt_masks in zip(matches, mask_preds_list, gt_labels_list, gt_masks_list):
+            m = match.long()
+            pos = m >= 0
+            k = min(mask_pred.shape[0], gt_labels.shape[0])
+            pos_inds = torch.nonzero_static(pos, size=k, fill_value=0).squeeze(1)
+            pos_gt = m[pos_inds].clamp(min=0)
+            if gt_labels.shape[0]:
+                labels = torch.where(pos, gt_labels[m.clamp(min=0)].long(), self.num_classes)
+            else:
+                labels = gt_labels.new_full((Q,), self.num_classes, dtype=torch.long)
+            labels_list.append(labels)
+            label_weights_list.append(gt_labels.new_ones((Q,)))
+            mask_targets_list.append(gt_masks.unsqueeze(1)[pos_gt])
+            mask_weights_list.append(pos.to(mask_pred.dtype))
+            num_total_pos += k
+            num_total_neg += mask_pred.shape[0] - k
+        return labels_list, label_weights_list, mask_targets_list, mask_weights_list, num_total_pos, num_total_neg
 
     # a4 -- box2mask_head.py:343-345
     @staticmethod

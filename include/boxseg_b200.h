@@ -422,6 +422,25 @@ int64_t bxs_corr_transfer_workspace_bytes(int64_t K, int64_t Hm, int64_t Wm);
 int bxs_corr_transfer(const float* T, const float* Cu, const float* m0, const float* m1, float* fg_ci, float* bg_ci,
                       void* workspace, int64_t K, int64_t h, int64_t w, int64_t Hm, int64_t Wm, bxs_stream_t stream);
 
+/* ---------------------------------------------------------------------------------------
+ * f1  Hungarian matching    replaces scipy.optimize.linear_sum_assignment in MaskHungarianAssigner.assign step 3
+ *     (mmdet/core/bbox/assigners/mask_hungarian_assigner.py:113-123) for a batch of independent problems.
+ * Problem p is the rows_host[p] x cols_host[p] row-major matrix at element offset_host[p] of `cost` (f32 or f64, as
+ * `dtype` names; widened to f64 exactly).  The *_host arrays are HOST arrays, copied into the kernel parameters in chunks
+ * (no H2D copy, no host read: the call can be captured in a CUDA graph).
+ * match i32 [sum rows]: problem p's rows follow those of the problems before it; entry = the matched column, or -1.
+ * status i32 [num_problems] on the device: 0 ok, 1 a NaN or -inf entry, 2 infeasible; a failed problem leaves its rows
+ * at -1.  The result equals scipy's (row_ind = the rows with match >= 0, col_ind = their match), ties included.
+ * workspace: bxs_lsap_workspace_bytes(rows_host, cols_host, num_problems) bytes (0 when every problem is empty).
+ * BXS_ERR_INVALID_ARG: a NULL pointer that the shapes need, a negative size or offset, an unknown dtype;
+ * BXS_ERR_UNSUPPORTED: a dimension above INT32_MAX.  All checks run before any device call.
+ * --------------------------------------------------------------------------------------- */
+typedef enum { BXS_LSAP_F32 = 0, BXS_LSAP_F64 = 1 } bxs_lsap_dtype_t;
+int64_t bxs_lsap_workspace_bytes(const int64_t* rows_host, const int64_t* cols_host, int64_t num_problems);
+int bxs_lsap_solve(const void* cost, const int64_t* offset_host, const int64_t* rows_host, const int64_t* cols_host,
+                   int64_t num_problems, int dtype, int32_t* match, int32_t* status, void* workspace,
+                   bxs_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
