@@ -9,23 +9,12 @@
 // instead of the reference's ~8 elementwise launches with [n,C,h,w] temporaries each.
 #include <algorithm>
 
-#include "common.cuh"
+#include "boxinst_common.cuh"         // fkey / fkey_inv / pack_key: one tie rule with the BoxInst loss kernels
 
 namespace bxs {
 namespace {
 
 constexpr int NT = 256;
-
-__device__ __forceinline__ unsigned fkey(float f) {
-  const unsigned b = __float_as_uint(f);
-  return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
-}
-__device__ __forceinline__ float fkey_inv(unsigned k) {
-  return __uint_as_float((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k);
-}
-__device__ __forceinline__ unsigned long long pack_key(unsigned key, int index) {
-  return ((unsigned long long)key << 32) | (unsigned long long)(0xffffffffu - (unsigned)index);
-}
 
 // ---------------------------------------------------------------------------------------
 // projection: row / column maxima of scores (with first arg-max) and of targets

@@ -97,6 +97,32 @@ def projection_losses(scores, targets, eps=1e-5):
     return dice_1d(row_s, row_t, eps) + dice_1d(col_s, col_t, eps)
 
 
+def projection_losses_logit_argmax(logits, targets, eps=1e-5):
+    """Per-instance projection loss [n] with the positions chosen on the LOGITS, in float64.
+
+    This is what the BoxInst kernels compute (DESIGN section 4, note (i)): the row / column
+    arg-max of the logits by torch.max(dim) -- the first index on exact ties, -0 equal to +0 --
+    then the sigmoid at those positions.  ``projection_losses(sigmoid(x))`` picks its positions
+    among the scores instead, which differ where the sigmoid saturates, so it cannot judge them.
+    """
+    x = logits.to(torch.float64)
+    t = targets.to(torch.float64)
+    s = torch.sigmoid(x)
+    row_s = s.gather(3, x.max(dim=3, keepdim=True)[1]).squeeze(3)   # [n,1,H]
+    col_s = s.gather(2, x.max(dim=2, keepdim=True)[1]).squeeze(2)   # [n,1,W]
+    return dice_1d(row_s, t.amax(dim=3), eps) + dice_1d(col_s, t.amax(dim=2), eps)
+
+
+def logit_argmax_mask(logits):
+    """bool [n,1,H,W]: the elements that are the first row or column arg-max of ``logits``
+    (torch.max(dim)); the only places the projection term sends a gradient."""
+    n, c, h, w = logits.shape
+    m = torch.zeros(n, c, h, w, dtype=torch.bool, device=logits.device)
+    m.scatter_(3, logits.max(dim=3, keepdim=True)[1], True)
+    m.scatter_(2, logits.max(dim=2, keepdim=True)[1], True)
+    return m
+
+
 # ----------------------------------------------------------------------------------------
 # a5: targets
 # ----------------------------------------------------------------------------------------

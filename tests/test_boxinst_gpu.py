@@ -265,8 +265,17 @@ def test_fused_loss_full_size_properties(dev):
     assert abs(prj.item() - prj_ref.item()) <= 1e-4 * abs(prj_ref.item())
     assert abs(pair.item() - pair_ref.item()) <= 1e-4 * abs(pair_ref.item())
     assert rel_err(gx, gref) <= 1e-3
-    # gradient is exactly zero where it must be: outside the dilated box and off the arg-max lines
+    # gradient is exactly zero where it must be: outside each instance's box grown by the dilation (2), except at the row /
+    # column arg-max positions of the logits (torch.max(dim))
+    from oracle.boxinst import logit_argmax_mask
     assert torch.isfinite(gx).all()
+    N, _, H, W = x.shape
+    j0, j1, i0, i1 = (t.rects[gi].long().cpu()[:, k].view(-1, 1, 1) for k in range(4))
+    ys, xs = torch.arange(H).view(1, H, 1), torch.arange(W).view(1, 1, W)
+    span = (j0 <= j1) & (i0 <= i1) & (ys >= j0 - 2) & (ys <= j1 + 2) & (xs >= i0 - 2) & (xs <= i1 + 2)
+    allowed = span[:, None] | logit_argmax_mask(x.detach().cpu())
+    assert (gx.cpu()[~allowed] == 0).all()
+    assert (gx.cpu()[~span[:, None].expand(N, 1, H, W)] != 0).any()      # the arg-max positions do carry gradient
 
 
 # ------------------------------------------------------------------ a6+a7+a8 single-pass schedule (boxinst_onepass.cu)
