@@ -53,6 +53,10 @@ SIGNATURES = {
     'bxs_meanfield_kernel': [c_p, c_p] + [c_i64] * 4 + [c_int, c_f, c_f, c_f, c_p],
     'bxs_meanfield_workspace_bytes': [c_i64] * 3,
     'bxs_meanfield_forward_inter': [c_p] * 5 + [c_f] + [c_p] * 4 + [c_i64] * 3 + [c_int, c_int, c_p],
+    'bxs_meanfield_forward_logits': [c_p] * 5 + [c_int] + [c_p] * 3 + [c_i64] * 3 + [c_int, c_int, c_p],
+    'bxs_discobox_loss_workspace_bytes': [c_i64] * 3,
+    'bxs_discobox_loss_forward': [c_p] * 3 + [c_int] + [c_p] * 2 + [c_i64] * 3 + [c_p],
+    'bxs_discobox_loss_backward': [c_p] * 3 + [c_int] + [c_p] * 3 + [c_i64] * 3 + [c_p],
     'bxs_mst_workspace_bytes': [c_i64] * 3,
     'bxs_mst_forward': [c_p] * 4 + [c_i64] * 3 + [c_p],
     'bxs_bfs_workspace_bytes': [c_i64] * 2,
@@ -86,7 +90,8 @@ _RESTYPE = {'bxs_mst_workspace_bytes': c_i64, 'bxs_bfs_workspace_bytes': c_i64, 
              'bxs_boxinst_loss_fused_workspace_bytes': c_i64, 'bxs_boxinst_loss_fused_sched_bytes': c_i64,
              'bxs_boxinst_loss_plan_bytes': c_i64, 'bxs_levelset_fused_workspace_bytes': c_i64,
              'bxs_dynconv1x1_backward_workspace_bytes': c_i64, 'bxs_corr_transfer_workspace_bytes': c_i64,
-             'bxs_dynconv1x1_half_backward_workspace_bytes': c_i64, 'bxs_lsap_workspace_bytes': c_i64}
+             'bxs_dynconv1x1_half_backward_workspace_bytes': c_i64, 'bxs_lsap_workspace_bytes': c_i64,
+             'bxs_discobox_loss_workspace_bytes': c_i64}
 
 _STATUS = {-1: 'invalid argument', -2: 'kernel launch failed', -3: 'unsupported shape', -4: 'no CUDA device'}
 

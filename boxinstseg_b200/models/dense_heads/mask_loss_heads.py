@@ -16,6 +16,7 @@ import torch
 import torch.nn as nn
 import torch.nn.functional as F
 
+from ...ops.discobox import HALF_DTYPES, discobox_mask_loss
 from ...ops.dynconv import box2mask_mask_pred, dynconv1x1, solo_dynamic_conv
 from ...ops.lsap import solve_batched
 from ...ops.resize import bilinear_resize, scale_target as _scale_target   # a18: F.interpolate / _scale_target as kernels
@@ -252,7 +253,10 @@ class DiscoBoxSOLOv2Head(nn.Module):
         color_feats [B,3,h,w] = image resized with align_corners=True (:1201).
         No host synchronisation and no boolean indexing: instances with an all-zero target (removed by the reference,
         :1283-1287) stay in the batch with weight 0 -- the mean over the kept instances is a weighted mean -- and ONE
-        mean-field module holds the bilateral kernels of all images (``obj_img`` picks the image of each object)."""
+        mean-field module holds the bilateral kernels of all images (``obj_img`` picks the image of each object).
+        A level whose student logits (and independent-teacher logits, if any) are float16 or bfloat16 -- the reference's
+        autocast training -- runs ``ops.discobox.discobox_mask_loss`` on them as they are; any other level, float32
+        included, the composition of ``_mask_loss_level_eager``.  The dtype of the input decides, not the autocast state."""
         mf = MeanField(color_feats, alpha0=self.alpha0, theta0=self.theta0, theta1=self.theta1, theta2=self.theta2,
                        iter=self.crf_max_iter, kernel_size=self.mkernel, base=self.crf_base) if use_loss_ts else None
         t_list = t_ins_pred_list if t_ins_pred_list is not None else s_ins_pred_list
@@ -260,16 +264,15 @@ class DiscoBoxSOLOv2Head(nn.Module):
         for s_in, t_in, img_inds, target in zip(s_ins_pred_list, t_list, img_ind_list, ins_labels):
             if s_in is None or s_in.shape[0] == 0:
                 continue
-            target = target.float()
-            keep = (target.flatten(1).sum(1) > 0).float()            # all-zero targets carry weight 0 (:1283-1287)
-            s = torch.sigmoid(s_in)
-            t = s if t_ins_pred_list is None else torch.sigmoid(t_in)
-            num_ins.append((mil_loss(None, s, s, target) * keep).sum())
-            den.append(keep.sum())
+            t_ind = t_in if t_ins_pred_list is not None else None
+            if s_in.dtype in HALF_DTYPES and (t_ind is None or t_ind.dtype == s_in.dtype):
+                n_ins, n_ts, cnt = discobox_mask_loss(s_in, target, img_inds, mf, t_ind, use_loss_ts)
+            else:
+                n_ins, n_ts, cnt = self._mask_loss_level_eager(s_in, t_ind, img_inds, target, mf, use_loss_ts)
+            num_ins.append(n_ins)
+            den.append(cnt)
             if use_loss_ts:
-                enlarged = F.max_pool2d(target.unsqueeze(1), kernel_size=3, stride=1, padding=1).squeeze(1)
-                pseudo, _ = mf(((t + s) / 2).unsqueeze(1), target.unsqueeze(1), obj_img=img_inds)
-                num_ts.append((_disco_dice(s * enlarged, pseudo) * keep).sum())
+                num_ts.append(n_ts)
         zero = color_feats.new_zeros(())
         if not num_ins:
             return dict(loss_ins=zero, loss_ts=zero)
@@ -277,6 +280,23 @@ class DiscoBoxSOLOv2Head(nn.Module):
         l_ins = torch.stack(num_ins).sum() / count * self.ins_loss_weight
         l_ts = torch.stack(num_ts).sum() / count * self.ts_loss_weight if (use_loss_ts and num_ts) else zero
         return dict(loss_ins=l_ins, loss_ts=l_ts)
+
+    @staticmethod
+    def _mask_loss_level_eager(s_in, t_in, img_inds, target, mf, use_loss_ts):
+        """One level of ``mask_loss`` as a composition of torch ops and the float32 kernels (projection loss, mean field):
+        (sum keep * mil, sum keep * d_ts or None, sum keep).  ``t_in``: independent-teacher logits or None."""
+        target = target.float()
+        keep = (target.flatten(1).sum(1) > 0).float()            # all-zero targets carry weight 0 (:1283-1287)
+        s = torch.sigmoid(s_in)
+        t = s if t_in is None else torch.sigmoid(t_in)
+        n_ins = (mil_loss(None, s, s, target) * keep).sum()
+        cnt = keep.sum()
+        n_ts = None
+        if use_loss_ts:
+            enlarged = F.max_pool2d(target.unsqueeze(1), kernel_size=3, stride=1, padding=1).squeeze(1)
+            pseudo, _ = mf(((t + s) / 2).unsqueeze(1), target.unsqueeze(1), obj_img=img_inds)
+            n_ts = (_disco_dice(s * enlarged, pseudo) * keep).sum()
+        return n_ins, n_ts, cnt
 
 
 def _disco_dice(x, t):

@@ -233,6 +233,44 @@ int bxs_meanfield_forward_inter(const float* K, const int32_t* obj_img, const fl
                                 float* valid, void* workspace, int64_t n, int64_t h, int64_t w, int kernel_size,
                                 int num_iter, bxs_stream_t stream);
 
+/* The mean field of the DiscoBox mask loss on 16-bit predictions (the reference under autocast, discobox_head.py:1142):
+ * s_logits, t_logits [n,h,w] of the type `dtype` (a bxs_half_t) names; t_logits NULL = no independent teacher (t = s);
+ * targets uint8 [n,h,w].  The initial state is x = (t + s) / 2 with s = round(sigmoid(s_logits)), t = round(sigmoid(
+ * t_logits)) and every step rounded to `dtype`, as torch computes it; the rounds are those of
+ * bxs_meanfield_forward_inter, and the result equals it on x.float() and the targets as float32, bit for bit.
+ * pseudo: uint8 [n,h,w] in {0,1}; no `valid` (the loss does not read it).  workspace: bxs_meanfield_workspace_bytes(n,h,w)
+ * bytes, or NULL for the per-object schedule (bit maps in shared memory, 2*h*w bytes <= 200 KB).
+ * BXS_ERR_INVALID_ARG: a NULL pointer (with n > 0), a negative n, a non-positive h / w, an even kernel size, a negative
+ * num_iter, an unknown dtype, or no workspace for a map too large for shared memory.  BXS_ERR_UNSUPPORTED: h*w >= 2^30.
+ * All checks run before any device call; n == 0 does nothing. */
+int bxs_meanfield_forward_logits(const float* K, const int32_t* obj_img, const void* s_logits, const void* t_logits,
+                                 const uint8_t* targets, int dtype, const float* neglog4_host, uint8_t* pseudo,
+                                 void* workspace, int64_t n, int64_t h, int64_t w, int kernel_size, int num_iter,
+                                 bxs_stream_t stream);
+
+/* ---------------------------------------------------------------------------------------
+ * a6 + a17  DiscoBox mask loss of one level on 16-bit logits     replaces, under autocast, the chain of
+ *     DiscoBoxSOLOv2Head.loss (discobox_head.py:1266-1300): sigmoid, mil_loss + dice_loss (:542-562), max_pool2d of
+ *     the target, s * enlarged and the teacher-student dice_loss against the mean-field pseudo-label.
+ * s_logits [n,h,w] of the type `dtype` names; targets uint8 [n,h,w] (non-zero = object); pseudo uint8 [n,h,w] from
+ * bxs_meanfield_forward_logits, or NULL without the teacher-student term.  s = round(sigmoid(s_logits)) as torch computes
+ * it; the row / column maxima and their first arg-max are taken on the rounded s; sums are float32 in a fixed order.
+ * forward: out float[3] on the device = {sum keep * mil, sum keep * d_ts, sum keep} over the n instances, keep = 0 for
+ *   an all-zero target, else 1 (d_ts = 0 without a pseudo-label).  For n == 0 out is zeroed.
+ * backward: g_out float[2] on the device = upstream d/d out[0], d/d out[1]; g_logits [n,h,w] of `dtype`, fully
+ *   overwritten: round(g_s * (1 - s) * s) with g_s in float32, exactly 0 for keep = 0.  Pass the inputs of the forward.
+ * workspace: bxs_discobox_loss_workspace_bytes(n,h,w) bytes, written by the forward and read by the backward.
+ * Deterministic (no atomics), no host synchronisation.  BXS_ERR_INVALID_ARG: a NULL pointer, a negative n, a non-positive
+ * h / w, an unknown dtype; BXS_ERR_UNSUPPORTED: h or w above INT32_MAX, or more than INT32_MAX CTAs.  All checks run
+ * before any device call.
+ * --------------------------------------------------------------------------------------- */
+int64_t bxs_discobox_loss_workspace_bytes(int64_t n, int64_t h, int64_t w);
+int bxs_discobox_loss_forward(const void* s_logits, const uint8_t* targets, const uint8_t* pseudo, int dtype,
+                              void* workspace, float* out, int64_t n, int64_t h, int64_t w, bxs_stream_t stream);
+int bxs_discobox_loss_backward(const void* s_logits, const uint8_t* targets, const uint8_t* pseudo, int dtype,
+                               const void* workspace, const float* g_out, void* g_logits, int64_t n, int64_t h,
+                               int64_t w, bxs_stream_t stream);
+
 /* ---------------------------------------------------------------------------------------
  * a12-a15  tree filter      replaces the pybind module tree_filter_cuda
  *     (mmdet/ops/tree_filter/src/tree_filter.cpp:7-13: mst_forward, bfs_forward, refine_forward,
