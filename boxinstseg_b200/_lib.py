@@ -80,8 +80,13 @@ SIGNATURES = {
     'bxs_levelset_fused_forward': [c_p] * 6 + [c_i64] * 4 + [c_f, c_int, c_p],
     'bxs_levelset_fused_backward': [c_p] * 7 + [c_i64] * 4 + [c_f, c_int, c_p],
     'bxs_corr_solve': [c_p, c_p] + [c_i64] * 3 + [c_int] * 3 + [c_p],
+    'bxs_corr_solve_batched': [c_p] * 3 + [c_i64] * 4 + [c_int] * 3 + [c_p],
     'bxs_corr_transfer_workspace_bytes': [c_i64] * 3,
     'bxs_corr_transfer': [c_p] * 7 + [c_i64] * 5 + [c_p],
+    'bxs_corr_transfer_batched': [c_p] * 8 + [c_i64] * 6 + [c_p],
+    'bxs_corr_retrieve': [c_p] * 19 + [c_i64] * 8 + [c_f] * 6 + [c_int] * 2 + [c_p],
+    'bxs_corr_paste': [c_p] * 5 + [c_i64] * 5 + [c_p],
+    'bxs_corr_bank_append': [c_p] * 12 + [c_i64] * 5 + [c_p],
     'bxs_fcos_targets': [c_p] * 7 + [c_i64] * 2 + [c_p] * 5 + [c_int, c_int, c_i64, c_p],
     'bxs_lsap_workspace_bytes': [c_p, c_p, c_i64],
     'bxs_lsap_solve': [c_p] * 4 + [c_i64, c_int] + [c_p] * 4,

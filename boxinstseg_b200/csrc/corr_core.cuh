@@ -193,4 +193,168 @@ BXS_HD void corr_transfer_pixel(const float* t2, float m0q, const float* m1, flo
   *bg_out = bg * scale;
 }
 
+// ---------------------------------------------------------------------------------------------------------------------------
+// corr_retrieve: get_similar_obj (:174-221) for every query object of a level at once, with the order dependence of the
+// reference's per-object loop resolved on the device.  The bank is a packed store of num_class x L slots; object i of the
+// level sees the bank of its class as the objects before it left it: slot s holds the LAST eligible earlier object of this
+// level (same class, ring position (ptr[c] + rank) % L, rank = its index among those objects) that targets s, else the
+// stored slot.  The class has a bank at query time if it had one before the level or an earlier object appended to it.
+//
+// Sources are int32: >= 0 a row of the store (class * L + slot), < 0 the level's own object -(src + 1) (its teacher RoI
+// feature / mask / box, which is what its append stores).  tests/host_harness/corr_retrieve_host.cpp compiles this part for
+// the host.
+// ---------------------------------------------------------------------------------------------------------------------------
+struct CorrBank {
+  const float* feat;        // [num_class * L, C * P]
+  const float* mask;        // [num_class * L, M]
+  const float* box;         // [num_class * L, 4]
+  const int32_t* ptr;       // [num_class] ring write pointer
+  const int32_t* exists;    // [num_class] 1 once the class's first append happened
+  int num_class, L;
+};
+
+struct CorrLevel {
+  const float* q_feat;        // [n, C * P] student RoI features (the query's)
+  const float* q_feat_first;  // [n, C * P] the same re-normalised (create_one :43): used by the first query the head sees
+  const float* q_mask;        // [n, M] student RoI masks
+  const float* t_feat;        // [n, C * P] teacher RoI features (what an append stores)
+  const float* t_mask;        // [n, M]
+  const float* box;           // [n, 4] x1, y1, x2, y2 (integer valued)
+  const int32_t* label;       // [n]
+  const int32_t* valid;       // [n] 0: the object takes no part (all-zero target)
+  int n;
+};
+
+struct CorrRetrieveCfg {
+  int C, h, w, Hm, Wm;
+  float fg_thr, bg_thr, app_thr, ratio_lo, ratio_hi, min_size;
+  int max_objs, min_objs;
+};
+
+// per-query outputs
+struct CorrRetrieveOut {
+  int32_t* src;        // [n, max(max_objs, 1)] the retrieved sources in ascending slot order (0 past `count`)
+  int32_t* count;      // [n] number retrieved (<= max_objs)
+  int32_t* kcount;     // [n] tables the loss uses: count if count >= min_objs, else 0
+  int32_t* slot;       // [n] the slot the object's append writes, -1 when it does not append
+  int32_t* exists;     // [n] the class had a bank at query time
+};
+
+BXS_HD bool corr_live(const CorrLevel& lv, int num_class, int j) {
+  return lv.valid[j] != 0 && lv.label[j] >= 0 && lv.label[j] < num_class;
+}
+
+// :1056-1057 -- an object is appended when both sides of its box exceed min_size
+BXS_HD bool corr_appends(const float* b, float min_size) {
+  return BXS_FSUB(b[2], b[0]) > min_size && BXS_FSUB(b[3], b[1]) > min_size;
+}
+
+// ObjectElements.get_ratio (:103-105)
+BXS_HD float corr_box_ratio(const float* b) {
+  return BXS_FDIV(BXS_FSUB(b[2], b[0]), BXS_FADD(BXS_FSUB(b[3], b[1]), 1e-5f));
+}
+
+// a Hm x Wm mask at cell p of the h x w grid: F.interpolate(bilinear, align_corners=False) (:188-199)
+BXS_HD float corr_mask_small(const float* m, int Hm, int Wm, int h, int w, int p) {
+  const CorrTap ty = corr_tap(p / w, Hm, h), tx = corr_tap(p % w, Wm, w);
+  return ty.l0 * (tx.l0 * m[ty.i0 * Wm + tx.i0] + tx.l1 * m[ty.i0 * Wm + tx.i1]) +
+         ty.l1 * (tx.l0 * m[ty.i1 * Wm + tx.i0] + tx.l1 * m[ty.i1 * Wm + tx.i1]);
+}
+
+constexpr int kCorrSums = 6;   // A*B, [A+B >= 1], (1-A)(1-B), [2-A-B >= 1], f0 f1 a b, a b
+
+// Scratch of one query (shared memory on the device): bytes of corr_retrieve_scratch(L, P).
+BXS_HD int64_t corr_retrieve_scratch(int L, int P) {
+  return (int64_t)4 * (L + 8 + P + (int64_t)L * P + (int64_t)L * kCorrSums * kCorrLanes + L);
+}
+
+// Query i of the level.  All threads of the CTA call it (phases synchronise); the host calls it query by query.
+BXS_HD void corr_retrieve_query(const CorrBank& bk, const CorrLevel& lv, const CorrRetrieveCfg& cf, int first_flag, int i,
+                                void* scratch, const CorrRetrieveOut& out) {
+  const int L = bk.L, P = cf.h * cf.w, M = cf.Hm * cf.Wm, CP = cf.C * P, K = cf.max_objs > 0 ? cf.max_objs : 1;
+  int32_t* src = static_cast<int32_t*>(scratch);     // [L]
+  int32_t* st = src + L;                              // [8]: live, exists, first, slot, count
+  float* a_small = reinterpret_cast<float*>(st + 8);  // [P]
+  float* b_small = a_small + P;                       // [L, P]
+  float* part = b_small + (int64_t)L * P;             // [L, kCorrSums, kCorrLanes]
+  int32_t* pass = reinterpret_cast<int32_t*>(part + (int64_t)L * kCorrSums * kCorrLanes);   // [L]
+  const bool live = corr_live(lv, bk.num_class, i);
+  const int c = live ? lv.label[i] : 0;
+  corr_phase(L, [&](int s) { src[s] = c * L + s; });
+  corr_phase(1, [&](int) {                          // the appends of the earlier objects of this level, in order
+    int rank = 0;
+    bool earlier_live = false;
+    for (int j = 0; j < i; ++j) {
+      if (!corr_live(lv, bk.num_class, j)) continue;
+      earlier_live = true;
+      if (lv.label[j] != c || !corr_appends(lv.box + 4 * j, cf.min_size)) continue;
+      src[(bk.ptr[c] + rank) % L] = -(j + 1);
+      ++rank;
+    }
+    st[0] = live;
+    st[1] = live && (bk.exists[c] != 0 || rank > 0);
+    st[2] = live && first_flag != 0 && !earlier_live;
+    st[3] = live && corr_appends(lv.box + 4 * i, cf.min_size) ? (bk.ptr[c] + rank) % L : -1;
+    out.slot[i] = st[3];
+    out.exists[i] = st[1];
+  });
+  if (!st[1]) {                                     // no bank: nothing retrieved (get_similar_obj returns None)
+    corr_phase(K, [&](int k) { out.src[(int64_t)i * K + k] = 0; });
+    corr_phase(1, [&](int) { out.count[i] = 0; out.kcount[i] = 0; });
+    return;
+  }
+  const float* qf = (st[2] ? lv.q_feat_first : lv.q_feat) + (int64_t)i * CP;
+  const float* qm = lv.q_mask + (int64_t)i * M;
+  auto smask = [&](int s) { const int v = src[s]; return v >= 0 ? bk.mask + (int64_t)v * M : lv.t_mask + (int64_t)(-v - 1) * M; };
+  auto sfeat = [&](int s) { const int v = src[s]; return v >= 0 ? bk.feat + (int64_t)v * CP : lv.t_feat + (int64_t)(-v - 1) * CP; };
+  auto sbox = [&](int s) { const int v = src[s]; return v >= 0 ? bk.box + (int64_t)v * 4 : lv.box + (int64_t)(-v - 1) * 4; };
+  corr_phase(P, [&](int p) { a_small[p] = corr_mask_small(qm, cf.Hm, cf.Wm, cf.h, cf.w, p); });
+  corr_phase(L * P, [&](int e) { b_small[e] = corr_mask_small(smask(e / P), cf.Hm, cf.Wm, cf.h, cf.w, e % P); });
+  // the six sums of every slot, kCorrLanes interleaved partials each (then reduced in lane order: a fixed order)
+  corr_phase(L * kCorrLanes, [&](int e) {
+    const int s = e / kCorrLanes, j = e - s * kCorrLanes;
+    const float* B = smask(s);
+    const float* f1 = sfeat(s);
+    const float* bs = b_small + (int64_t)s * P;
+    float ab = 0.f, un = 0.f, nab = 0.f, nun = 0.f, app = 0.f, den = 0.f;
+    for (int q = j; q < M; q += kCorrLanes) {
+      const float a = qm[q], b = B[q];
+      ab = BXS_FADD(ab, BXS_FMUL(a, b));
+      un = BXS_FADD(un, BXS_FADD(a, b) >= 1.f ? 1.f : 0.f);
+      nab = BXS_FADD(nab, BXS_FMUL(BXS_FSUB(1.f, a), BXS_FSUB(1.f, b)));
+      nun = BXS_FADD(nun, BXS_FSUB(BXS_FSUB(2.f, a), b) >= 1.f ? 1.f : 0.f);
+    }
+    for (int q = j; q < CP; q += kCorrLanes) {
+      const int p = q % P;
+      app = BXS_FADD(app, BXS_FMUL(BXS_FMUL(BXS_FMUL(qf[q], f1[q]), a_small[p]), bs[p]));
+    }
+    for (int p = j; p < P; p += kCorrLanes) den = BXS_FADD(den, BXS_FMUL(a_small[p], bs[p]));
+    float* o = part + (int64_t)s * kCorrSums * kCorrLanes + j;
+    o[0 * kCorrLanes] = ab; o[1 * kCorrLanes] = un; o[2 * kCorrLanes] = nab;
+    o[3 * kCorrLanes] = nun; o[4 * kCorrLanes] = app; o[5 * kCorrLanes] = den;
+  });
+  // the four tests (:205-221).  NaN (0/0 of an all-zero slot) fails every comparison, an infinite ratio fails the upper bound.
+  corr_phase(L, [&](int s) {
+    float v[kCorrSums];
+    for (int t = 0; t < kCorrSums; ++t) {
+      const float* o = part + ((int64_t)s * kCorrSums + t) * kCorrLanes;
+      float acc = o[0];
+      for (int j = 1; j < kCorrLanes; ++j) acc = BXS_FADD(acc, o[j]);
+      v[t] = acc;
+    }
+    const float fg = BXS_FDIV(v[0], v[1]), bg = BXS_FDIV(v[2], v[3]);
+    const float app = BXS_FDIV(v[4], BXS_FADD(v[5], 1e-6f));
+    const float ratio = BXS_FDIV(corr_box_ratio(lv.box + 4 * i), corr_box_ratio(sbox(s)));
+    pass[s] = fg > cf.fg_thr && bg > cf.bg_thr && app > cf.app_thr && ratio >= cf.ratio_lo && ratio <= cf.ratio_hi;
+  });
+  corr_phase(1, [&](int) {                          // ascending slot order, at most max_objs
+    int k = 0;
+    for (int s = 0; s < L && k < cf.max_objs; ++s)
+      if (pass[s]) out.src[(int64_t)i * K + k++] = src[s];
+    for (int r = k; r < K; ++r) out.src[(int64_t)i * K + r] = 0;
+    out.count[i] = k;
+    out.kcount[i] = k >= cf.min_objs ? k : 0;
+  });
+}
+
 }  // namespace bxs

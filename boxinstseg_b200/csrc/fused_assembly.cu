@@ -18,6 +18,7 @@
 #include <algorithm>
 
 #include "common.cuh"
+#include "resize_core.cuh"
 
 namespace cg = cooperative_groups;
 
@@ -27,28 +28,8 @@ namespace {
 constexpr int NT = 256;
 
 // ---------------------------------------------------------------------------------------
-// a18: bilinear resize (ATen UpSample.cuh semantics)
+// a18: bilinear resize (ATen UpSample.cuh semantics; the arithmetic is in resize_core.cuh)
 // ---------------------------------------------------------------------------------------
-__device__ __forceinline__ float rs_scale(int in, int out, bool align) {
-  if (align) return out > 1 ? (float)(in - 1) / (float)(out - 1) : 0.f;
-  return (float)in / (float)out;
-}
-__device__ __forceinline__ float rs_src(float scale, int dst, bool align) {
-  if (align) return scale * (float)dst;
-  const float s = scale * ((float)dst + 0.5f) - 0.5f;
-  return s < 0.f ? 0.f : s;
-}
-struct RsTap { int i0, ip; float l0, l1; };      // first tap, 0/1 offset of the second, weights
-__device__ __forceinline__ RsTap rs_tap(float scale, int dst, int in, bool align) {
-  RsTap t;
-  const float r = rs_src(scale, dst, align);
-  t.i0 = (int)r;
-  t.ip = t.i0 < in - 1 ? 1 : 0;
-  t.l1 = r - (float)t.i0;
-  t.l0 = 1.f - t.l1;
-  return t;
-}
-
 __global__ void __launch_bounds__(NT) resize_fwd_kernel(const float* __restrict__ in, float* __restrict__ out, int64_t NC,
                                                         int h, int w, int H, int W, bool align) {
   const float sh = rs_scale(h, H, align), sw = rs_scale(w, W, align);
@@ -56,10 +37,7 @@ __global__ void __launch_bounds__(NT) resize_fwd_kernel(const float* __restrict_
   for (int64_t i = blockIdx.x * (int64_t)NT + threadIdx.x; i < total; i += (int64_t)gridDim.x * NT) {
     const int ox = (int)(i % W), oy = (int)((i / W) % H);
     const int64_t nc = i / ((int64_t)W * H);
-    const RsTap ty = rs_tap(sh, oy, h, align), tx = rs_tap(sw, ox, w, align);
-    const float* p = in + (nc * h + ty.i0) * w + tx.i0;
-    const float v00 = __ldg(p), v01 = __ldg(p + tx.ip), v10 = __ldg(p + ty.ip * w), v11 = __ldg(p + ty.ip * w + tx.ip);
-    out[i] = ty.l0 * (tx.l0 * v00 + tx.l1 * v01) + ty.l1 * (tx.l0 * v10 + tx.l1 * v11);
+    out[i] = rs_pixel(in + nc * h * w, h, w, sh, sw, oy, ox, align);
   }
 }
 

@@ -2,17 +2,21 @@
 (``ObjectElements`` / ``ObjectQueues`` :69-226), ``SemanticCorrSolver.solve`` (:369-411) and the per-object body of
 ``corr_loss`` (:1059-1125: retrieval, solve, InfoNCE term, transfer of the retrieved masks into the query's box, bank update).
 
-What runs where:
-  * cosine table ``Cu`` (:386-391): normalise + ``torch.matmul`` ([49,C] x [C,49] per retrieved object: a library GEMM, and the
-    only part with a gradient -- to the query's RoI feature);
-  * the regularised table ``T`` (:393-410): ONE launch of ``bxs_corr_solve`` (the reference: ~25 slice-assign / element-wise
-    kernels per round, 10 rounds, per query object);
-  * the transfer (:1086-1096 + ``superres_T`` :851-865): ``bxs_corr_transfer`` -- none of the reference's six [K,784,784]
-    intermediates (12 MB each at K = 5) exists;
-  * resizing the two 28 x 28 maps to the query's box (:1098-1103): the a18 kernel;
-  * the bank: device ring buffers, retrieval tests as a handful of batched reductions; ONE host read per query object (the
-    retrieved indices: the reference's control flow -- ``if kobjs['mask'].shape[0] >= 5`` -- is decided on the host there too,
-    after ~12 implicit synchronisations).
+The reference runs the body object by object; here ALL objects of a level go through it at once (``corr_level``), with the
+same sequential semantics: object i sees the bank exactly as the objects before it -- those of its own level included --
+left it.  A fixed number of launches per level, whatever the number of objects, and no host synchronisation:
+  * retrieval (:174-221) of every query against the virtual bank of its class: ONE launch of ``bxs_corr_retrieve``;
+  * cosine tables ``Cu`` (:386-391) of all (query, retrieved) pairs: gathers + normalise + one batched ``torch.matmul`` (a
+    library GEMM, and the only part with a gradient -- to the queries' RoI features);
+  * the regularised tables ``T`` (:393-410): ONE launch of ``bxs_corr_solve`` over the level's n x max_retrieval_objs tables
+    (the unused ones cost nothing);
+  * the InfoNCE terms (:1080-1084): batched, masked per query; the count ``num`` stays on the device;
+  * the transfer (:1086-1096 + ``superres_T`` :851-865): ONE launch pair of ``bxs_corr_transfer`` -- none of the reference's
+    six [K,784,784] intermediates (12 MB each at K = 5) exists;
+  * resizing the two 28 x 28 maps to each query's box and writing them into ``iiu`` (:1098-1107): ``bxs_corr_paste``;
+  * the ring append (:1113-1124): ``bxs_corr_bank_append``.
+The bank is ONE packed device store per ``ObjectQueues`` (feature / mask / box of every (class, slot), int32 ``ptr`` and
+``exists`` per class); the head's "first query" state (:1060-1066) is a device flag too.
 
 Third party and absent from the reference checkout: ``mmcv.ops.RoIAlign`` -- the RoI features / masks are inputs here
 (``torchvision.ops.roi_align(x, rois, size, 1.0, 0, True)`` is the same operator).
@@ -21,7 +25,6 @@ import torch
 import torch.nn.functional as F
 
 from ... import _lib as L
-from ...ops.resize import bilinear_resize
 
 
 def relu_and_l2_norm_feat(feat, dim=1):
@@ -79,34 +82,119 @@ def create_one(mask, feature, box, category):
     return q
 
 
+class _BankView(ObjectElements):
+    """Class c of a packed store as an ``ObjectElements``: ``feature`` / ``mask`` / ``box`` are views of the store's rows
+    [c*L, (c+1)*L); ``ptr`` reads (synchronises) and writes the store's device pointer."""
+
+    def __init__(self, queues, c):                       # noqa -- no slot allocation: the store owns the memory
+        rows = slice(c * queues.len_queue, (c + 1) * queues.len_queue)
+        self._queues = queues
+        self.feature, self.mask, self.box = queues.feature[rows], queues.mask[rows], queues.box[rows]
+        self.img = None
+        self.category = int(c)
+
+    @property
+    def ptr(self):
+        return int(self._queues.ptr[self.category])
+
+    @ptr.setter
+    def ptr(self, value):
+        self._queues.ptr[self.category] = int(value)
+
+
+class _BankList:
+    """``ObjectQueues.queues``: ``queues[c]`` is None until class c has a bank (a read of the device ``exists`` flag:
+    synchronises -- for inspection), else a ``_BankView``; assigning an ``ObjectElements`` loads it into the store, assigning
+    None drops the class's bank."""
+
+    def __init__(self, queues):
+        self._q = queues
+
+    def __len__(self):
+        return self._q.num_class
+
+    def __getitem__(self, c):
+        q = self._q
+        if not -q.num_class <= c < q.num_class:
+            raise IndexError(c)
+        c %= q.num_class
+        if q.feature is None or not bool(q.exists[c]):
+            return None
+        return _BankView(q, c)
+
+    def __setitem__(self, c, elems):
+        self._q.load(c % self._q.num_class, elems)
+
+    def __iter__(self):
+        return (self[c] for c in range(len(self)))
+
+
 class ObjectQueues:
-    """:132-226, same constructor arguments.  All banks live on the device (the reference spills to host memory after
-    ``num_gpu_bank`` classes: 80 classes x 100 slots x (128 x 7 x 7 + 28 x 28) floats = 226 MB -- nothing on a 180 GB part)."""
+    """:132-226, same constructor arguments.  ONE packed store for all classes: ``feature`` [num_class*L,C,fh,fw], ``mask``
+    [num_class*L,mh,mw], ``box`` [num_class*L,4] (class c owns rows [c*L, (c+1)*L)), int32 ``ptr`` / ``exists``
+    [num_class]; allocated (zeros) on the first use, from the feature / mask shapes and the device it sees there.  The
+    reference keeps one holder per class and spills to host memory after ``num_gpu_bank`` classes: 80 classes x 100 slots x
+    (128 x 7 x 7 + 28 x 28) floats = 226 MB here, all on the device."""
 
     def __init__(self, num_class, len_queue, fg_iou_thresh, bg_iou_thresh, ratio_range, appear_thresh, max_retrieval_objs):
         self.num_class = num_class
-        self.queues = [None] * num_class
         self.len_queue = len_queue
         self.fg_iou_thresh = fg_iou_thresh
         self.bg_iou_thresh = bg_iou_thresh
         self.appear_thresh = appear_thresh
         self.ratio_range = ratio_range
         self.max_retrieval_objs = max_retrieval_objs
+        self.feature = self.mask = self.box = self.ptr = self.exists = None
+        self.queues = _BankList(self)
+
+    def allocate(self, n_channel, feat_hw, mask_hw, device):
+        """The store for features [n_channel, *feat_hw] and masks [*mask_hw] on ``device`` (zeros); a no-op when it exists
+        with these shapes.  No data-dependent step: callable before anything is known about the objects."""
+        feat_hw, mask_hw, device = tuple(int(v) for v in feat_hw), tuple(int(v) for v in mask_hw), torch.device(device)
+        if self.feature is not None:
+            if (self.feature.shape[1:] != (n_channel,) + feat_hw or self.mask.shape[1:] != mask_hw or
+                    self.feature.device != device):
+                raise ValueError(f'object bank holds {tuple(self.feature.shape[1:])} / {tuple(self.mask.shape[1:])} features / '
+                                 f'masks on {self.feature.device}, got {(n_channel,) + feat_hw} / {mask_hw} on {device}')
+            return
+        rows = self.num_class * self.len_queue
+        self.feature = torch.zeros((rows, n_channel) + feat_hw, device=device)
+        self.mask = torch.zeros((rows,) + mask_hw, device=device)
+        self.box = torch.zeros(rows, 4, device=device)
+        self.ptr = torch.zeros(self.num_class, dtype=torch.int32, device=device)
+        self.exists = torch.zeros(self.num_class, dtype=torch.int32, device=device)
+
+    @torch.no_grad()
+    def load(self, c, elems):
+        """Class c's bank := ``elems`` (an ``ObjectElements`` of ``len_queue`` slots, its ``ptr`` included); None drops it."""
+        if elems is None:
+            if self.exists is not None:
+                self.exists[c] = 0
+                self.ptr[c] = 0
+            return
+        if len(elems) != self.len_queue:
+            raise ValueError(f'a bank has {self.len_queue} slots, got {len(elems)}')
+        self.allocate(elems.feature.shape[1], elems.feature.shape[2:], elems.mask.shape[1:], elems.mask.device)
+        rows = slice(c * self.len_queue, (c + 1) * self.len_queue)
+        self.feature[rows] = elems.feature
+        self.mask[rows] = elems.mask
+        self.box[rows] = elems.box
+        self.ptr[c] = int(elems.ptr)
+        self.exists[c] = 1
 
     @torch.no_grad()
     def append(self, class_idx, idx, feature, mask, box, img=None, device=None):
         """:146-172: entry ``idx`` of the three batched tensors goes to the class's write pointer.  True when the bank was
-        created by this call."""
-        created = self.queues[class_idx] is None
-        if created:
-            self.queues[class_idx] = ObjectElements(size=self.len_queue, feat_size=feature.shape[2], mask_size=mask.shape[1],
-                                                    n_channel=feature.shape[1], device=device or mask.device,
-                                                    category=class_idx)
-        q = self.queues[class_idx]
-        q.feature[q.ptr] = feature[idx]
-        q.mask[q.ptr] = mask[idx]
-        q.box[q.ptr] = box[idx]
-        q.ptr = (q.ptr + 1) % self.len_queue
+        created by this call.  One object at a time, reading the pointer on the host (the batched path is ``corr_level``)."""
+        self.allocate(feature.shape[1], feature.shape[2:], mask.shape[1:], device or mask.device)
+        created = not bool(self.exists[class_idx])
+        p = int(self.ptr[class_idx])
+        row = class_idx * self.len_queue + p
+        self.feature[row] = feature[idx]
+        self.mask[row] = mask[idx]
+        self.box[row] = box[idx]
+        self.ptr[class_idx] = (p + 1) % self.len_queue
+        self.exists[class_idx] = 1
         return created
 
     @torch.no_grad()
@@ -149,23 +237,30 @@ class SemanticCorrSolver:
 
     def cosine_table(self, f0, f1):
         """:386-391: f0 [1,C,h,w], f1 [K,C,h,w] -> Cu [K,P,P] (differentiable w.r.t. f0)."""
-        a = f0.float().reshape(f0.shape[0], f0.shape[1], -1).transpose(2, 1)
-        b = f1.float().reshape(f1.shape[0], f1.shape[1], -1)
-        a = a / (torch.norm(a, p=2, dim=2, keepdim=True) + 1e-4)
-        b = b / (torch.norm(b, p=2, dim=1, keepdim=True) + 1e-4)
+        return self.cosine_tables(f0, f1[None])[0]
+
+    def cosine_tables(self, f0, f1):
+        """:386-391 for n queries at once: f0 [n,C,h,w], f1 [n,K,C,h,w] -> Cu [n,K,P,P] (differentiable w.r.t. f0)."""
+        a = f0.float().reshape(f0.shape[0], 1, f0.shape[1], -1).transpose(3, 2)                        # [n,1,P,C]
+        b = f1.float().reshape(f1.shape[0], f1.shape[1], f1.shape[2], -1)                                # [n,K,C,P]
+        a = a / (torch.norm(a, p=2, dim=3, keepdim=True) + 1e-4)
+        b = b / (torch.norm(b, p=2, dim=2, keepdim=True) + 1e-4)
         with torch.autocast('cuda', enabled=False):
             return torch.matmul(a, b)
 
     @torch.no_grad()
-    def votes(self, Cu, h, w):
+    def votes(self, Cu, h, w, counts=None):
         """:393-410: the regularised table for a given Cu [K,P,P] (one launch).  No gradient: the reference uses T only
-        through argmax and inside no_grad (:1081,1086-1088)."""
+        through argmax and inside no_grad (:1081,1086-1088).  With ``counts`` (int32 [n], K = n * kmax), table j of query q
+        is solved only for j < counts[q]; the others are zeros."""
         Cu = Cu.detach().contiguous().float()
-        L.require_cuda(Cu)
+        L.require_cuda(Cu, counts)
         T = torch.empty_like(Cu)
+        n = counts.shape[0] if counts is not None else 1
         with torch.cuda.device(Cu.device):
-            L.check(L.lib().bxs_corr_solve(L.ptr(Cu), L.ptr(T), Cu.shape[0], h, w, int(self.dist_kernel), int(self.num_iter),
-                                           int(self.num_smooth_iter), L.stream()), 'corr_solve')
+            L.check(L.lib().bxs_corr_solve_batched(L.ptr(Cu), L.ptr(T), L.ptr(counts), n, Cu.shape[0] // n, h, w,
+                                                   int(self.dist_kernel), int(self.num_iter), int(self.num_smooth_iter),
+                                                   L.stream()), 'corr_solve')
         return T
 
     def solve(self, qobjs, kobjs, f0, return_masks=False):
@@ -185,57 +280,119 @@ class SemanticCorrSolver:
     @torch.no_grad()
     def transfer(self, T, Cu, qmask, kmask, h, w):
         """:1086-1096 + superres_T: T, Cu [K,P,P], qmask [1,Hm,Wm], kmask [K,Hm,Wm] -> (fg_ci, bg_ci) [Hm,Wm]."""
+        fg, bg = self.transfer_batched(T, Cu, qmask, kmask, h, w)
+        return fg[0], bg[0]
+
+    @torch.no_grad()
+    def transfer_batched(self, T, Cu, qmask, kmask, h, w, counts=None):
+        """The transfer for n queries in one launch pair: T, Cu [n*kmax,P,P], qmask [n,Hm,Wm], kmask [n*kmax,Hm,Wm], counts
+        int32 [n] (None: kmax tables each) -> (fg_ci, bg_ci) [n,Hm,Wm], the mean over each query's counts[q] tables (zeros
+        for a query without any)."""
         T, Cu = T.contiguous().float(), Cu.detach().contiguous().float()
         m0, m1 = qmask.detach().contiguous().float(), kmask.detach().contiguous().float()
-        L.require_cuda(T, Cu, m0, m1)
-        K, Hm, Wm = m1.shape
-        fg = torch.empty((Hm, Wm), dtype=torch.float32, device=T.device)
+        L.require_cuda(T, Cu, m0, m1, counts)
+        n, (K, Hm, Wm) = m0.shape[0], m1.shape
+        fg = torch.empty((n, Hm, Wm), dtype=torch.float32, device=T.device)
         bg = torch.empty_like(fg)
         lib = L.lib()
         ws = torch.empty(lib.bxs_corr_transfer_workspace_bytes(K, Hm, Wm), dtype=torch.uint8, device=T.device)
         with torch.cuda.device(T.device):
-            L.check(lib.bxs_corr_transfer(L.ptr(T), L.ptr(Cu), L.ptr(m0), L.ptr(m1), L.ptr(fg), L.ptr(bg), L.ptr(ws), K, h, w,
-                                          Hm, Wm, L.stream()), 'corr_transfer')
+            L.check(lib.bxs_corr_transfer_batched(L.ptr(T), L.ptr(Cu), L.ptr(m0), L.ptr(m1), L.ptr(counts), L.ptr(fg),
+                                                  L.ptr(bg), L.ptr(ws), n, K // n, h, w, Hm, Wm, L.stream()), 'corr_transfer')
         return fg, bg
+
+
+def corr_level(solver, queues, first, roi_s_feat, roi_t_feat, roi_s_mask, roi_t_mask, boxes, labels, valid, iiu, min_size,
+               min_objs=5):
+    """The per-object body of ``corr_loss`` (:1056-1125) for ALL n objects of one level, with the reference's sequential
+    semantics, on the device and without host synchronisation (a fixed number of launches for any n).
+
+    roi_s_feat [n,C,h,w] (student RoI features, normalised, carries the gradient), roi_t_feat / roi_s_mask / roi_t_mask
+    (detached RoI tensors), boxes [n,4] (x1,y1,x2,y2 on the mask-feature grid, integer valued), labels [n], valid [n] bool
+    (False: the object takes no part -- an all-zero target), iiu [2n,H,W] zeros, first: the head's int32 [1] device flag
+    "no query seen yet" (consumed by the first valid object).  Object i:
+      1. retrieves from the bank of its class as the objects before it left it (``bxs_corr_retrieve``);
+      2. with >= min_objs retrieved: adds its InfoNCE term, transfers the retrieved masks and pastes them over its box into
+         iiu[2i] (background) / iiu[2i+1] (foreground);
+      3. appends its teacher RoI feature / mask and box when both box sides exceed min_size (``bxs_corr_bank_append``).
+    Returns (sum of the InfoNCE terms, number of terms as a device int32 scalar, the retrieval record: dict of int32 src
+    [n,kmax], count, kcount, slot, exists [n] -- see include/boxseg_b200.h, bxs_corr_retrieve)."""
+    n, C, h, w = roi_s_feat.shape
+    Hm, Wm = roi_s_mask.shape[1:]
+    H, W = iiu.shape[1:]
+    dev = roi_s_feat.device
+    queues.allocate(C, (h, w), (Hm, Wm), dev)
+    if n == 0:
+        none = torch.empty(0, dtype=torch.int32, device=dev)
+        return roi_s_feat.new_zeros(()), none.sum(dtype=torch.int32), dict(src=none.view(0, 1), count=none, kcount=none,
+                                                                           slot=none, exists=none)
+    kmax = max(int(queues.max_retrieval_objs), 1)
+    P = h * w
+    qf = roi_s_feat.detach().float().contiguous()
+    qf_first = relu_and_l2_norm_feat(qf).contiguous()                   # ObjectFactory.create_one (:43)
+    tf = roi_t_feat.detach().float().contiguous()
+    sm, tm = roi_s_mask.detach().float().contiguous(), roi_t_mask.detach().float().contiguous()
+    bx = boxes.detach().float().contiguous()
+    lab, val = labels.to(torch.int32).contiguous(), valid.to(torch.int32).contiguous()
+    L.require_cuda(qf, tf, sm, tm, bx, lab, val, iiu, first, queues.feature)
+    src = torch.empty((n, kmax), dtype=torch.int32, device=dev)
+    count, kcount, slot, exists = torch.empty((4, n), dtype=torch.int32, device=dev).unbind(0)
+    lib = L.lib()
+    with torch.cuda.device(dev):
+        L.check(lib.bxs_corr_retrieve(
+            L.ptr(queues.feature), L.ptr(queues.mask), L.ptr(queues.box), L.ptr(queues.ptr), L.ptr(queues.exists), L.ptr(first),
+            L.ptr(qf), L.ptr(qf_first), L.ptr(sm), L.ptr(tf), L.ptr(tm), L.ptr(bx), L.ptr(lab), L.ptr(val), L.ptr(src),
+            L.ptr(count), L.ptr(kcount), L.ptr(slot), L.ptr(exists), n, queues.num_class, queues.len_queue, C, h, w, Hm, Wm,
+            float(queues.fg_iou_thresh), float(queues.bg_iou_thresh), float(queues.appear_thresh),
+            float(queues.ratio_range[0]), float(queues.ratio_range[1]), float(min_size), int(queues.max_retrieval_objs),
+            int(min_objs), L.stream()), 'corr_retrieve')
+    # the retrieved objects: rows of the store, or this level's own appended objects (their teacher RoI tensors)
+    own = (src < 0).reshape(-1)
+    bank_row = torch.where(own, 0, src.reshape(-1)).long()
+    lvl_row = torch.where(own, -1 - src.reshape(-1), 0).long()
+    f1 = torch.where(own[:, None], tf.reshape(n, -1).index_select(0, lvl_row),
+                     queues.feature.reshape(queues.feature.shape[0], -1).index_select(0, bank_row))
+    m1 = torch.where(own[:, None], tm.reshape(n, -1).index_select(0, lvl_row),
+                     queues.mask.reshape(queues.mask.shape[0], -1).index_select(0, bank_row))
+    Cu = solver.cosine_tables(roi_s_feat, f1.view(n, kmax, C, h, w))                 # [n,kmax,P,P]
+    T = solver.votes(Cu.reshape(n * kmax, P, P), h, w, counts=kcount)
+    # :1080-1084 -- cross entropy of softmax(Cu) against argmax(T), the mean over the K_i * P rows of each query
+    asg = T.view(n, kmax, P, P).argmax(3, keepdim=True)
+    ce = -F.log_softmax(F.softmax(Cu.float(), 3), 3).gather(3, asg)[..., 0]        # [n,kmax,P]
+    used = torch.arange(kmax, device=dev)[None, :] < kcount[:, None]                 # [n,kmax]
+    per_query = torch.where(used[..., None], ce, 0).sum((1, 2)) / (kcount.clamp(min=1) * P)
+    loss = per_query.sum()
+    num = (kcount > 0).sum(dtype=torch.int32)
+    fg, bg = solver.transfer_batched(T, Cu, sm, m1.view(n * kmax, Hm, Wm), h, w, counts=kcount)
+    with torch.cuda.device(dev):
+        L.check(lib.bxs_corr_paste(L.ptr(fg), L.ptr(bg), L.ptr(bx), L.ptr(kcount), L.ptr(iiu), n, Hm, Wm, H, W, L.stream()),
+                'corr_paste')
+        L.check(lib.bxs_corr_bank_append(L.ptr(queues.feature), L.ptr(queues.mask), L.ptr(queues.box), L.ptr(queues.ptr),
+                                         L.ptr(queues.exists), L.ptr(first), L.ptr(tf), L.ptr(tm), L.ptr(bx), L.ptr(lab),
+                                         L.ptr(val), L.ptr(slot), n, queues.num_class, queues.len_queue, C * P, Hm * Wm,
+                                         L.stream()), 'corr_bank_append')
+    return loss, num, dict(src=src, count=count, kcount=kcount, slot=slot, exists=exists)
 
 
 def corr_objects(solver, queues, qobj, roi_s_feat, roi_t_feat, roi_s_mask, roi_t_mask, boxes, kernel_labels, iiu,
                  objbank_min_size, min_objs=5):
-    """The per-object loop of ``corr_loss`` (:1056-1125) for the n objects of one level.
+    """The per-object loop of ``corr_loss`` (:1056-1125) for the n objects of one level, all of them valid: ``corr_level``
+    with a host count.
 
     roi_s_feat [n,C,h,w] (student RoI features, normalised, carries the gradient), roi_t_feat / roi_s_mask / roi_t_mask
     (detached RoI tensors), boxes [n,4] (x1,y1,x2,y2 on the mask-feature grid, integer valued), kernel_labels [n], iiu
-    [2n,H,W] zeros.  Returns (sum of the InfoNCE terms, number of terms, qobj); fills ``iiu`` and updates the bank.
-    ``qobj`` is the head's one-slot query holder (None on the first call, :1060-1066)."""
+    [2n,H,W] zeros.  Returns (sum of the InfoNCE terms, number of terms (a host int: synchronises), qobj); fills ``iiu`` and
+    updates the bank.  ``qobj`` is the head's one-slot query holder (None on the first call, :1060-1066)."""
     n = roi_s_feat.shape[0]
-    box_l = [[int(v) for v in b] for b in boxes.tolist()]                 # ONE host read for all boxes of the level
-    labels = [int(v) for v in kernel_labels.tolist()]
-    loss = roi_s_feat.new_zeros(())
-    num = 0
-    h, w = roi_s_feat.shape[2:]
-    for i in range(n):
-        x1, y1, x2, y2 = box_l[i]
-        if qobj is None:
-            qobj = create_one(roi_s_mask[i:i + 1].detach(), roi_s_feat[i:i + 1].detach(), boxes[i:i + 1].detach(), labels[i])
-        else:                                                             # :1067-1071 (no re-normalisation there)
-            qobj.mask[...] = roi_s_mask[i:i + 1].detach()
-            qobj.feature[...] = roi_s_feat[i:i + 1].detach()
-            qobj.box[...] = boxes[i:i + 1].detach()
-            qobj.category = labels[i]
-        idx = queues.similar_indices(qobj)
-        if idx is not None and idx.numel() >= min_objs:                   # the host decision of :1075 (one read)
-            kobjs = queues.queues[labels[i]][idx]
-            Cu, T, _, _ = solver.solve(qobj, kobjs, roi_s_feat[i:i + 1])
-            assignment = T.argmax(2).reshape(-1)                          # :1081-1084
-            loss = loss + F.cross_entropy(F.softmax(Cu.float(), 2).reshape(-1, Cu.shape[2]), assignment)
-            num += 1
-            fg, bg = solver.transfer(T, Cu, qobj.mask, kobjs['mask'], h, w)
-            if y2 > y1 and x2 > x1:                                       # :1098-1107
-                iiu[2 * i, y1:y2, x1:x2] = bilinear_resize(bg[None, None], (y2 - y1, x2 - x1))[0, 0]
-                iiu[2 * i + 1, y1:y2, x1:x2] = bilinear_resize(fg[None, None], (y2 - y1, x2 - x1))[0, 0]
-        if (x2 - x1) > objbank_min_size and (y2 - y1) > objbank_min_size:   # :1056-1057, 1113-1124
-            queues.append(labels[i], i, roi_t_feat, roi_t_mask, boxes.detach())
-    return loss, num, qobj
+    dev = roi_s_feat.device
+    first = torch.full((1,), int(qobj is None), dtype=torch.int32, device=dev)
+    valid = torch.ones(n, dtype=torch.bool, device=dev)
+    loss, num, _ = corr_level(solver, queues, first, roi_s_feat, roi_t_feat, roi_s_mask, roi_t_mask, boxes, kernel_labels,
+                              valid, iiu, objbank_min_size, min_objs)
+    if qobj is None and n > 0:                                           # the holder of the last query, like the reference's
+        qobj = create_one(roi_s_mask[n - 1:].detach(), roi_s_feat[n - 1:].detach(), boxes[n - 1:].detach(),
+                          int(kernel_labels[n - 1]))
+    return loss, int(num), qobj
 
 
 def _torchvision_roi_align(out_size):
@@ -265,9 +422,10 @@ def mask_boxes(target):
 
 class DiscoCorr:
     """The state and the per-level body of ``DiscoBoxSOLOv2Head.corr_loss`` (:900-1139) after the dynamic convolutions: per
-    level, drop the empty targets, box every target, RoI-align the student / teacher features and masks, run the per-object
-    loop (``corr_objects``), then the mean field WITH the transferred inter-image maps and the dice against its pseudo labels.
-    Built from the head's ``loss_corr`` config dict (:720-749)."""
+    level, box every target, RoI-align the student / teacher features and masks, run the per-object body for all objects at
+    once (``corr_level``), then the mean field WITH the transferred inter-image maps and the dice against its pseudo labels.
+    Objects with an all-zero target (which the reference drops, :1024-1028) stay in the level with a placeholder box and take
+    no part in anything.  Built from the head's ``loss_corr`` config dict (:720-749)."""
 
     def __init__(self, num_classes, loss_corr, roi_align=_torchvision_roi_align):
         bank = loss_corr['obj_bank']
@@ -280,34 +438,52 @@ class DiscoCorr:
                                           max_retrieval_objs=bank['max_retrieval_objs'])
         self.feat_roi_align = roi_align((bank['feat_height'], bank['feat_width']))
         self.mask_roi_align = roi_align((bank['mask_height'], bank['mask_width']))
+        self.feat_hw = (bank['feat_height'], bank['feat_width'])
+        self.mask_hw = (bank['mask_height'], bank['mask_width'])
         self.objbank_min_size = bank['min_size']
         self.min_objs = 5                                                    # the literal of :1075
         self.corr_loss_weight = loss_corr['loss_weight']
-        self.qobj = None
+        self.first = None              # int32 [1] on the device: no query seen yet (the reference's ``qobj is None``)
+        self._qobj = None
 
-    def levels(self, s_ins_pred_list, t_ins_pred_list, img_ind_list, ins_labels, kernel_label_list, s_feat, t_feat, mean_field,
-               use_ind_teacher=False):
-        """Per level l: s_ins_pred_list[l] [n,H,W] student mask LOGITS (None: no object), t_ins_pred_list[l] the teacher's
-        (ignored unless use_ind_teacher), img_ind_list[l] [n], ins_labels[l] [n,H,W] targets, kernel_label_list[l] [n];
-        s_feat / t_feat [B,C,H,W]; mean_field: ONE ``MeanField`` over the batch's colour features (``obj_img`` selects the
-        image; the reference keeps one module per image).  Returns (corr_loss / (num + 1e-4), [per-level dice terms [n_l]])."""
+    @property
+    def qobj(self):
+        """The reference's query holder: None until the first query (reads the device flag: synchronises; inspection only)."""
+        first = self._qobj is None if self.first is None else bool(self.first.item())
+        return None if first else (self._qobj if self._qobj is not None else True)
+
+    @qobj.setter
+    def qobj(self, value):
+        self._qobj = value
+        if self.first is not None:
+            self.first.fill_(int(value is None))
+
+    def _state(self, s_feat):
+        """The bank store and the first-query flag on s_feat's device (allocated on the first call: run one call eagerly
+        before capturing this in a CUDA graph)."""
+        self.object_queues.allocate(s_feat.shape[1], self.feat_hw, self.mask_hw, s_feat.device)
+        if self.first is None:
+            self.first = torch.full((1,), int(self._qobj is None), dtype=torch.int32, device=s_feat.device)
+
+    def levels_masked(self, s_ins_pred_list, t_ins_pred_list, img_ind_list, ins_labels, kernel_label_list, s_feat, t_feat,
+                      mean_field, use_ind_teacher=False):
+        """``levels`` without host synchronisation: returns (corr_loss / (num + 1e-4), [(dice terms [n_l], valid [n_l] bool)
+        per level with objects]); the terms of objects with an all-zero target are 0 and not valid."""
+        self._state(s_feat)
         total = s_feat.new_zeros(())
-        num = 0
-        loss_ts = []
+        num = torch.zeros((), dtype=torch.int32, device=s_feat.device)
+        out = []
         for s_in, t_in, img_inds, target, klabels in zip(s_ins_pred_list, t_ins_pred_list, img_ind_list, ins_labels,
                                                          kernel_label_list):
             if s_in is None or s_in.shape[0] == 0:
                 continue
-            keep = (target.flatten(1) != 0).any(1).nonzero().flatten()       # remove all-zero targets (:1024-1028); one sync
-            if keep.numel() == 0:
-                continue
-            s = torch.sigmoid(s_in).index_select(0, keep)
-            t = torch.sigmoid(t_in).index_select(0, keep) if use_ind_teacher else s
-            img_inds = img_inds.to(s.device).index_select(0, keep)
-            target = target.index_select(0, keep)
-            klabels = klabels.index_select(0, keep)
+            valid = (target.flatten(1) != 0).any(1)                           # the reference drops the others (:1024-1028)
+            s = torch.sigmoid(s_in)
+            t = torch.sigmoid(t_in) if use_ind_teacher else s
+            img_inds = img_inds.to(s.device)
             n = s.shape[0]
-            boxes = mask_boxes(target)
+            placeholder = (torch.arange(4, device=s.device) >= 2).float()     # (0, 0, 1, 1): RoIAlign of an empty target
+            boxes = torch.where(valid[:, None], mask_boxes(target), placeholder)
             rois = torch.cat([img_inds.to(s_feat)[:, None], boxes], 1)
             roi_s_feat = relu_and_l2_norm_feat(self.feat_roi_align(s_feat, rois))
             with torch.no_grad():
@@ -315,18 +491,32 @@ class DiscoCorr:
                 own = torch.cat([torch.arange(n, device=s.device).to(s)[:, None], boxes], 1)
                 roi_s_mask = self.mask_roi_align(s.detach()[:, None], own)[:, 0]
                 roi_t_mask = self.mask_roi_align(t.detach()[:, None], own)[:, 0]
-                iiu = s.new_zeros((2 * n,) + tuple(s.shape[1:]))
-            lvl_loss, lvl_num, self.qobj = corr_objects(self.solver, self.object_queues, self.qobj, roi_s_feat, roi_t_feat,
-                                                        roi_s_mask, roi_t_mask, boxes, klabels, iiu, self.objbank_min_size,
-                                                        self.min_objs)
+                iiu = torch.zeros((2 * n,) + tuple(s.shape[1:]), dtype=torch.float32, device=s.device)
+            lvl_loss, lvl_num, _ = corr_level(self.solver, self.object_queues, self.first, roi_s_feat, roi_t_feat, roi_s_mask,
+                                              roi_t_mask, boxes, klabels, valid, iiu, self.objbank_min_size, self.min_objs)
             total = total + lvl_loss
-            num += lvl_num
+            num = num + lvl_num
             iiu = iiu.view(n, 2, *iiu.shape[1:])
             tf = target.float()
             enlarged = F.max_pool2d(tf[:, None], kernel_size=3, stride=1, padding=1)[:, 0]                  # :1128
             pseudo, _ = mean_field(((t + s) / 2)[:, None], tf[:, None], iiu, obj_img=img_inds)              # :1130-1132
             cropped = s * enlarged
             cropped = cropped * mean_field.gamma + cropped.detach() * (1 - mean_field.gamma)                # :1134
-            x, p = cropped.flatten(1).float(), pseudo.flatten(1).float()                                    # dice_loss :542-550
-            loss_ts.append(1 - 2 * (x * p).sum(1) / ((x * x).sum(1) + 0.001 + (p * p).sum(1) + 0.001))
-        return total / (num + 1e-4), loss_ts
+            x = cropped.flatten(1).float()                                                                  # dice_loss :542-550
+            p = torch.where(valid[:, None], pseudo.flatten(1).float(), 0)
+            ts = 1 - 2 * (x * p).sum(1) / ((x * x).sum(1) + 0.001 + (p * p).sum(1) + 0.001)
+            out.append((torch.where(valid, ts, 0), valid))
+        return total / (num + 1e-4), out
+
+    def levels(self, s_ins_pred_list, t_ins_pred_list, img_ind_list, ins_labels, kernel_label_list, s_feat, t_feat, mean_field,
+               use_ind_teacher=False):
+        """Per level l: s_ins_pred_list[l] [n,H,W] student mask LOGITS (None: no object), t_ins_pred_list[l] the teacher's
+        (ignored unless use_ind_teacher), img_ind_list[l] [n], ins_labels[l] [n,H,W] targets, kernel_label_list[l] [n];
+        s_feat / t_feat [B,C,H,W]; mean_field: ONE ``MeanField`` over the batch's colour features (``obj_img`` selects the
+        image; the reference keeps one module per image).  Returns (corr_loss / (num + 1e-4), [per-level dice terms [n_l] of
+        the objects with a non-empty target]).  Compacting those lists costs one host synchronisation per level;
+        ``levels_masked`` returns the same without it."""
+        loss, per_level = self.levels_masked(s_ins_pred_list, t_ins_pred_list, img_ind_list, ins_labels, kernel_label_list,
+                                             s_feat, t_feat, mean_field, use_ind_teacher)
+        kept = [ts[valid] for ts, valid in per_level]
+        return loss, [k for k in kept if k.numel()]

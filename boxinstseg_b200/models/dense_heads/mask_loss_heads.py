@@ -171,14 +171,21 @@ class DiscoBoxSOLOv2Head(nn.Module):
         """The part of ``corr_loss`` after the dynamic convolutions (per-level lists as ``mask_loss`` takes them, plus the
         class of every object and the student / teacher feature maps [B,C,H,W]).  Returns (loss_corr * weight,
         mean of the correspondence-aware teacher-student dice terms) -- what ``loss`` adds to ``loss_corr`` / ``loss_ts``
-        (:1329-1337).  Stateful: the object bank of ``self.corr`` is updated."""
+        (:1329-1337).  Stateful: the object bank of ``self.corr`` is updated.  No host synchronisation (after one eager call,
+        which allocates the bank, it can be captured in a CUDA graph)."""
         if self.corr is None:
             raise RuntimeError('DiscoBoxSOLOv2Head was built without loss_corr')
         mf = MeanField(color_feats, alpha0=self.alpha0, theta0=self.theta0, theta1=self.theta1, theta2=self.theta2,
                        iter=self.crf_max_iter, kernel_size=self.mkernel, base=self.crf_base, gamma=gamma)
-        loss, ts = self.corr.levels(s_ins_pred_list, t_ins_pred_list or [None] * len(s_ins_pred_list), img_ind_list,
-                                    ins_labels, kernel_label_list, s_feat, t_feat, mf, use_ind_teacher)
-        ts_mean = torch.cat(ts).mean() if ts else loss.new_zeros(())
+        loss, per_level = self.corr.levels_masked(s_ins_pred_list, t_ins_pred_list or [None] * len(s_ins_pred_list),
+                                                  img_ind_list, ins_labels, kernel_label_list, s_feat, t_feat, mf,
+                                                  use_ind_teacher)
+        if per_level:                                   # the mean over the objects with a non-empty target
+            total = sum(ts.sum() for ts, _ in per_level)
+            count = sum(valid.sum() for _, valid in per_level)
+            ts_mean = total / count.clamp(min=1)
+        else:
+            ts_mean = loss.new_zeros(())
         return loss * self.corr.corr_loss_weight, ts_mean
 
     def _grid_cfg(self):

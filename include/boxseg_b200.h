@@ -448,17 +448,61 @@ int bxs_fcos_targets(const float* points, const float* gt_boxes, const int64_t* 
  * bxs_corr_solve: Cu f32 [K,P,P] (cosine similarities of the query cells x the cells of K retrieved objects,
  *   P = h*w) -> T [K,P,P]: C = Cu * window(dist_kernel), then num_iter x { votes = C; num_smooth x (pass_message,
  *   rows /= sum + 1e-4); C = Cu + votes; rows /= sum + 1e-4 }.  One CTA per object, state in shared memory;
- *   dist_kernel odd; (2 P^2 + 9 P) * 4 bytes <= 200 KB (P <= 156).
+ *   dist_kernel odd; (2 P^2 + 9 P) * 4 bytes <= 200 KB (P <= 156); K <= 65535.
+ * bxs_corr_solve_batched: the same for n queries of kmax tables each (Cu, T [n*kmax,P,P]); counts i32 [n] (NULL: all):
+ *   table j of query q is solved only when j < counts[q], the others are zero-filled (and cost no solve).
  * bxs_corr_transfer: T, Cu [K,P,P], m0 f32 [Hm*Wm] (query RoI mask), m1 f32 [K,Hm*Wm] (masks of the objects) ->
  *   fg_ci, bg_ci f32 [Hm*Wm]: T2 = T * softmax(Cu, 2), rows /= sum + 1e-5, super-resolution h x w -> Hm x Wm of both
  *   index pairs (x P / (Hm Wm)), contraction with [m0 m1 > .5] clamp(m1, .1, .9) resp. [(1-m0)(1-m1) > .5]
  *   clamp(1-m1, .1, .9), mean over the K objects (fixed order).  workspace: bxs_corr_transfer_workspace_bytes.
+ * bxs_corr_transfer_batched: the same for n queries in one launch pair: T, Cu [n*kmax,P,P], m0 [n,Hm*Wm], m1
+ *   [n*kmax,Hm*Wm], counts i32 [n] (NULL: kmax each) -> fg_ci, bg_ci [n,Hm*Wm], the mean over query q's first counts[q]
+ *   tables (0 when it has none); workspace bxs_corr_transfer_workspace_bytes(n*kmax, Hm, Wm).  n, kmax <= 65535.
+ *   bxs_corr_transfer is its n = 1 case.
+ * bxs_corr_retrieve: get_similar_obj (:174-221) for the n query objects of a level at once, each against the bank of its
+ *   class as the objects before it in the level leave it.  Bank: a packed store of num_class x L slots, feat f32
+ *   [num_class*L, C*h*w], mask f32 [num_class*L, Hm*Wm], box f32 [num_class*L, 4], ptr / exists i32 [num_class];
+ *   first i32 [1]: the head has not seen a query yet (the first live query then uses q_feat_first, the create_one
+ *   re-normalisation :43).  Level: q_feat, q_feat_first, t_feat f32 [n, C*h*w], q_mask, t_mask f32 [n, Hm*Wm], box f32
+ *   [n,4] (integer valued), label, valid i32 [n] (valid 0 or a label outside [0, num_class): the object takes no part).
+ *   An object appends when both box sides exceed min_size; the j-th appending object of class c in the level writes slot
+ *   (ptr[c] + j) % L.  Outputs per query: src i32 [n, max(max_objs, 1)] the passing slots in ascending order, at most
+ *   max_objs (>= 0: store row class*L + slot; < 0: the level's object -(src+1), i.e. its t_feat / t_mask / box; 0 past
+ *   count), count i32 [n], kcount i32 [n] (count when count >= min_objs, else 0), slot i32 [n] (append slot or -1),
+ *   exists i32 [n] (the class had a bank at query time).  One CTA per query; shared memory corr_retrieve_scratch(L, h*w)
+ *   <= 200 KB (L = 100, 7 x 7: 40 KB).  Reads the bank, writes nothing of it.
+ * bxs_corr_paste: fg, bg f32 [n,Hm,Wm], box f32 [n,4], counts i32 [n] -> for every query with counts > 0 and a
+ *   non-empty box, iiu f32 [2n,H,W] planes 2q / 2q+1 over the box = the bilinear resize (align_corners False, the
+ *   arithmetic of bxs_bilinear_resize_forward) of bg / fg to the box; everything else of iiu is left unchanged.
+ * bxs_corr_bank_append: the ordered ring append of the level after bxs_corr_retrieve: every object with slot >= 0
+ *   copies t_feat / t_mask / box to row label*L + slot unless a later object of the level writes the same row; ptr[c]
+ *   = last slot + 1 mod L and exists[c] = 1 for every class that appended; first = 0 if the level had a live object.
+ * All four are sync-free; n == 0 is a no-op.  BXS_ERR_INVALID_ARG: a NULL pointer, a non-positive size;
+ * BXS_ERR_UNSUPPORTED: a dimension above INT32_MAX or the shared-memory bound.
  * --------------------------------------------------------------------------------------- */
 int bxs_corr_solve(const float* Cu, float* T, int64_t K, int64_t h, int64_t w, int dist_kernel, int num_iter,
                    int num_smooth, bxs_stream_t stream);
+int bxs_corr_solve_batched(const float* Cu, float* T, const int32_t* counts, int64_t n, int64_t kmax, int64_t h, int64_t w,
+                           int dist_kernel, int num_iter, int num_smooth, bxs_stream_t stream);
 int64_t bxs_corr_transfer_workspace_bytes(int64_t K, int64_t Hm, int64_t Wm);
 int bxs_corr_transfer(const float* T, const float* Cu, const float* m0, const float* m1, float* fg_ci, float* bg_ci,
                       void* workspace, int64_t K, int64_t h, int64_t w, int64_t Hm, int64_t Wm, bxs_stream_t stream);
+int bxs_corr_transfer_batched(const float* T, const float* Cu, const float* m0, const float* m1, const int32_t* counts,
+                              float* fg_ci, float* bg_ci, void* workspace, int64_t n, int64_t kmax, int64_t h, int64_t w,
+                              int64_t Hm, int64_t Wm, bxs_stream_t stream);
+int bxs_corr_retrieve(const float* bank_feat, const float* bank_mask, const float* bank_box, const int32_t* bank_ptr,
+                      const int32_t* bank_exists, const int32_t* first, const float* q_feat, const float* q_feat_first,
+                      const float* q_mask, const float* t_feat, const float* t_mask, const float* box, const int32_t* label,
+                      const int32_t* valid, int32_t* src, int32_t* count, int32_t* kcount, int32_t* slot, int32_t* exists,
+                      int64_t n, int64_t num_class, int64_t L, int64_t C, int64_t h, int64_t w, int64_t Hm, int64_t Wm,
+                      float fg_thr, float bg_thr, float app_thr, float ratio_lo, float ratio_hi, float min_size, int max_objs,
+                      int min_objs, bxs_stream_t stream);
+int bxs_corr_paste(const float* fg, const float* bg, const float* box, const int32_t* counts, float* iiu, int64_t n, int64_t Hm,
+                   int64_t Wm, int64_t H, int64_t W, bxs_stream_t stream);
+int bxs_corr_bank_append(float* bank_feat, float* bank_mask, float* bank_box, int32_t* bank_ptr, int32_t* bank_exists,
+                         int32_t* first, const float* t_feat, const float* t_mask, const float* box, const int32_t* label,
+                         const int32_t* valid, const int32_t* slot, int64_t n, int64_t num_class, int64_t L, int64_t CP,
+                         int64_t M, bxs_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------
  * f1  Hungarian matching    replaces scipy.optimize.linear_sum_assignment in MaskHungarianAssigner.assign step 3
