@@ -74,6 +74,7 @@ SIGNATURES = {
     'bxs_upsampled_rowcol_max': [c_p] * 4 + [c_i64] * 5 + [c_int, c_p],
     'bxs_bilinear_resize_forward': [c_p, c_p] + [c_i64] * 5 + [c_int, c_p],
     'bxs_bilinear_resize_backward': [c_p, c_p] + [c_i64] * 5 + [c_int, c_p],
+    'bxs_box2mask_attn_mask': [c_p, c_p] + [c_i64] * 7 + [c_int, c_int, c_p],
     'bxs_tree_edge_weight_forward': [c_p] * 4 + [c_i64] * 4 + [c_f, c_p],
     'bxs_tree_edge_weight_backward': [c_p] * 7 + [c_i64] * 4 + [c_f, c_p],
     'bxs_levelset_fused_workspace_bytes': [c_i64],

@@ -1,7 +1,9 @@
 // a18: the per-pixel arithmetic of the bilinear resize (ATen UpSample.cuh semantics: source index, lambdas, the order of the
-// four products), shared by bxs_bilinear_resize_forward (fused_assembly.cu) and bxs_corr_paste (corr.cu) so that both give
-// the same bits for the same input.
+// four products), shared by bxs_bilinear_resize_forward (fused_assembly.cu), bxs_corr_paste (corr.cu) and
+// bxs_box2mask_attn_mask (box2mask_attn.cu) so that all give the same bits for the same input.
 #pragma once
+#include <cuda_bf16.h>
+#include <cuda_fp16.h>
 
 namespace bxs {
 
@@ -25,12 +27,18 @@ __device__ __forceinline__ RsTap rs_tap(float scale, int dst, int in, bool align
   return t;
 }
 
+// a tap widened to float: a 16-bit plane is interpolated in float32, as ATen does (accscalar_t)
+__device__ __forceinline__ float rs_load(const float* p) { return __ldg(p); }
+__device__ __forceinline__ float rs_load(const __half* p) { return __half2float(__ldg(p)); }
+__device__ __forceinline__ float rs_load(const __nv_bfloat16* p) { return __bfloat162float(__ldg(p)); }
+
 // output pixel (oy, ox) of one h x w plane `in` resized with the scales sh, sw
-__device__ __forceinline__ float rs_pixel(const float* __restrict__ in, int h, int w, float sh, float sw, int oy, int ox,
+template <typename T>
+__device__ __forceinline__ float rs_pixel(const T* __restrict__ in, int h, int w, float sh, float sw, int oy, int ox,
                                           bool align) {
   const RsTap ty = rs_tap(sh, oy, h, align), tx = rs_tap(sw, ox, w, align);
-  const float* p = in + ty.i0 * w + tx.i0;
-  const float v00 = __ldg(p), v01 = __ldg(p + tx.ip), v10 = __ldg(p + ty.ip * w), v11 = __ldg(p + ty.ip * w + tx.ip);
+  const T* p = in + ty.i0 * w + tx.i0;
+  const float v00 = rs_load(p), v01 = rs_load(p + tx.ip), v10 = rs_load(p + ty.ip * w), v11 = rs_load(p + ty.ip * w + tx.ip);
   return ty.l0 * (tx.l0 * v00 + tx.l1 * v01) + ty.l1 * (tx.l0 * v10 + tx.l1 * v11);
 }
 

@@ -16,6 +16,7 @@ import torch
 import torch.nn as nn
 import torch.nn.functional as F
 
+from ...ops.box2mask import attention_mask
 from ...ops.discobox import HALF_DTYPES, discobox_mask_loss
 from ...ops.dynconv import box2mask_mask_pred, dynconv1x1, solo_dynamic_conv
 from ...ops.lsap import solve_batched
@@ -384,6 +385,64 @@ class Box2MaskHead(nn.Module):
     @staticmethod
     def mask_pred(mask_embed, mask_feature):
         return box2mask_mask_pred(mask_embed, mask_feature)
+
+    # a4 -- box2mask_head.py:338-359, the reference's signature
+    def forward_head(self, decoder_out, mask_feature, attn_mask_target_size):
+        """(cls_pred, mask_pred, attn_mask, levelset_feat) after one decoder layer, as the reference returns them.
+        ``mask_pred`` is the wgmma dynamic convolution (``mask_pred``: TF32 for float32 operands, the operand dtype under
+        autocast); ``attn_mask`` [B*num_heads, Q, h*w] bool is ``ops.box2mask.attention_mask`` of it, bit for bit the
+        reference's interpolate / repeat / sigmoid / compare lines on the same ``mask_pred``."""
+        return self._forward_head(decoder_out, mask_feature, attn_mask_target_size, reset_full_rows=False)
+
+    def _forward_head(self, decoder_out, mask_feature, attn_mask_target_size, reset_full_rows):
+        missing = [n for n in ('transformer_decoder', 'cls_embed', 'mask_embed', 'levelset_bottom', 'num_heads')
+                   if not hasattr(self, n)]
+        if missing:
+            raise RuntimeError('Box2MaskHead.forward_head needs the modules the reference constructor builds (mmdet '
+                               f'installed); this head has no {", ".join(missing)}')
+        decoder_out = self.transformer_decoder.post_norm(decoder_out).transpose(0, 1)
+        cls_pred = self.cls_embed(decoder_out)
+        mask_embed = self.mask_embed(decoder_out)
+        mask_pred = self.mask_pred(mask_embed, mask_feature)
+        attn_mask = attention_mask(mask_pred, attn_mask_target_size, self.num_heads, reset_full_rows=reset_full_rows)
+        levelset_feat = self.levelset_bottom(mask_feature)
+        return cls_pred, mask_pred, attn_mask, levelset_feat
+
+    # box2mask_head.py:361-419, the reference's signature
+    def forward(self, feats, img_metas):
+        """(cls_pred_list, mask_pred_list, lst_feat_list) of the query-feature head and every decoder layer, as the reference
+        computes them.  The mask a decoder layer receives comes out of the attention-mask kernel with its all-True rows
+        already cleared (the reference clears them with a ``torch.where``, :397, one host synchronisation per layer), so
+        nothing here synchronises with the host: after one eager call the forward can be captured in a CUDA graph."""
+        batch_size = len(img_metas)
+        mask_features, multi_scale_memorys = self.pixel_decoder(feats)
+        decoder_inputs, decoder_positional_encodings = [], []
+        for i in range(self.num_transformer_feat_level):
+            decoder_input = self.decoder_input_projs[i](multi_scale_memorys[i])
+            decoder_input = decoder_input.flatten(2).permute(2, 0, 1)
+            decoder_input = decoder_input + self.level_embed.weight[i].view(1, 1, -1)
+            mask = decoder_input.new_zeros((batch_size, ) + multi_scale_memorys[i].shape[-2:], dtype=torch.bool)
+            decoder_positional_encoding = self.decoder_positional_encoding(mask).flatten(2).permute(2, 0, 1)
+            decoder_inputs.append(decoder_input)
+            decoder_positional_encodings.append(decoder_positional_encoding)
+        query_feat = self.query_feat.weight.unsqueeze(1).repeat((1, batch_size, 1))
+        query_embed = self.query_embed.weight.unsqueeze(1).repeat((1, batch_size, 1))
+
+        cls_pred, mask_pred, attn_mask, lst_feat = self._forward_head(query_feat, mask_features,
+                                                                      multi_scale_memorys[0].shape[-2:], True)
+        cls_pred_list, mask_pred_list, lst_feat_list = [cls_pred], [mask_pred], [lst_feat]
+        for i in range(self.num_transformer_decoder_layers):
+            level_idx = i % self.num_transformer_feat_level
+            query_feat = self.transformer_decoder.layers[i](
+                query=query_feat, key=decoder_inputs[level_idx], value=decoder_inputs[level_idx], query_pos=query_embed,
+                key_pos=decoder_positional_encodings[level_idx], attn_masks=[attn_mask, None],
+                query_key_padding_mask=None, key_padding_mask=None)
+            cls_pred, mask_pred, attn_mask, lst_feat = self._forward_head(
+                query_feat, mask_features, multi_scale_memorys[(i + 1) % self.num_transformer_feat_level].shape[-2:], True)
+            cls_pred_list.append(cls_pred)
+            mask_pred_list.append(mask_pred)
+            lst_feat_list.append(lst_feat)
+        return cls_pred_list, mask_pred_list, lst_feat_list
 
     # a17 -- box2mask_head.py:229-233, 269-335
     def mask_loss_single(self, mask_preds, mask_targets, num_per_img, norm_img, lst_feat, trees=None):

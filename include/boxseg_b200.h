@@ -386,6 +386,23 @@ int bxs_bilinear_resize_backward(const float* g_out, float* g_in, int64_t NC, in
                                  int64_t W, int align_corners, bxs_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------
+ * a4  Box2Mask cross-attention mask    replaces the attention-mask lines of Box2MaskHead.forward_head
+ *     (mmdet/models/dense_heads/box2mask_head.py:346-355) and, with reset_full_rows, the reset of its forward loop (:397).
+ * mask_pred [B,Q,H,W] of the type `dtype` names -> attn uint8 [B*heads, Q, h*w] (0 / 1: the bytes of a torch.bool tensor),
+ * row (b*heads + k, q) = row (b, q) for every head k.  Bit = sigmoid(r) < 0.5 with r the bilinear resize to (h, w),
+ * align_corners False, in the arithmetic of bxs_bilinear_resize_forward; 16-bit inputs are interpolated in float32 and
+ * rounded to `dtype`, their sigmoid is computed in float32 and rounded to `dtype` again (torch's rounding points).  NaN gives
+ * 0.  reset_full_rows != 0: a (b, q) row whose bits are all 1 is written as all 0 (no count leaves the kernel).
+ * Sync-free, no workspace; B*Q == 0 is a no-op.  BXS_ERR_INVALID_ARG: a NULL pointer, a negative B or Q, a non-positive
+ * H, W, h, w, heads < 1, an unknown dtype.  BXS_ERR_UNSUPPORTED: a side >= 2^24, H*W or heads*h*w above INT32_MAX, an
+ * element count above INT64_MAX, or a row h*w above 1.6 M pixels (8 CTAs x 200 KB of shared memory).  All checks run
+ * before any device call.
+ * --------------------------------------------------------------------------------------- */
+typedef enum { BXS_ATTN_F32 = 0, BXS_ATTN_F16 = 1, BXS_ATTN_BF16 = 2 } bxs_attn_dtype_t;
+int bxs_box2mask_attn_mask(const void* mask_pred, uint8_t* attn, int64_t B, int64_t Q, int64_t H, int64_t W, int64_t h,
+                           int64_t w, int64_t heads, int dtype, int reset_full_rows, bxs_stream_t stream);
+
+/* ---------------------------------------------------------------------------------------
  * a14  tree edge weights     replaces TreeFilter2D.build_edge_weight with the default norm2 distance
  *     (mmdet/ops/tree_filter/modules/tree_filter.py:72-108) and its autograd.
  * embed [B*groups, C, V] (vertex order; a [B, groups*C, V] tensor viewed per group), sorted_index / sorted_parent
