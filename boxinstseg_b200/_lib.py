@@ -68,6 +68,10 @@ SIGNATURES = {
     'bxs_dynconv1x1_forward': [c_p] * 3 + [c_i64] * 4 + [c_p],
     'bxs_dynconv1x1_backward_workspace_bytes': [c_i64] * 4,
     'bxs_dynconv1x1_backward': [c_p] * 6 + [c_i64] * 4 + [c_p],
+    'bxs_dynconv1x1_cells_forward_workspace_bytes': [c_p] + [c_i64] * 3,
+    'bxs_dynconv1x1_cells_forward': [c_p] * 9 + [c_i64] * 4 + [c_p],
+    'bxs_dynconv1x1_cells_backward_workspace_bytes': [c_p] * 4 + [c_i64] * 4,
+    'bxs_dynconv1x1_cells_backward': [c_p] * 11 + [c_i64] * 4 + [c_p],
     'bxs_dynconv1x1_half_forward': [c_p] * 3 + [c_i64] * 4 + [c_int, c_p],
     'bxs_dynconv1x1_half_backward_workspace_bytes': [c_i64] * 4 + [c_int],
     'bxs_dynconv1x1_half_backward': [c_p] * 6 + [c_i64] * 4 + [c_int, c_p],
@@ -97,7 +101,8 @@ _RESTYPE = {'bxs_mst_workspace_bytes': c_i64, 'bxs_bfs_workspace_bytes': c_i64, 
              'bxs_boxinst_loss_plan_bytes': c_i64, 'bxs_levelset_fused_workspace_bytes': c_i64,
              'bxs_dynconv1x1_backward_workspace_bytes': c_i64, 'bxs_corr_transfer_workspace_bytes': c_i64,
              'bxs_dynconv1x1_half_backward_workspace_bytes': c_i64, 'bxs_lsap_workspace_bytes': c_i64,
-             'bxs_discobox_loss_workspace_bytes': c_i64}
+             'bxs_discobox_loss_workspace_bytes': c_i64, 'bxs_dynconv1x1_cells_forward_workspace_bytes': c_i64,
+             'bxs_dynconv1x1_cells_backward_workspace_bytes': c_i64}
 
 _STATUS = {-1: 'invalid argument', -2: 'kernel launch failed', -3: 'unsupported shape', -4: 'no CUDA device'}
 

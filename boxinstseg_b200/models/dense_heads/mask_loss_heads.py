@@ -18,7 +18,7 @@ import torch.nn.functional as F
 
 from ...ops.box2mask import attention_mask
 from ...ops.discobox import HALF_DTYPES, discobox_mask_loss
-from ...ops.dynconv import box2mask_mask_pred, dynconv1x1, solo_dynamic_conv
+from ...ops.dynconv import box2mask_mask_pred, dynconv1x1, solo_cells_conv, solo_dynamic_conv
 from ...ops.lsap import solve_batched
 from ...ops.resize import bilinear_resize, scale_target as _scale_target   # a18: F.interpolate / _scale_target as kernels
 from ...ops._streams import Forked, run_concurrently
@@ -51,18 +51,17 @@ class BoxSOLOv2Head(nn.Module):
 
     # a2 -- box_solov2_head.py:204-217
     def dynamic_conv(self, feature_pred, kernel_pred, out_size=None, cells=None):
-        """feature_pred [B,C,h,w], kernel_pred [B,C,S,S] -> [B,S*S,h',w'].  ``cells`` (list of per-image index
+        """feature_pred [B,C,h,w], kernel_pred [B,C,S,S] -> [B,S*S,h',w'].  ``cells`` (list of per-image ascending index
         tensors) restricts the convolution to the positive grid cells the loss will index (:317-320), which is
-        what the training loss needs; without it all S*S cells are computed as the reference does."""
-        if cells is None:
-            ins = solo_dynamic_conv(feature_pred, kernel_pred)
-        else:
-            B, C, S, _ = kernel_pred.shape
-            flat = kernel_pred.permute(0, 2, 3, 1).reshape(B, S * S, C)
-            ins = [dynconv1x1(feature_pred[b:b + 1], flat[b:b + 1, cells[b]])[0] for b in range(B)]
+        what the training loss needs, and returns the per-image list of [n_b,h',w'] rows (``solo_cells_conv``: one launch,
+        the resize applied to feature_pred); without it all S*S cells are computed as the reference does."""
+        if cells is not None:
+            size = tuple(out_size) if out_size is not None else tuple(feature_pred.shape[-2:])
+            rows = solo_cells_conv(feature_pred, [kernel_pred], [cells], [size])[0]
+            return list(rows.split([int(c.numel()) for c in cells]))
+        ins = solo_dynamic_conv(feature_pred, kernel_pred)
         if out_size is not None:
-            up = lambda t: bilinear_resize(t, out_size)   # noqa: E731  (:213, align_corners=False)
-            ins = up(ins) if cells is None else [up(t[None])[0] for t in ins]
+            ins = bilinear_resize(ins, out_size)          # :213, align_corners=False
         return ins
 
     # a17 -- box_solov2_head.py:334-367

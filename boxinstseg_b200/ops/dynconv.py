@@ -10,9 +10,12 @@ FP16 / BF16 operands run the 16-bit kernels (bxs_dynconv1x1_half_*: FP32 accumul
 operand dtype), and under ``torch.autocast('cuda')`` both operands are cast to the autocast dtype first, as autocast does
 for the ``F.conv2d`` this op replaces.
 """
+import ctypes
+
 import torch
 
 from .. import _lib as L
+from .resize import bilinear_resize
 
 _HALF = {torch.float16: 0, torch.bfloat16: 1}          # bxs_half_t
 _AUTOCAST_ELIGIBLE = (torch.float32, torch.float16, torch.bfloat16)
@@ -119,6 +122,110 @@ def solo_dynamic_conv(feature_pred, kernel_pred):
     -> [B,S*S,h,w] with cell s = gy*S+gx (the reference's permute(0,2,3,1).view(-1,C) order)."""
     B, C, S, _ = kernel_pred.shape
     return dynconv1x1(feature_pred, kernel_pred.permute(0, 2, 3, 1).reshape(B, S * S, C))
+
+
+def _i64(vals):
+    return (ctypes.c_int64 * len(vals))(*vals)
+
+
+def _ptrs(tensors):
+    return (ctypes.c_void_p * len(tensors))(*[None if t is None else t.data_ptr() for t in tensors])
+
+
+class _SoloCells(torch.autograd.Function):
+    """Levels -> positive rows on bxs_dynconv1x1_cells_*.  Inputs: the plan (host lists), the device cell list, then the
+    operands and the raw kernel grids."""
+
+    @staticmethod
+    def forward(ctx, plan, cells, *tensors):
+        level_op, counts = plan
+        n_ops = len(tensors) - len(level_op)
+        ops, kerns = tensors[:n_ops], tensors[n_ops:]
+        B, C = ops[0].shape[:2]
+        outs = [ops[o].new_empty((sum(n), ops[o].shape[2], ops[o].shape[3])) for o, n in zip(level_op, counts)]
+        ctx.save_for_backward(cells, *tensors)
+        ctx.plan = plan
+        args = (_i64([o.shape[2] * o.shape[3] for o in ops]), _ptrs(kerns), _i64([k.shape[-1] for k in kerns]),
+                _i64(level_op), _i64([c for n in counts for c in n]))
+        ctx.args = args
+        flat = args[-1]
+        with torch.cuda.device(ops[0].device):
+            ws = torch.empty(L.lib().bxs_dynconv1x1_cells_forward_workspace_bytes(flat, len(kerns), B, C), dtype=torch.uint8,
+                             device=ops[0].device)
+            L.check(L.lib().bxs_dynconv1x1_cells_forward(_ptrs(ops), args[0], args[1], args[2], args[3], flat, L.ptr(cells),
+                                                         _ptrs(outs), L.ptr(ws), len(kerns), n_ops, B, C, L.stream()),
+                    'dynconv1x1_cells_forward')
+        return tuple(outs)
+
+    @staticmethod
+    def backward(ctx, *g_outs):
+        cells, *tensors = ctx.saved_tensors
+        level_op, counts = ctx.plan
+        n_ops = len(tensors) - len(level_op)
+        ops, kerns = tensors[:n_ops], tensors[n_ops:]
+        B, C = ops[0].shape[:2]
+        need_op = any(ctx.needs_input_grad[2:2 + n_ops])
+        need_k = any(ctx.needs_input_grad[2 + n_ops:])
+        g = [torch.zeros((sum(n),) + ops[o].shape[2:], device=ops[0].device) if t is None else t.contiguous().float()
+             for t, o, n in zip(g_outs, level_op, counts)]
+        g_ops = [torch.empty_like(o) for o in ops] if need_op else None
+        g_k = [torch.empty_like(k) for k in kerns] if need_k else None
+        sizes, kp, grid, lop, flat = ctx.args
+        lib = L.lib()
+        with torch.cuda.device(ops[0].device):
+            ws = torch.empty(lib.bxs_dynconv1x1_cells_backward_workspace_bytes(sizes, grid, lop, flat, len(kerns), n_ops, B, C),
+                             dtype=torch.uint8, device=ops[0].device)
+            call = lambda gop, gk: lib.bxs_dynconv1x1_cells_backward(      # noqa: E731
+                _ptrs(ops), sizes, kp, grid, lop, flat, L.ptr(cells), _ptrs(g), gop, gk, L.ptr(ws), len(kerns), n_ops, B, C,
+                L.stream())
+            rc = call(_ptrs(g_ops) if need_op else None, _ptrs(g_k) if need_k else None)
+            if rc == -3 and need_op:
+                # more than 256 kernels in a problem: d/d operand through cuBLAS, as dynconv1x1 does beyond 256 kernels
+                g_ops = _cells_operand_grad_mm(ops, kerns, cells, g, level_op, counts)
+                rc = call(None, _ptrs(g_k)) if need_k else 0
+            L.check(rc, 'dynconv1x1_cells_backward')
+        return (None, None, *(g_ops if need_op else [None] * n_ops), *(g_k if need_k else [None] * len(kerns)))
+
+
+def _cells_operand_grad_mm(ops, kerns, cells, g, level_op, counts):
+    g_ops = [torch.zeros_like(o) for o in ops]
+    start = 0
+    for l, (o, n) in enumerate(zip(level_op, counts)):
+        C = kerns[l].shape[1]
+        row = 0
+        for b, nb in enumerate(n):
+            if nb:
+                k = kerns[l][b].reshape(C, -1)[:, cells[start:start + nb].long()]
+                g_ops[o][b] += (k @ g[l][row:row + nb].flatten(1)).view_as(g_ops[o][b])
+            start, row = start + nb, row + nb
+    return g_ops
+
+
+def solo_cells_conv(feature_pred, kernel_preds, cells, out_sizes):
+    """The positive rows of BoxSOLOv2's per-level dynamic convolution (box_solov2_head.py:204-216, indexed as :317-320).
+
+    feature_pred [B,C,h,w]; kernel_preds: per level the raw grid [B,C,S,S] (as ``solo_kernel`` produces it); cells: per level
+    a list of B int tensors, the ascending positive cells (gy*S + gx) of each image; out_sizes: per level (h_l, w_l).
+    Returns per level [n_l, h_l, w_l] = interpolate(conv2d(feature_pred, cells), (h_l, w_l), bilinear)[positives], images
+    in order: the reference's rows.  The resize is applied to the operand instead of the result (both are linear and
+    per channel): levels of feature_pred's own size convolve it directly, every other size convolves one
+    ``bilinear_resize`` of it, shared by the consecutive levels of that size.  All levels and images run in one launch
+    (TF32 operands, FP32 accumulation); other dtypes are promoted to float32.  Differentiable with respect to
+    feature_pred and kernel_preds; gradients are deterministic.  C % 32 == 0, C <= 256, h_l*w_l % 4 == 0."""
+    f = feature_pred.contiguous().float()
+    L.require_cuda(f)
+    sizes = [(int(s[0]), int(s[1])) for s in out_sizes]
+    level_op, op_sizes = [], []
+    for s in sizes:
+        if not op_sizes or op_sizes[-1] != s:
+            op_sizes.append(s)
+        level_op.append(len(op_sizes) - 1)
+    ops = [f if s == tuple(f.shape[-2:]) else bilinear_resize(f, s) for s in op_sizes]
+    kerns = [k.contiguous().float() for k in kernel_preds]
+    counts = [[int(c.numel()) for c in lvl] for lvl in cells]
+    flat = [c.reshape(-1) for lvl in cells for c in lvl]
+    flat = torch.cat(flat).to(device=f.device, dtype=torch.int32) if flat else f.new_zeros(0, dtype=torch.int32)
+    return list(_SoloCells.apply((level_op, counts), flat, *ops, *kerns))
 
 
 def box2mask_mask_pred(mask_embed, mask_feature):
