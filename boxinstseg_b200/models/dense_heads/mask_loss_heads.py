@@ -19,6 +19,7 @@ import torch.nn.functional as F
 from ...ops.box2mask import attention_mask
 from ...ops.discobox import HALF_DTYPES, discobox_mask_loss
 from ...ops.dynconv import box2mask_mask_pred, dynconv1x1, solo_cells_conv, solo_dynamic_conv
+from ...ops.focal import sigmoid_focal_loss_levels
 from ...ops.lsap import solve_batched
 from ...ops.resize import bilinear_resize, scale_target as _scale_target   # a18: F.interpolate / _scale_target as kernels
 from ...ops._streams import Forked, run_concurrently
@@ -35,19 +36,217 @@ def _phi_and_pixels(mask_pred, box_mask):
     return phi, pix
 
 
+class SoloLevelPred:
+    """One level of ``BoxSOLOv2Head.forward``'s training ``ins_pred``, not computed: the reference tensor is
+    ``interpolate(conv2d(feature_pred, kernel_pred cells, groups=B), out_size, bilinear)`` [B,S*S,*out_size]
+    (box_solov2_head.py:204-216).  ``shape`` / ``size()`` report that tensor's shape, ``dense()`` computes it."""
+
+    def __init__(self, feature_pred, kernel_pred, out_size):
+        self.feature_pred, self.kernel_pred, self.out_size = feature_pred, kernel_pred, tuple(int(s) for s in out_size)
+
+    @property
+    def shape(self):
+        B, _, S, _ = self.kernel_pred.shape
+        return torch.Size((B, S * S) + self.out_size)
+
+    def size(self, dim=None):
+        return self.shape if dim is None else self.shape[dim]
+
+    def dense(self):
+        return bilinear_resize(solo_dynamic_conv(self.feature_pred, self.kernel_pred), self.out_size)
+
+
+class SoloInsPreds(list):
+    """``BoxSOLOv2Head.forward``'s training ``ins_preds``: one ``SoloLevelPred`` per level, all of one ``feature_pred``.
+    ``BoxSOLOv2Head.loss`` convolves only the positive cells of it; the reference's ``loss`` reads nothing but
+    ``featmap.size()[-2:]`` from its ``ins_preds`` (:281)."""
+
+    @property
+    def feature_pred(self):
+        return self[0].feature_pred
+
+
+def _coord_feat(x):
+    """The two coordinate channels of box_solov2_head.py:190-196, 230-235: x then y, linspace(-1, 1) each."""
+    x_range = torch.linspace(-1, 1, x.shape[-1], device=x.device)
+    y_range = torch.linspace(-1, 1, x.shape[-2], device=x.device)
+    y, xx = torch.meshgrid(y_range, x_range, indexing='ij')
+    return torch.cat([xx.expand([x.shape[0], 1, -1, -1]), y.expand([x.shape[0], 1, -1, -1])], 1)
+
+
+_SOLO_TOWERS = ('feature_convs', 'kernel_convs', 'cate_convs', 'solo_kernel', 'solo_cate', 'solo_mask', 'levelset_bottom')
+
+
 @register(HEADS, partial=True)
 class BoxSOLOv2Head(nn.Module):
-    """BoxLevelset head: mask-loss path only."""
+    """BoxLevelset head: ``forward`` / ``loss`` with the reference's signatures on the positive grid cells only, and the
+    mask-loss path (``mask_loss``, ``dynamic_conv``).  The conv towers are the reference constructor's modules (mmdet
+    installed, or attached by the caller); the standalone constructor builds only the losses."""
 
-    def __init__(self, num_classes=80, in_channels=256, loss_boxpro=None, loss_levelset=None, **cfg):
+    def __init__(self, num_classes=80, in_channels=256, loss_cate=None, loss_boxpro=None, loss_levelset=None,
+                 num_grids=None, strides=(4, 8, 16, 32, 64),
+                 scale_ranges=((8, 32), (16, 64), (32, 128), (64, 256), (128, 512)), sigma=0.2, cate_down_pos=0, **cfg):
         super().__init__()
         self.num_classes = num_classes
+        self.cate_out_channels = num_classes
         self.in_channels = in_channels
+        self.seg_num_grids, self.strides, self.scale_ranges, self.sigma = num_grids, strides, scale_ranges, sigma
+        self.cate_down_pos = cate_down_pos
         self.cfg = cfg
+        self.loss_cate_cfg = loss_cate or dict(type='FocalLoss', use_sigmoid=True, gamma=2.0, alpha=0.25, loss_weight=1.0)
         self.loss_boxpro = build_loss(loss_boxpro or dict(type='BoxProjectionLoss', loss_weight=3.0))
         self.loss_levelset = build_loss(loss_levelset or dict(type='LevelsetLoss', loss_weight=1.0))
         self.mst = MinimumSpanningTree(TreeFilter2D.norm2_distance)
         self.tree_filter = TreeFilter2D()
+        self._bxs_post_init()
+
+    def _bxs_post_init(self):
+        """Also runs after the REFERENCE class's ``__init__`` when mmdet is importable: the focal parameters are then read
+        from the FocalLoss module it built (``self.loss_cate``)."""
+        ref = getattr(self, 'loss_cate', None)
+        if isinstance(ref, nn.Module):
+            cfg = dict(use_sigmoid=ref.use_sigmoid, gamma=ref.gamma, alpha=ref.alpha, reduction=ref.reduction,
+                       loss_weight=ref.loss_weight, activated=getattr(ref, 'activated', False))
+        else:
+            cfg = self.loss_cate_cfg
+        if not cfg.get('use_sigmoid', True) or cfg.get('activated', False) or cfg.get('reduction', 'mean') != 'mean':
+            raise NotImplementedError('BoxSOLOv2Head: the category loss is the sigmoid focal loss on logits with reduction '
+                                      f"'mean' only, got {cfg}")
+        self.focal = (float(cfg.get('gamma', 2.0)), float(cfg.get('alpha', 0.25)), float(cfg.get('loss_weight', 1.0)))
+
+    # box_solov2_head.py:179-217, the reference's signature
+    def forward(self, feats, eval=False):
+        """(ins_preds, cate_preds, levelset_feats) as the reference returns them, with one difference in training: ``ins_preds``
+        is a ``SoloInsPreds`` -- feature_pred, the raw kernel grids and the output sizes -- instead of the dense
+        [B,S*S,h,w] predictions, which ``loss`` never needs (it convolves the positive cells only).  ``eval=True``: the
+        reference's outputs, the sigmoid of the dense convolution (wgmma) and the local-max-masked category scores."""
+        missing = [n for n in _SOLO_TOWERS if not hasattr(self, n)]
+        if missing:
+            raise RuntimeError('BoxSOLOv2Head.forward needs the modules the reference constructor builds (mmdet installed); '
+                               f'this head has no {", ".join(missing)}')
+        feats = [feat.float() for feat in feats]
+        new_feats = self.split_feats(feats)
+        featmap_sizes = [featmap.size()[-2:] for featmap in new_feats]
+        kernel_pred, cate_pred = zip(*[self.forward_single(x, i, eval=eval) for i, x in enumerate(new_feats)])
+        coord_feat = _coord_feat(feats[-2])
+        feature_add_all_level = self.feature_convs[0](feats[0])
+        for i in range(1, 3):
+            feature_add_all_level = feature_add_all_level + self.feature_convs[i](feats[i])
+        feature_add_all_level = feature_add_all_level + self.feature_convs[3](torch.cat([feats[3], coord_feat], 1))
+        feature_pred = self.solo_mask(feature_add_all_level)
+        levelset_feats = self.levelset_bottom(feature_pred)
+        if eval:
+            return [torch.sigmoid(self.dynamic_conv(feature_pred, k)) for k in kernel_pred], list(cate_pred), levelset_feats
+        ins_pred = SoloInsPreds(SoloLevelPred(feature_pred, k, (2 * s[0], 2 * s[1])) for k, s in zip(kernel_pred, featmap_sizes))
+        return ins_pred, list(cate_pred), levelset_feats
+
+    # box_solov2_head.py:219-224
+    @staticmethod
+    def split_feats(feats):
+        return (F.interpolate(feats[0], scale_factor=0.5, mode='bilinear'), feats[1], feats[2], feats[3],
+                F.interpolate(feats[4], size=feats[3].shape[-2:], mode='bilinear'))
+
+    # box_solov2_head.py:226-260
+    def forward_single(self, x, idx, eval=False):
+        kernel_feat = torch.cat([x, _coord_feat(x)], 1)
+        cate_feat = x
+        for i, kernel_layer in enumerate(self.kernel_convs):
+            if i == self.cate_down_pos:
+                kernel_feat = F.interpolate(kernel_feat, size=self.seg_num_grids[idx], mode='bilinear')
+            kernel_feat = kernel_layer(kernel_feat)
+        kernel_pred = self.solo_kernel(kernel_feat)
+        for i, cate_layer in enumerate(self.cate_convs):
+            if i == self.cate_down_pos:
+                cate_feat = F.interpolate(cate_feat, size=self.seg_num_grids[idx], mode='bilinear')
+            cate_feat = cate_layer(cate_feat)
+        cate_pred = self.solo_cate(cate_feat)
+        if eval:
+            cate_pred = cate_pred.sigmoid()
+            local_max = F.max_pool2d(cate_pred, (2, 2), stride=1, padding=1)
+            cate_pred = (cate_pred * (local_max[:, :, :-1, :-1] == cate_pred)).permute(0, 2, 3, 1)
+        return kernel_pred, cate_pred
+
+    # box_solov2_head.py:262-388, the reference's signature
+    def loss(self, ins_preds, cate_preds, levelset_feats, gt_bbox_list, gt_label_list, gt_mask_list, img, img_metas, cfg,
+             gt_bboxes_ignore=None):
+        """dict(loss_boxpro, loss_levelset, loss_cate) as the reference computes them.  ``ins_preds``: ``forward``'s
+        ``SoloInsPreds`` (only the positive cells are convolved, ``solo_cells_conv``: one launch for every level and image)
+        or the reference's dense per-level [B,S*S,h,w] tensors (their positive rows are gathered).  ``gt_mask_list``: per
+        image uint8 [G,H,W] tensors, or anything with mmdet's ``to_tensor(dtype, device)`` (BitmapMasks).
+        The grid targets are built on the device (``solo_grid_targets``), the image and level-set targets stay per image (the
+        trees are shared by its instances), ``loss_cate`` is ``sigmoid_focal_loss_levels`` on the [B,C,S,S] maps as they lie.
+        ONE read back to the host: the positive count of every (level, image).
+        A batch without any positive (the reference raises at :366) gives zero ``loss_boxpro`` / ``loss_levelset`` attached
+        to the graph, and ``loss_cate`` over the all-background labels."""
+        from .solo_targets import solo_grid_targets
+        grids = list(self.seg_num_grids)
+        n_lv, B = len(grids), len(gt_label_list)
+        dev = levelset_feats.device
+        sizes = [tuple(int(s) for s in p.size()[-2:]) for p in ins_preds]
+        masks = [(m if torch.is_tensor(m) else m.to_tensor(dtype=torch.uint8, device=dev)).to(dev, torch.uint8)
+                 for m in gt_mask_list]
+        per_img = [solo_grid_targets(b, l, m, sizes, self.scale_ranges, self.strides, grids, self.sigma, self.num_classes,
+                                     dense=False) for b, l, m in zip(gt_bbox_list, gt_label_list, masks)]
+        ind = [torch.stack([per_img[b][2][lv] for b in range(B)]) for lv in range(n_lv)]            # [B,S^2] bool
+        counts = torch.cat([i.sum(1) for i in ind])
+        counts_host = counts.tolist()                                        # the one host read: n of every (level, image)
+        n = [sum(counts_host[lv * B:(lv + 1) * B]) for lv in range(n_lv)]
+        flat = torch.nonzero_static(torch.cat([i.flatten() for i in ind]), size=sum(n)).squeeze(1)
+        avg_factor = counts.sum() + 1                                        # num_ins + 1 (:329, 383), on the device
+        cate_labels = [torch.stack([per_img[b][1][lv] for b in range(B)]) for lv in range(n_lv)]
+        loss_cate = sigmoid_focal_loss_levels(cate_preds, cate_labels, avg_factor, *self.focal)
+        if sum(n) == 0:
+            # 0 whatever the leaves hold (0 * Inf would be NaN), with zero gradients to every leaf
+            off = torch.zeros((), dtype=torch.bool, device=dev)
+            zero = sum(p.reshape(-1)[:1].sum().where(off, 0.) for p in self._graph_leaves(ins_preds, levelset_feats))
+            return dict(loss_boxpro=zero, loss_levelset=zero.clone(), loss_cate=loss_cate)
+
+        # ascending positives, level-major then image-major: the rows of the reference's boolean indexing (:294-320)
+        local, start = [], 0
+        for lv, S in enumerate(grids):
+            local.append(flat[start:start + n[lv]] - B * sum(s * s for s in grids[:lv]))    # b * S^2 + cell
+            start += n[lv]
+        inst_imgs = [(loc // (S * S)).to(torch.int32) for loc, S in zip(local, grids)]
+        cells = [loc % (S * S) for loc, S in zip(local, grids)]
+        ins_labels = [self._box_mask_rows(per_img, lv, loc, grids[lv], sizes[lv], gt_label_list, dev)
+                      for lv, loc in enumerate(local)]
+        resized = {}
+        for s in sizes:                                                      # :412-415, per image
+            if s not in resized:
+                resized[s] = (bilinear_resize(img.float(), s), bilinear_resize(levelset_feats, s))
+        if isinstance(ins_preds, SoloInsPreds):
+            per_level_cells = [list(c.split(counts_host[lv * B:(lv + 1) * B])) for lv, c in enumerate(cells)]
+            rows = solo_cells_conv(ins_preds.feature_pred, [p.kernel_pred for p in ins_preds], per_level_cells, sizes)
+        else:
+            rows = [p.reshape((-1,) + tuple(p.shape[2:])).index_select(0, loc) for p, loc in zip(ins_preds, local)]
+        out = self.mask_loss(rows, ins_labels, [resized[s][0] for s in sizes], [resized[s][1] for s in sizes],
+                             inst_imgs=inst_imgs)
+        return dict(loss_boxpro=out['loss_boxpro'], loss_levelset=out['loss_levelset'], loss_cate=loss_cate)
+
+    @staticmethod
+    def _box_mask_rows(per_img, lv, loc, S, size, gt_label_list, dev):
+        """[n, h, w] uint8 box-mask targets of a level's positives: ``small[winner[cell]]`` of their image placed top-left
+        (:459-466).  Each image's masks have their own size (mmdet pads them to the image's own pad shape), so every image's
+        rescaled masks are placed on a level-sized canvas before the rows are gathered."""
+        B, (h, w) = len(per_img), size
+        smalls = [per_img[b][0][lv][1] for b in range(B) if len(gt_label_list[b])]
+        if not smalls or loc.numel() == 0:
+            return torch.zeros((loc.numel(), h, w), dtype=torch.uint8, device=dev)
+        first = [sum(len(g) for g in gt_label_list[:b]) for b in range(B)]                  # ground truths before image b
+        winner = torch.stack([per_img[b][0][lv][0] + first[b] for b in range(B)])           # into the images' concatenation
+        canvas = torch.zeros((sum(s.shape[0] for s in smalls), h, w), dtype=torch.uint8, device=dev)
+        g0 = 0
+        for s in smalls:
+            sh, sw = min(h, s.shape[1]), min(w, s.shape[2])
+            canvas[g0:g0 + s.shape[0], :sh, :sw] = s[:, :sh, :sw]
+            g0 += s.shape[0]
+        return canvas[winner.flatten()[loc]]
+
+    @staticmethod
+    def _graph_leaves(ins_preds, levelset_feats):
+        if isinstance(ins_preds, SoloInsPreds):
+            return [ins_preds.feature_pred, levelset_feats] + [p.kernel_pred for p in ins_preds]
+        return [levelset_feats] + list(ins_preds)
 
     # a2 -- box_solov2_head.py:204-217
     def dynamic_conv(self, feature_pred, kernel_pred, out_size=None, cells=None):

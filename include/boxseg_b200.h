@@ -574,6 +574,29 @@ int bxs_lsap_solve(const void* cost, const int64_t* offset_host, const int64_t* 
                    int64_t num_problems, int dtype, int32_t* match, int32_t* status, void* workspace,
                    bxs_stream_t stream);
 
+/* ---------------------------------------------------------------------------------------
+ * a2  BoxSOLOv2's category loss over every level    replaces the permute / reshape / cat of the category maps and
+ *     FocalLoss(use_sigmoid=True)(preds, labels, avg_factor=num_ins + 1) (box_solov2_head.py:370-383,
+ *     mmdet/models/losses/focal_loss.py, utils.py weight_reduce_loss).
+ * Level l (n_levels): logits_host[l] f32 [B,C,S_l,S_l] in its own NCHW layout (S_l = grid_host[l]), labels_host[l] i64
+ * [B,S_l^2]; a label outside [0, C) makes its cell all-negative (C is the background label).  avg_factor: f32 scalar on the
+ * DEVICE.  loss (device f32 scalar) = loss_weight * sum FL(x, t) / (avg_factor + FLT_EPSILON), with FL the numerically
+ * stable form of py_sigmoid_focal_loss: BCE-with-logits (softplus) * (alpha t + (1-alpha)(1-t)) * pt^gamma.
+ * grad_host[l] f32 [B,C,S_l,S_l] (grad_host NULL: not needed) = d loss / d logits in the same pass:
+ *   -alpha (1-p)^gamma (1 - p - gamma p log p) for a positive, -(1-alpha) p^gamma (gamma (1-p) log(1-p) - p) for a
+ *   negative, times loss_weight / (avg_factor + FLT_EPSILON).
+ * Two launches: one CTA per (level, image, 64-cell tile) leaves an FP32 partial, a one-CTA launch sums them in a fixed
+ * order: bit-identical from run to run, no atomics, no host synchronisation.  The *_host arrays are HOST arrays, copied
+ * into kernel parameters.  workspace: bxs_sigmoid_focal_loss_levels_forward_workspace_bytes(grid_host, n_levels, B) bytes
+ * (0 for invalid arguments).  BXS_ERR_INVALID_ARG: a NULL pointer, n_levels, B, C or an S_l <= 0, gamma < 0 or NaN.
+ * BXS_ERR_UNSUPPORTED: n_levels > 8, S_l > 32768.  All checks run before any device call.
+ * --------------------------------------------------------------------------------------- */
+int64_t bxs_sigmoid_focal_loss_levels_forward_workspace_bytes(const int64_t* grid_host, int64_t n_levels, int64_t B);
+int bxs_sigmoid_focal_loss_levels_forward(const float* const* logits_host, const int64_t* const* labels_host,
+                                          const int64_t* grid_host, float* const* grad_host, const float* avg_factor,
+                                          float* loss, void* workspace, int64_t n_levels, int64_t B, int64_t C, float gamma,
+                                          float alpha, float loss_weight, bxs_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
