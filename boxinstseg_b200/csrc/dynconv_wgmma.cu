@@ -20,6 +20,9 @@
 //   warps 0-7: two consumer warpgroups, 64 pixels of a 128-pixel tile each (ld.shared -> wgmma -> global stores)
 //   warp 8   : TMA producer (B once, then a ring of 16 KB A stages)
 // synchronised with mbarriers only (full/empty per stage).
+// Each pipeline loop is written once: dynconv_tf32_body (TF32 pixel streaming) and dynconv_wgrad_body (split-K weight
+// gradient, TF32 or 16-bit) are driven by a job object per kernel that says where its operands and results are.  The
+// host path of each product (forward, backward) is one template over the operand dtype.
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
@@ -51,6 +54,29 @@ struct SmemLayout {
   alignas(8) uint64_t full[STAGES];
   uint64_t empty[STAGES];
   uint64_t b_full;
+};
+
+// elements of one 128-byte swizzle row, the K-block of every TMA box: 32 floats or 64 16-bit values
+template <typename T>
+constexpr int KBLOCK = 128 / (int)sizeof(T);
+
+// the operand dtypes: tensor-map data type, and the rounding of an FP32 result to the dtype (the identity for float)
+template <typename T>
+struct Operand;
+template <>
+struct Operand<float> {
+  static constexpr CUtensorMapDataType tma = CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
+  static __device__ __forceinline__ float round(float x) { return x; }
+};
+template <>
+struct Operand<__half> {
+  static constexpr CUtensorMapDataType tma = CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
+  static __device__ __forceinline__ __half round(float x) { return __float2half_rn(x); }
+};
+template <>
+struct Operand<__nv_bfloat16> {
+  static constexpr CUtensorMapDataType tma = CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
+  static __device__ __forceinline__ __nv_bfloat16 round(float x) { return __float2bfloat16_rn(x); }
 };
 
 __device__ __forceinline__ void tma_load_2d(const CUtensorMap* map, uint64_t* bar, void* dst, int x, int y) {
@@ -162,6 +188,13 @@ __device__ __forceinline__ void wgmma_ss(float (&d)[BN / 2], uint64_t adesc, uin
   else if constexpr (BN == 128) wgmma_ss_n128(d, adesc, bdesc);
   else wgmma_ss_n256(d, adesc, bdesc);
 }
+// the MMA of dynconv_wgrad_body for TF32 operands
+struct Tf32Mma {
+  template <int BN>
+  static __device__ __forceinline__ void mma(float (&d)[BN / 2], uint64_t adesc, uint64_t bdesc) {
+    wgmma_ss<BN>(d, adesc, bdesc);
+  }
+};
 
 // Pixel (inside its 32-pixel box) of accumulator row `r` (0..7) of a warp, for the row group `j` (0..3).  A warp's
 // 16 accumulator rows are two groups j = 2h (rows 0-7) and j = 2h + 1 (rows 8-15) of the box; row r is pixel
@@ -172,8 +205,8 @@ __device__ __forceinline__ float lds_box(const uint8_t* box, int k, int p) {
   return *reinterpret_cast<const float*>(box + k * 128 + ((((p >> 2) ^ (k & 7))) << 4) + (p & 3) * 4);
 }
 
-// The pixel-streaming loop of dynconv_tf32_kernel for the problem-table kernels below (dynconv_tf32_kernel keeps its
-// own, so that its code generation stays exactly as measured).  `job` says where its operands and results are:
+// The pixel-streaming loop of the positive-cell forward and d/d operand kernels (dynconv_tf32_kernel writes it out; see
+// there).  `job` says where its operands and results are:
 //   job.C, job.P, job.I  : channels (the reduction), pixels, kernels of the job's problem
 //   job.kmap, job.krow<BN>(): B = rows [krow, krow + BN) of the 2-D kernel map, K-blocks of 32 channels, resident
 //   job.load_a(bar, dst, pixel, kb): the [32 channels][32 pixels] box of K-block kb at `pixel`
@@ -280,6 +313,9 @@ struct DenseOut {
 
 // grid: (ctas_per_group, B * n_chunks).  CTA (x, g): image b = g / n_chunks, kernel chunk g % n_chunks of BN kernels,
 // pixel tiles x, x + gridDim.x, ...
+// The loop is dynconv_tf32_body's, written out: run on dynconv_tf32_body through a job object, this kernel compiles to
+// different address arithmetic and fragment-load order, and at BN = 32 it measured 1.3-2 % slower (H100 80GB HBM3,
+// 700 W power limit, I = 16 at 200 x 256 pixels).
 template <int BN>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 dynconv_tf32_kernel(const __grid_constant__ CUtensorMap tm_feat, const __grid_constant__ CUtensorMap tm_kern,
@@ -349,22 +385,7 @@ dynconv_tf32_kernel(const __grid_constant__ CUtensorMap tm_feat, const __grid_co
         if (lane == 0) mbar_arrive(&S.empty[stage]);
         if (++stage == STAGES) { stage = 0; phase ^= 1; }
       }
-      // accumulator elements 4 j .. 4 j + 3: kernels n = 8 j + 2 c4 + {0, 1} of rows r (pixel p0) and r + 8 (pixel p1)
-      const int pix = mt * BLOCK_M + box * 32;
-      const bool in0 = pix + p0 < P, in1 = pix + p1 < P;
-      float* dst = out + ((int64_t)b * I + chunk * BN + 2 * c4) * P + pix;
-      int n = chunk * BN + 2 * c4;
-#pragma unroll
-      for (int j = 0; j < BN / 8; ++j, n += 8, dst += 8 * (int64_t)P) {
-        if (n < I) {
-          if (in0) dst[p0] = acc[4 * j];
-          if (in1) dst[p1] = acc[4 * j + 2];
-        }
-        if (n + 1 < I) {
-          if (in0) dst[P + p0] = acc[4 * j + 1];
-          if (in1) dst[P + p1] = acc[4 * j + 3];
-        }
-      }
+      DenseOut{out, P, I, b, chunk}.store<BN>(acc, mt, box, p0, p1, c4);
     }
   }
 }
@@ -385,40 +406,32 @@ EncodeTiledFn encode_fn() {
   return fn;
 }
 
-// row-major [rows, cols] float32 matrix, box = [box_rows, 32 floats], 128-byte swizzle, zero fill out of bounds
-bool make_map(CUtensorMap* map, const float* base, int64_t rows, int64_t cols, int box_rows) {
+// The tensor map of a row-major [batch, rows, cols] tensor of T, box = [1, box_rows, KBLOCK<T> columns = 128 bytes],
+// 128-byte swizzle, zero fill out of bounds.  Rank 3: rows beyond `rows` of a batch entry are OUT OF BOUNDS and read as
+// zeros (a 2-D [batch * rows, cols] view would run into the next entry instead).  Rank 2: the [rows, cols] matrix of a
+// batch of 1, for kernels that issue 2-D loads.  false, with the last error set, when the driver cannot encode it.
+template <typename T>
+bool make_map(CUtensorMap* map, int rank, const T* base, int64_t batch, int64_t rows, int64_t cols, int box_rows) {
   EncodeTiledFn fn = encode_fn();
-  if (!fn) return false;
-  cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
-  cuuint64_t strides[1] = {(cuuint64_t)cols * 4};
-  cuuint32_t box[2] = {32, (cuuint32_t)box_rows};
-  cuuint32_t estr[2] = {1, 1};
-  return fn(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(base), dims, strides, box, estr,
-            CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-            CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
-}
-
-// [batch, rows, cols] float32 tensor, box = [1, box_rows, 32 floats], 128-byte swizzle: rows beyond `rows` of a batch
-// entry are OUT OF BOUNDS and read as zeros (a 2-D [batch * rows, cols] view would run into the next entry instead)
-bool make_map3(CUtensorMap* map, const float* base, int64_t batch, int64_t rows, int64_t cols, int box_rows) {
-  EncodeTiledFn fn = encode_fn();
-  if (!fn) return false;
-  cuuint64_t dims[3] = {(cuuint64_t)cols, (cuuint64_t)rows, (cuuint64_t)batch};
-  cuuint64_t strides[2] = {(cuuint64_t)cols * 4, (cuuint64_t)cols * (cuuint64_t)rows * 4};
-  cuuint32_t box[3] = {32, (cuuint32_t)box_rows, 1};
-  cuuint32_t estr[3] = {1, 1, 1};
-  return fn(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(base), dims, strides, box, estr,
-            CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-            CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+  const cuuint64_t dims[3] = {(cuuint64_t)cols, (cuuint64_t)rows, (cuuint64_t)batch};
+  const cuuint64_t strides[2] = {(cuuint64_t)cols * sizeof(T), (cuuint64_t)cols * (cuuint64_t)rows * sizeof(T)};
+  const cuuint32_t box[3] = {KBLOCK<T>, (cuuint32_t)box_rows, 1}, estr[3] = {1, 1, 1};
+  if (fn && fn(map, Operand<T>::tma, rank, const_cast<T*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+               CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+               CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS)
+    return true;
+  set_last_error(cudaErrorNotSupported);
+  return false;
 }
 
 // kT[b, c, i] = kernels[b, i, c] for i < I, 0 for I <= i < Ipad   (the K-major B operand of d/d feat = K^T . G)
-__global__ void transpose_pad_kernel(const float* __restrict__ k, float* __restrict__ kt, int I, int C, int Ipad, int64_t total) {
+template <typename T>
+__global__ void transpose_pad_kernel(const T* __restrict__ k, T* __restrict__ kt, int I, int C, int Ipad, int64_t total) {
   for (int64_t idx = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; idx < total; idx += (int64_t)gridDim.x * blockDim.x) {
     const int i = (int)(idx % Ipad);
     const int c = (int)((idx / Ipad) % C);
     const int64_t b = idx / ((int64_t)Ipad * C);
-    kt[idx] = i < I ? __ldg(k + (b * I + i) * C + c) : 0.f;
+    kt[idx] = i < I ? __ldg(k + (b * I + i) * C + c) : T();
   }
 }
 
@@ -427,13 +440,14 @@ __global__ void transpose_pad_kernel(const float* __restrict__ k, float* __restr
 // tiny output (I x C).  Both operands are K-major (the pixel index is contiguous in g and in feat), so wgmma reads both
 // from shared memory with the 128-byte swizzle.  Split-K: CTA (split, b * chunks + chunk) reduces pixels [p0, p1) of
 // image b for 128 rows of g (64 per consumer warpgroup) into a 128 x C register accumulator (C <= 256 columns) and
-// stores it as a partial; dynconv_wgrad_reduce sums the partials in split order (deterministic).
+// stores it as a partial; dynconv_wgrad_reduce sums the partials in split order (deterministic).  A stage holds one
+// K-block of pixels, one 128-byte swizzle row: 32 pixels for TF32 operands, 64 for 16-bit ones.
 //   warps 0-7: two consumer warpgroups (wgmma, epilogue)
-//   warp 8   : TMA producer (A = g tile 128 x 32, B = feat tile C x 32 per stage, 4 stages)
+//   warp 8   : TMA producer (A = g tile 128 rows x 128 bytes, B = feat tile C rows x 128 bytes per stage, 4 stages)
 // =====================================================================================================================
 constexpr int WG_STAGES = 4;
-constexpr int WG_A_BYTES = 128 * BLOCK_K * 4;      // 16 KB
-constexpr int WG_B_BYTES = 256 * BLOCK_K * 4;      // 32 KB
+constexpr int WG_A_BYTES = 128 * 128;              // 16 KB
+constexpr int WG_B_BYTES = 256 * 128;              // 32 KB
 
 struct WgSmem {
   alignas(1024) uint8_t a[WG_STAGES][WG_A_BYTES];
@@ -443,11 +457,12 @@ struct WgSmem {
 };
 
 // The split-K loop of one CTA.  `job`:
-//   job.C, job.kb0, job.kb1     : columns of the result (rows of B), the job's K-blocks of 32 pixels
-//   job.load_g(bar, dst, kb)    : A = 128 rows of g x 32 pixels;  job.load_f(bar, dst, kb): B = C rows x 32 pixels
+//   job.C, job.kb0, job.kb1     : columns of the result (rows of B), the job's K-blocks of pixels
+//   job.load_g(bar, dst, kb)    : A = 128 rows of g x 1 K-block;  job.load_f(bar, dst, kb): B = C rows x 1 K-block
 //   job.template store<BN>(acc, wg, w, r, c4): the accumulator of a warp (see DenseWgJob)
+// Mma::template mma<BN>(acc, adesc, bdesc): the wgmma over 32 bytes of K of both (K-major) operands, TF32 or 16-bit.
 // BN: C rounded up to 32, 64, 128 or 256 (the columns beyond C are computed from unused shared memory and dropped)
-template <int BN, class Job>
+template <int BN, class Mma, class Job>
 __device__ __forceinline__ void dynconv_wgrad_body(const Job& job) {
   extern __shared__ uint8_t smem_raw[];
   WgSmem& S = *reinterpret_cast<WgSmem*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -462,7 +477,7 @@ __device__ __forceinline__ void dynconv_wgrad_body(const Job& job) {
       int stage = 0, phase = 0;
       for (int kb = job.kb0; kb < job.kb1; ++kb) {
         mbar_wait(&S.empty[stage], phase ^ 1);
-        mbar_expect_tx(&S.full[stage], WG_A_BYTES + (uint32_t)job.C * BLOCK_K * 4);
+        mbar_expect_tx(&S.full[stage], WG_A_BYTES + (uint32_t)job.C * 128);
         job.load_g(&S.full[stage], S.a[stage], kb);
         job.load_f(&S.full[stage], S.b[stage], kb);
         if (++stage == WG_STAGES) { stage = 0; phase ^= 1; }
@@ -479,8 +494,7 @@ __device__ __forceinline__ void dynconv_wgrad_body(const Job& job) {
       const uint32_t a_base = smem_u32(S.a[stage]) + wg * (64 * 128), b_base = smem_u32(S.b[stage]);
       wgmma_fence();
 #pragma unroll
-      for (int k4 = 0; k4 < BLOCK_K / MMA_K; ++k4)
-        wgmma_ss<BN>(acc, make_desc(a_base + k4 * (MMA_K * 4)), make_desc(b_base + k4 * (MMA_K * 4)));
+      for (int k = 0; k < 128 / 32; ++k) Mma::template mma<BN>(acc, make_desc(a_base + k * 32), make_desc(b_base + k * 32));
       wgmma_commit();
       wgmma_wait_all();
       fence_acc(acc);
@@ -492,17 +506,26 @@ __device__ __forceinline__ void dynconv_wgrad_body(const Job& job) {
   }
 }
 
-// bxs_dynconv1x1_backward: rows [128 chunk, 128 chunk + 128) of g [B,I,P] of image b, pixels of split `split`
+// the dense d/d kernel: rows [128 chunk, 128 chunk + 128) of g [B,I,P] of image b = blockIdx.y / chunks, chunk =
+// blockIdx.y % chunks, the pixels of split `split` = blockIdx.x in K-blocks of BK pixels
+template <int BK>
 struct DenseWgJob {
   const CUtensorMap* g;
   const CUtensorMap* feat;
   float* partial;
   int C, I, b, chunk, split, splits, kb0, kb1;
+  __device__ __forceinline__ DenseWgJob(const CUtensorMap& tm_g, const CUtensorMap& tm_feat, float* partial_, int C_, int P,
+                                        int I_, int chunks, int splits_, int kb_per_split)
+      : g(&tm_g), feat(&tm_feat), partial(partial_), C(C_), I(I_), b(blockIdx.y / chunks), chunk(blockIdx.y % chunks),
+        split(blockIdx.x), splits(splits_) {
+    kb0 = split * kb_per_split;
+    kb1 = min(kb0 + kb_per_split, (P + BK - 1) / BK);
+  }
   __device__ __forceinline__ void load_g(uint64_t* bar, void* dst, int kb) const {
-    tma_load_3d(g, bar, dst, kb * BLOCK_K, chunk * 128, b);       // rows >= I: zeros
+    tma_load_3d(g, bar, dst, kb * BK, chunk * 128, b);       // rows >= I: zeros
   }
   __device__ __forceinline__ void load_f(uint64_t* bar, void* dst, int kb) const {
-    tma_load_3d(feat, bar, dst, kb * BLOCK_K, 0, b);
+    tma_load_3d(feat, bar, dst, kb * BK, 0, b);
   }
   // accumulator elements (i, i + 1), i even: row 16 w + r (+ 8 when i % 4 == 2), columns 8 (i / 4) + 2 c4 + {0, 1}
   template <int BN>
@@ -521,148 +544,50 @@ template <int BN>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 dynconv_wgrad_kernel(const __grid_constant__ CUtensorMap tm_g, const __grid_constant__ CUtensorMap tm_feat,
                      float* __restrict__ partial, int C, int P, int I, int chunks, int splits, int kb_per_split) {
-  const int split = blockIdx.x, b = blockIdx.y / chunks, chunk = blockIdx.y % chunks;
-  const int kb_total = (P + BLOCK_K - 1) / BLOCK_K;
-  const int kb0 = split * kb_per_split, kb1 = min(kb0 + kb_per_split, kb_total);
-  const DenseWgJob job{&tm_g, &tm_feat, partial, C, I, b, chunk, split, splits, kb0, kb1};
-  dynconv_wgrad_body<BN>(job);
+  dynconv_wgrad_body<BN, Tf32Mma>(DenseWgJob<BLOCK_K>(tm_g, tm_feat, partial, C, P, I, chunks, splits, kb_per_split));
 }
 
-__global__ void dynconv_wgrad_reduce(const float* __restrict__ partial, float* __restrict__ out, int splits, int64_t per_image,
+// out[b, r] = the partials of image b summed in split order (deterministic), rounded to the operand dtype
+template <typename T>
+__global__ void dynconv_wgrad_reduce(const float* __restrict__ partial, T* __restrict__ out, int splits, int64_t per_image,
                                      int64_t total) {
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
     const int64_t b = i / per_image, r = i - b * per_image;
     const float* p = partial + b * splits * per_image + r;
     float acc = 0.f;
     for (int s = 0; s < splits; ++s) acc += p[(int64_t)s * per_image];          // split order: deterministic
-    out[i] = acc;
+    out[i] = Operand<T>::round(acc);
   }
-}
-
-// out[b, i, p] for i in [0, I): kernels `tm_kern` ([B * I, C], boxes of BN rows), features `tm_feat` ([B, C, P])
-template <int BN>
-int launch_forward(const CUtensorMap& tm_feat, const CUtensorMap& tm_kern, float* out, int64_t B, int64_t C, int64_t P,
-                   int64_t I, cudaStream_t st) {
-  const int n_chunks = (int)ceil_div(I, BN);
-  const int64_t groups = B * n_chunks;
-  if (groups > 65535) return BXS_ERR_UNSUPPORTED;
-  const int tiles_m = (int)ceil_div(P, BLOCK_M);
-  const int per_group = std::min((int)std::max<int64_t>(1, sm_count() / groups), tiles_m);
-  const size_t smem = sizeof(SmemLayout) + 1024;
-  if (opt_in_smem(dynconv_tf32_kernel<BN>, smem) != BXS_OK) return BXS_ERR_LAUNCH;
-  dynconv_tf32_kernel<BN><<<dim3(per_group, (unsigned)groups), NUM_THREADS, smem, st>>>(tm_feat, tm_kern, out, (int)C,
-                                                                                        (int)P, (int)I, n_chunks);
-  return check_launch();
 }
 
 // the narrowest accumulator that holds I kernels (chunks of 128 beyond that)
 inline int forward_bn(int64_t I) { return I <= 32 ? 32 : I <= 64 ? 64 : 128; }
 
-int dynconv_forward(const float* feat3, int64_t feat_rows, const float* kern, float* out, int64_t B, int64_t C, int64_t P,
-                    int64_t I, cudaStream_t st) {
-  const int bn = forward_bn(I);
-  CUtensorMap tm_feat, tm_kern;
-  if (!make_map3(&tm_feat, feat3, B, feat_rows, P, BLOCK_K) || !make_map(&tm_kern, kern, B * I, C, bn)) {
-    set_last_error(cudaErrorNotSupported);
-    return BXS_ERR_LAUNCH;
-  }
-  if (bn == 32) return launch_forward<32>(tm_feat, tm_kern, out, B, C, P, I, st);
-  if (bn == 64) return launch_forward<64>(tm_feat, tm_kern, out, B, C, P, I, st);
-  return launch_forward<128>(tm_feat, tm_kern, out, B, C, P, I, st);
+// the grid of the pixel-streaming kernels: `groups` rows of CTAs that share the SMs, each row no wider than its `tiles`
+inline dim3 persistent_grid(int64_t groups, int tiles) {
+  return dim3(std::min((int)std::max<int64_t>(1, sm_count() / groups), tiles), (unsigned)groups);
 }
+
+// opts `kern` in to `smem` bytes of dynamic shared memory and launches it with NUM_THREADS threads per CTA
+template <class Kernel, class... Args>
+int launch(Kernel kern, dim3 grid, size_t smem, cudaStream_t st, const Args&... args) {
+  if (opt_in_smem(kern, smem) != BXS_OK) return BXS_ERR_LAUNCH;
+  kern<<<grid, NUM_THREADS, smem, st>>>(args...);
+  return check_launch();
+}
+
+// 1-D grid of the grid-stride kernels (256 threads per CTA)
+inline unsigned stride_grid(int64_t total) { return (unsigned)std::max<int64_t>(1, std::min<int64_t>(ceil_div(total, 256), 1024)); }
+
+template <typename T>
+inline T* align1k(void* p) { return reinterpret_cast<T*>((reinterpret_cast<uintptr_t>(p) + 1023) & ~uintptr_t(1023)); }
+
+inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 
 }  // namespace
 }  // namespace bxs
 
 using namespace bxs;
-
-// feat [B,C,P], kernels [B,I,C] -> out [B,I,P] (all float32, contiguous).  Requirements of the TMA/wgmma path:
-// C % 32 == 0, C <= 256, P % 4 == 0, 16-byte aligned bases.  BXS_ERR_UNSUPPORTED otherwise.
-extern "C" int bxs_dynconv1x1_forward(const float* feat, const float* kernels, float* out, int64_t B, int64_t C, int64_t P,
-                                      int64_t I, bxs_stream_t stream) {
-  if (!feat || !kernels || !out || B <= 0 || C <= 0 || P <= 0 || I <= 0) return BXS_ERR_INVALID_ARG;
-  if (C % BLOCK_K || C > BLOCK_K * MAX_KBLOCKS || P % 4 || (reinterpret_cast<uintptr_t>(feat) & 15) ||
-      (reinterpret_cast<uintptr_t>(kernels) & 15) || B * C >= (int64_t(1) << 31) || B * I >= (int64_t(1) << 31))
-    return BXS_ERR_UNSUPPORTED;
-  return dynconv_forward(feat, C, kernels, out, B, C, P, I, as_stream(stream));
-}
-
-
-// ---------------------------------------------------------------------------------------
-// backward of the dynamic 1x1 convolution (the autograd of box_solov2_head.py:209-211, discobox_head.py:1219,
-// box2mask_head.py:345; the reference gets it from cuDNN / cuBLAS)
-//   d/d feat  [B,C,P] = K^T . G : the FORWARD kernel with the roles swapped -- "feat" := g_out [B,I,P] (its rows beyond I
-//       read as zeros through the 3-D tensor map), "kernels" := K^T zero-padded to a multiple of 32 instances
-//       (transpose_pad_kernel, in the workspace).  I <= 256.
-//   d/d kernel [B,I,C] = G . F^T : dynconv_wgrad_kernel (split-K) + dynconv_wgrad_reduce.
-// workspace: bxs_dynconv1x1_backward_workspace_bytes(B, C, P, I) bytes.
-// ---------------------------------------------------------------------------------------
-namespace {
-inline int wg_splits(int64_t B, int64_t P, int64_t I, int block_k = BLOCK_K) {
-  const int64_t chunks = ceil_div(I, 128), kb_total = ceil_div(P, block_k);
-  int64_t s = std::max<int64_t>(1, (2 * (int64_t)sm_count()) / (B * chunks));
-  s = std::min<int64_t>(s, std::max<int64_t>(1, kb_total / (256 / block_k)));   // at least 256 pixels per CTA
-  return (int)s;
-}
-
-template <int BN>
-int launch_wgrad(const CUtensorMap& tm_g, const CUtensorMap& tm_f, float* partial, int64_t B, int64_t C, int64_t P,
-                 int64_t I, int chunks, int splits, int kb_per, cudaStream_t st) {
-  const size_t smem = sizeof(WgSmem) + 1024;
-  if (opt_in_smem(dynconv_wgrad_kernel<BN>, smem) != BXS_OK) return BXS_ERR_LAUNCH;
-  dynconv_wgrad_kernel<BN><<<dim3((unsigned)splits, (unsigned)(B * chunks)), NUM_THREADS, smem, st>>>(
-      tm_g, tm_f, partial, (int)C, (int)P, (int)I, chunks, splits, kb_per);
-  return check_launch();
-}
-}  // namespace
-
-extern "C" int64_t bxs_dynconv1x1_backward_workspace_bytes(int64_t B, int64_t C, int64_t P, int64_t I) {
-  if (B <= 0 || C <= 0 || P <= 0 || I <= 0) return 0;
-  const int64_t ipad = ceil_div(I, 32) * 32;
-  return 4 * B * C * ipad + 1024 + 4 * B * (int64_t)wg_splits(B, P, I) * I * C + 1024;
-}
-
-extern "C" int bxs_dynconv1x1_backward(const float* feat, const float* kernels, const float* g_out, float* g_feat,
-                                       float* g_kernels, void* workspace, int64_t B, int64_t C, int64_t P, int64_t I,
-                                       bxs_stream_t stream) {
-  if (!feat || !kernels || !g_out || (!g_feat && !g_kernels) || !workspace || B <= 0 || C <= 0 || P <= 0 || I <= 0)
-    return BXS_ERR_INVALID_ARG;
-  if (C % BLOCK_K || C > BLOCK_K * MAX_KBLOCKS || P % 4 || (g_feat && I > 256) || (reinterpret_cast<uintptr_t>(feat) & 15) ||
-      (reinterpret_cast<uintptr_t>(g_out) & 15) || (reinterpret_cast<uintptr_t>(kernels) & 15))
-    return BXS_ERR_UNSUPPORTED;
-  cudaStream_t st = as_stream(stream);
-  const int64_t ipad = ceil_div(I, 32) * 32;
-  float* kt = reinterpret_cast<float*>((reinterpret_cast<uintptr_t>(workspace) + 1023) & ~uintptr_t(1023));
-  float* partial = reinterpret_cast<float*>((reinterpret_cast<uintptr_t>(kt + B * C * ipad) + 1023) & ~uintptr_t(1023));
-  if (g_feat) {
-    const int64_t total = B * C * ipad;
-    transpose_pad_kernel<<<(unsigned)std::min<int64_t>(ceil_div(total, 256), 1024), 256, 0, st>>>(kernels, kt, (int)I, (int)C,
-                                                                                                  (int)ipad, total);
-    // out[b, c, p] = sum_i kT[b, c, i] * g[b, i, p]: "C" := I (zero-filled up to ipad), "I" := C
-    int rc = dynconv_forward(g_out, I, kt, g_feat, B, ipad, P, C, st);
-    if (rc != BXS_OK) return rc;
-  }
-  if (g_kernels) {
-    const int chunks = (int)ceil_div(I, 128), splits = wg_splits(B, P, I);
-    const int kb_total = (int)ceil_div(P, BLOCK_K), kb_per = (int)ceil_div(kb_total, splits);
-    CUtensorMap tm_g, tm_f;
-    if (!make_map3(&tm_g, g_out, B, I, P, 128) || !make_map3(&tm_f, feat, B, C, P, (int)C)) {
-      set_last_error(cudaErrorNotSupported);
-      return BXS_ERR_LAUNCH;
-    }
-    int rc = C <= 32    ? launch_wgrad<32>(tm_g, tm_f, partial, B, C, P, I, chunks, splits, kb_per, st)
-             : C <= 64  ? launch_wgrad<64>(tm_g, tm_f, partial, B, C, P, I, chunks, splits, kb_per, st)
-             : C <= 128 ? launch_wgrad<128>(tm_g, tm_f, partial, B, C, P, I, chunks, splits, kb_per, st)
-                        : launch_wgrad<256>(tm_g, tm_f, partial, B, C, P, I, chunks, splits, kb_per, st);
-    if (rc != BXS_OK) return rc;
-    const int64_t total = B * I * C;
-    dynconv_wgrad_reduce<<<(unsigned)std::min<int64_t>(ceil_div(total, 256), 1024), 256, 0, st>>>(partial, g_kernels, splits,
-                                                                                                  I * C, total);
-    rc = check_launch();
-    if (rc != BXS_OK) return rc;
-  }
-  return BXS_OK;
-}
 
 
 // =====================================================================================================================
@@ -880,7 +805,7 @@ template <int BN>
 __global__ void __launch_bounds__(NUM_THREADS, 1) dynconv_cells_wgrad_kernel(const __grid_constant__ CellsPlan pl,
                                                                              float* __restrict__ partial) {
   const CellsWgJob job(pl, partial);
-  dynconv_wgrad_body<BN>(job);
+  dynconv_wgrad_body<BN, Tf32Mma>(job);
 }
 
 // d kernel_pred[l][b, c, cell] = the split-ordered sum of the partials of the positive cell's row, 0 for other cells.
@@ -983,28 +908,6 @@ int cells_wgrad_splits(CellsPlan& pl) {
                                                           std::max(1, kb_min / (256 / BLOCK_K))));
   return chunks;
 }
-
-inline float* align1k(void* p) { return reinterpret_cast<float*>((reinterpret_cast<uintptr_t>(p) + 1023) & ~uintptr_t(1023)); }
-
-inline unsigned stride_grid(int64_t total) { return (unsigned)std::max<int64_t>(1, std::min<int64_t>(ceil_div(total, 256), 1024)); }
-
-template <int BN>
-int launch_cells_forward(const CellsPlan& pl, int groups, int per_group, cudaStream_t st) {
-  const size_t smem = sizeof(SmemLayout) + 1024;
-  if (opt_in_smem(dynconv_cells_kernel<BN>, smem) != BXS_OK) return BXS_ERR_LAUNCH;
-  dynconv_cells_kernel<BN><<<dim3(per_group, groups), NUM_THREADS, smem, st>>>(pl);
-  return check_launch();
-}
-
-template <int BN>
-int launch_cells_wgrad(const CellsPlan& pl, float* partial, int chunks, cudaStream_t st) {
-  const size_t smem = sizeof(WgSmem) + 1024;
-  if (opt_in_smem(dynconv_cells_wgrad_kernel<BN>, smem) != BXS_OK) return BXS_ERR_LAUNCH;
-  dynconv_cells_wgrad_kernel<BN><<<dim3(pl.splits, chunks), NUM_THREADS, smem, st>>>(pl, partial);
-  return check_launch();
-}
-
-inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 }  // namespace
 }  // namespace bxs
 
@@ -1049,25 +952,18 @@ extern "C" int bxs_dynconv1x1_cells_forward(const float* const* operands_host, c
   }
   pl.chunk0[n_ops * B] = groups;
   if (groups > 65535) return BXS_ERR_UNSUPPORTED;
-  float* kpack = align1k(workspace);
+  float* kpack = align1k<float>(workspace);
   for (int o = 0; o < n_ops; ++o) {
     tiles = std::max(tiles, (int)ceil_div(pl.P[o], BLOCK_M));
-    if (!make_map3(&pl.a[o], operands_host[o], B, C, pl.P[o], BLOCK_K)) {
-      set_last_error(cudaErrorNotSupported);
-      return BXS_ERR_LAUNCH;
-    }
+    if (!make_map(&pl.a[o], 3, operands_host[o], B, C, pl.P[o], BLOCK_K)) return BXS_ERR_LAUNCH;
   }
-  if (!make_map(&pl.b[0], kpack, total, C, bn)) {
-    set_last_error(cudaErrorNotSupported);
-    return BXS_ERR_LAUNCH;
-  }
+  if (!make_map(&pl.b[0], 2, kpack, 1, total, C, bn)) return BXS_ERR_LAUNCH;
   cudaStream_t st = as_stream(stream);
   cells_pack_kernel<<<stride_grid((int64_t)total * C), 256, 0, st>>>(pl, kpack, (int64_t)total * C);
   if ((rc = check_launch()) != BXS_OK) return rc;
-  const int per_group = std::min((int)std::max<int64_t>(1, sm_count() / groups), tiles);
-  if (bn == 32) return launch_cells_forward<32>(pl, groups, per_group, st);
-  if (bn == 64) return launch_cells_forward<64>(pl, groups, per_group, st);
-  return launch_cells_forward<128>(pl, groups, per_group, st);
+  const dim3 grid = persistent_grid(groups, tiles);
+  auto go = [&](auto kernel) { return launch(kernel, grid, sizeof(SmemLayout) + 1024, st, pl); };
+  return bn == 32 ? go(dynconv_cells_kernel<32>) : bn == 64 ? go(dynconv_cells_kernel<64>) : go(dynconv_cells_kernel<128>);
 }
 
 extern "C" int64_t bxs_dynconv1x1_cells_backward_workspace_bytes(const int64_t* op_size_host, const int64_t* grid_host,
@@ -1106,9 +1002,8 @@ extern "C" int bxs_dynconv1x1_cells_backward(const float* const* operands_host, 
   pl.cells = cells;
   cudaStream_t st = as_stream(stream);
   const int chunks = cells_wgrad_splits(pl);         // fills chunk0 / splits of the d/d kernel table
-  float* kt = align1k(workspace);
-  float* partial = align1k(kt + (int64_t)n_ops * B * C * pl.KP);
-  auto fail = []() -> int { set_last_error(cudaErrorNotSupported); return BXS_ERR_LAUNCH; };
+  float* kt = align1k<float>(workspace);
+  float* partial = align1k<float>(kt + (int64_t)n_ops * B * C * pl.KP);
   if (g_operands_host) {
     CellsPlan d = pl;
     for (int o = 0; o < n_ops; ++o) d.out[o] = g_operands_host[o];
@@ -1118,25 +1013,19 @@ extern "C" int bxs_dynconv1x1_cells_backward(const float* const* operands_host, 
     } else {
       for (int l = 0; l < n_levels; ++l) {
         const int n = d.start[(l + 1) * B] - d.start[l * B];
-        if (n && !make_map3(&d.a[l], g_out_host[l], 1, n, d.P[d.op_of(l)], BLOCK_K)) return fail();
+        if (n && !make_map(&d.a[l], 3, g_out_host[l], 1, n, d.P[d.op_of(l)], BLOCK_K)) return BXS_ERR_LAUNCH;
       }
       const int bn = forward_bn(C), n_chunks = (int)ceil_div(C, bn);
-      if (!make_map(&d.b[0], kt, (int64_t)n_ops * B * C, d.KP, bn)) return fail();
+      if (!make_map(&d.b[0], 2, kt, 1, (int64_t)n_ops * B * C, d.KP, bn)) return BXS_ERR_LAUNCH;
       const int64_t total = (int64_t)n_ops * B * C * d.KP;
       cells_pack_t_kernel<<<stride_grid(total), 256, 0, st>>>(d, kt, total);
       if ((rc = check_launch()) != BXS_OK) return rc;
       int tiles = 0;
       for (int o = 0; o < n_ops; ++o) tiles = std::max(tiles, (int)ceil_div(d.P[o], BLOCK_M));
-      const int groups = n_ops * (int)B * n_chunks;
-      const int per_group = std::min((int)std::max<int64_t>(1, sm_count() / groups), tiles);
-      const size_t smem = sizeof(SmemLayout) + 1024;
-      auto launch = [&](auto kern) -> int {
-        if (opt_in_smem(kern, smem) != BXS_OK) return BXS_ERR_LAUNCH;
-        kern<<<dim3(per_group, groups), NUM_THREADS, smem, st>>>(d, n_chunks);
-        return check_launch();
-      };
-      rc = bn == 32 ? launch(dynconv_cells_dgrad_kernel<32>) : bn == 64 ? launch(dynconv_cells_dgrad_kernel<64>)
-                                                                         : launch(dynconv_cells_dgrad_kernel<128>);
+      const dim3 grid = persistent_grid(n_ops * (int)B * n_chunks, tiles);
+      auto go = [&](auto kernel) { return launch(kernel, grid, sizeof(SmemLayout) + 1024, st, d, n_chunks); };
+      rc = bn == 32 ? go(dynconv_cells_dgrad_kernel<32>) : bn == 64 ? go(dynconv_cells_dgrad_kernel<64>)
+                                                                     : go(dynconv_cells_dgrad_kernel<128>);
       if (rc != BXS_OK) return rc;
     }
   }
@@ -1146,14 +1035,16 @@ extern "C" int bxs_dynconv1x1_cells_backward(const float* const* operands_host, 
     if (chunks) {
       for (int l = 0; l < n_levels; ++l) {
         const int n = w.start[(l + 1) * B] - w.start[l * B];
-        if (n && !make_map3(&w.a[l], g_out_host[l], 1, n, w.P[w.op_of(l)], 128)) return fail();
+        if (n && !make_map(&w.a[l], 3, g_out_host[l], 1, n, w.P[w.op_of(l)], 128)) return BXS_ERR_LAUNCH;
       }
       for (int o = 0; o < n_ops; ++o)
-        if (!make_map3(&w.b[o], operands_host[o], B, C, w.P[o], (int)C)) return fail();
-      rc = C <= 32    ? launch_cells_wgrad<32>(w, partial, chunks, st)
-           : C <= 64  ? launch_cells_wgrad<64>(w, partial, chunks, st)
-           : C <= 128 ? launch_cells_wgrad<128>(w, partial, chunks, st)
-                      : launch_cells_wgrad<256>(w, partial, chunks, st);
+        if (!make_map(&w.b[o], 3, operands_host[o], B, C, w.P[o], (int)C)) return BXS_ERR_LAUNCH;
+      const dim3 grid(w.splits, chunks);
+      auto go = [&](auto kernel) { return launch(kernel, grid, sizeof(WgSmem) + 1024, st, w, partial); };
+      rc = C <= 32    ? go(dynconv_cells_wgrad_kernel<32>)
+           : C <= 64  ? go(dynconv_cells_wgrad_kernel<64>)
+           : C <= 128 ? go(dynconv_cells_wgrad_kernel<128>)
+                      : go(dynconv_cells_wgrad_kernel<256>);
       if (rc != BXS_OK) return rc;
     }
     int64_t total = 0;
@@ -1195,19 +1086,6 @@ struct HSmem {
   alignas(8) uint64_t full[H_STAGES];
   uint64_t empty[H_STAGES];
   uint64_t b_full;
-};
-
-template <typename T>
-struct Half16;
-template <>
-struct Half16<__half> {
-  static constexpr CUtensorMapDataType tma = CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
-  static __device__ __forceinline__ __half round(float x) { return __float2half_rn(x); }
-};
-template <>
-struct Half16<__nv_bfloat16> {
-  static constexpr CUtensorMapDataType tma = CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
-  static __device__ __forceinline__ __nv_bfloat16 round(float x) { return __float2bfloat16_rn(x); }
 };
 
 // D[64 x 32] += A[64 x 16] * B[32 x 16]^T, both in shared memory, F16 in, FP32 accumulate; TA = 1: A is MN-major
@@ -1297,6 +1175,14 @@ __device__ __forceinline__ void wgmma16(float (&d)[BN / 2], uint64_t adesc, uint
     else wgmma_bf16_n256<TA>(d, adesc, bdesc);
   }
 }
+// the MMA of dynconv_wgrad_body for 16-bit operands (both K-major)
+template <typename T>
+struct Mma16 {
+  template <int BN>
+  static __device__ __forceinline__ void mma(float (&d)[BN / 2], uint64_t adesc, uint64_t bdesc) {
+    wgmma16<T, BN, 0>(d, adesc, bdesc);
+  }
+};
 
 // wgmma shared-memory descriptor of an MN-major operand with the 128-byte swizzle (PTX ISA, canonical layouts of the
 // matrix descriptor): the layout is ((64 MN elements, m), (8 K rows, k)) with the MN index contiguous, a K row every
@@ -1385,7 +1271,7 @@ dynconv_h_kernel(const __grid_constant__ CUtensorMap tm_feat, const __grid_const
 #pragma unroll
         for (int e = 0; e < 4; ++e) {
           const int n = 8 * j + 2 * c4 + (e & 1), p = 16 * w + r + ((e & 2) ? 8 : 0);
-          *reinterpret_cast<T*>(tile + out_off(n, p)) = Half16<T>::round(acc[4 * j + e]);
+          *reinterpret_cast<T*>(tile + out_off(n, p)) = Operand<T>::round(acc[4 * j + e]);
         }
       }
       warpgroup_bar(wg);
@@ -1400,218 +1286,164 @@ dynconv_h_kernel(const __grid_constant__ CUtensorMap tm_feat, const __grid_const
   }
 }
 
-// kT[b, c, i] = kernels[b, i, c] for i < I, 0 for I <= i < Ipad; the bits are moved as they are (+0 is 0 in both dtypes)
-__global__ void transpose_pad_h_kernel(const uint16_t* __restrict__ k, uint16_t* __restrict__ kt, int I, int C, int Ipad,
-                                       int64_t total) {
-  for (int64_t idx = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; idx < total; idx += (int64_t)gridDim.x * blockDim.x) {
-    const int i = (int)(idx % Ipad);
-    const int c = (int)((idx / Ipad) % C);
-    const int64_t b = idx / ((int64_t)Ipad * C);
-    kt[idx] = i < I ? __ldg(k + (b * I + i) * C + c) : (uint16_t)0;
-  }
-}
-
-// d/d kernel, 16-bit operands: dynconv_wgrad_kernel with 64-pixel stages (A = g: 128 rows x 64 pixels, B = feat:
-// C rows x 64 pixels, both K-major; 4 stages of 48 KB)
-constexpr int HW_STAGES = 4;
-constexpr int HW_A_BYTES = 128 * H_BLOCK_K * 2;    // 16 KB
-constexpr int HW_B_BYTES = 256 * H_BLOCK_K * 2;    // 32 KB
-
-struct HWgSmem {
-  alignas(1024) uint8_t a[HW_STAGES][HW_A_BYTES];
-  alignas(1024) uint8_t b[HW_STAGES][HW_B_BYTES];
-  alignas(8) uint64_t full[HW_STAGES];
-  uint64_t empty[HW_STAGES];
-};
-
+// d/d kernel, 16-bit operands: dynconv_wgrad_kernel with 64-pixel K-blocks
 template <typename T, int BN>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 dynconv_h_wgrad_kernel(const __grid_constant__ CUtensorMap tm_g, const __grid_constant__ CUtensorMap tm_feat,
                        float* __restrict__ partial, int C, int P, int I, int chunks, int splits, int kb_per_split) {
-  extern __shared__ uint8_t smem_raw[];
-  HWgSmem& S = *reinterpret_cast<HWgSmem*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int split = blockIdx.x, b = blockIdx.y / chunks, chunk = blockIdx.y % chunks;
-  const int kb_total = (P + H_BLOCK_K - 1) / H_BLOCK_K;
-  const int kb0 = split * kb_per_split, kb1 = min(kb0 + kb_per_split, kb_total);
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < HW_STAGES; ++s) { mbar_init(&S.full[s], 1); mbar_init(&S.empty[s], CONSUMER_WARPS); }
-    fence_mbarrier_init();
-  }
-  __syncthreads();
-  if (warp == CONSUMER_WARPS) {
-    if (lane == 0) {
-      int stage = 0, phase = 0;
-      for (int kb = kb0; kb < kb1; ++kb) {
-        mbar_wait(&S.empty[stage], phase ^ 1);
-        mbar_expect_tx(&S.full[stage], HW_A_BYTES + (uint32_t)C * H_BLOCK_K * 2);
-        tma_load_3d(&tm_g, &S.full[stage], S.a[stage], kb * H_BLOCK_K, chunk * 128, b);     // rows >= I: zeros
-        tma_load_3d(&tm_feat, &S.full[stage], S.b[stage], kb * H_BLOCK_K, 0, b);
-        if (++stage == HW_STAGES) { stage = 0; phase ^= 1; }
-      }
-    }
-  } else {
-    const int wg = warp >> 2, w = warp & 3, r = lane >> 2, c4 = lane & 3;
-    float acc[BN / 2];
-#pragma unroll
-    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
-    int stage = 0, phase = 0;
-    for (int kb = kb0; kb < kb1; ++kb) {
-      mbar_wait(&S.full[stage], phase);
-      const uint32_t a_base = smem_u32(S.a[stage]) + wg * (64 * 128), b_base = smem_u32(S.b[stage]);
-      wgmma_fence();
-#pragma unroll
-      for (int k = 0; k < H_BLOCK_K / H_MMA_K; ++k)
-        wgmma16<T, BN, 0>(acc, make_desc(a_base + k * (H_MMA_K * 2)), make_desc(b_base + k * (H_MMA_K * 2)));
-      wgmma_commit();
-      wgmma_wait_all();
-      fence_acc(acc);
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&S.empty[stage]);
-      if (++stage == HW_STAGES) { stage = 0; phase ^= 1; }
-    }
-    // accumulator elements (i, i + 1), i even: row 16 w + r (+ 8 when i % 4 == 2), columns 8 (i / 4) + 2 c4 + {0, 1}
-    const int row0 = chunk * 128 + wg * 64 + w * 16 + r;
-    float* dst = partial + (((int64_t)b * splits + split) * I) * C;
-#pragma unroll
-    for (int i = 0; i < BN / 2; i += 2) {
-      const int row = row0 + ((i & 2) ? 8 : 0), n = 8 * (i >> 2) + 2 * c4;
-      if (row < I && n < C) *reinterpret_cast<float2*>(dst + (int64_t)row * C + n) = make_float2(acc[i], acc[i + 1]);
-    }
-  }
+  dynconv_wgrad_body<BN, Mma16<T>>(DenseWgJob<H_BLOCK_K>(tm_g, tm_feat, partial, C, P, I, chunks, splits, kb_per_split));
 }
 
-template <typename T>
-__global__ void dynconv_h_wgrad_reduce(const float* __restrict__ partial, T* __restrict__ out, int splits,
-                                       int64_t per_image, int64_t total) {
-  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
-    const int64_t b = i / per_image, r = i - b * per_image;
-    const float* p = partial + b * splits * per_image + r;
-    float acc = 0.f;
-    for (int s = 0; s < splits; ++s) acc += p[(int64_t)s * per_image];          // split order: deterministic
-    out[i] = Half16<T>::round(acc);
-  }
-}
-
-// [batch, rows, cols] 16-bit tensor, box = [1, box_rows, 64 elements], 128-byte swizzle, zero fill out of bounds.  A
-// 2-D [rows, cols] matrix is the batch == 1 case.
-bool make_map3_h(CUtensorMap* map, CUtensorMapDataType dt, const void* base, int64_t batch, int64_t rows, int64_t cols,
-                 int box_rows) {
-  EncodeTiledFn fn = encode_fn();
-  if (!fn) return false;
-  cuuint64_t dims[3] = {(cuuint64_t)cols, (cuuint64_t)rows, (cuuint64_t)batch};
-  cuuint64_t strides[2] = {(cuuint64_t)cols * 2, (cuuint64_t)cols * (cuuint64_t)rows * 2};
-  cuuint32_t box[3] = {H_BLOCK_K, (cuuint32_t)box_rows, 1};
-  cuuint32_t estr[3] = {1, 1, 1};
-  return fn(map, dt, 3, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-            CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
-}
-
-template <typename T, int BN>
-int launch_forward_h(const CUtensorMap& tm_feat, const CUtensorMap& tm_kern, T* out, int64_t B, int64_t C, int64_t P,
-                     int64_t I, cudaStream_t st) {
-  const int n_chunks = (int)ceil_div(I, BN);
-  const int64_t groups = B * n_chunks;
-  if (groups > 65535) return BXS_ERR_UNSUPPORTED;
-  const int tiles_m = (int)ceil_div(P, BLOCK_M);
-  const int per_group = std::min((int)std::max<int64_t>(1, sm_count() / groups), tiles_m);
-  const size_t smem = sizeof(HSmem) + 1024;
-  if (opt_in_smem(dynconv_h_kernel<T, BN>, smem) != BXS_OK) return BXS_ERR_LAUNCH;
-  dynconv_h_kernel<T, BN><<<dim3(per_group, (unsigned)groups), NUM_THREADS, smem, st>>>(tm_feat, tm_kern, out, (int)C,
-                                                                                       (int)P, (int)I, n_chunks);
-  return check_launch();
-}
-
-// out[b, i, p] = sum_c kern[b, i, c] * feat3[b, c, p] for c < C; rows c >= feat_rows of feat3 read as zeros
-template <typename T>
-int dynconv_forward_h(const T* feat3, int64_t feat_rows, const T* kern, T* out, int64_t B, int64_t C, int64_t P,
-                      int64_t I, cudaStream_t st) {
-  const int bn = forward_bn(I);
-  CUtensorMap tm_feat, tm_kern;
-  if (!make_map3_h(&tm_feat, Half16<T>::tma, feat3, B, feat_rows, P, H_BLOCK_K) ||
-      !make_map3_h(&tm_kern, Half16<T>::tma, kern, 1, B * I, C, bn)) {
-    set_last_error(cudaErrorNotSupported);
-    return BXS_ERR_LAUNCH;
-  }
-  if (bn == 32) return launch_forward_h<T, 32>(tm_feat, tm_kern, out, B, C, P, I, st);
-  if (bn == 64) return launch_forward_h<T, 64>(tm_feat, tm_kern, out, B, C, P, I, st);
-  return launch_forward_h<T, 128>(tm_feat, tm_kern, out, B, C, P, I, st);
-}
-
-template <typename T, int BN>
-int launch_wgrad_h(const CUtensorMap& tm_g, const CUtensorMap& tm_f, float* partial, int64_t B, int64_t C, int64_t P,
-                   int64_t I, int chunks, int splits, int kb_per, cudaStream_t st) {
-  const size_t smem = sizeof(HWgSmem) + 1024;
-  if (opt_in_smem(dynconv_h_wgrad_kernel<T, BN>, smem) != BXS_OK) return BXS_ERR_LAUNCH;
-  dynconv_h_wgrad_kernel<T, BN><<<dim3((unsigned)splits, (unsigned)(B * chunks)), NUM_THREADS, smem, st>>>(
-      tm_g, tm_f, partial, (int)C, (int)P, (int)I, chunks, splits, kb_per);
-  return check_launch();
-}
-
-template <typename T>
-int dynconv_backward_h(const T* feat, const T* kernels, const T* g_out, T* g_feat, T* g_kernels, void* workspace,
-                       int64_t B, int64_t C, int64_t P, int64_t I, cudaStream_t st) {
-  const int64_t ipad = ceil_div(I, 32) * 32;
-  T* kt = reinterpret_cast<T*>((reinterpret_cast<uintptr_t>(workspace) + 1023) & ~uintptr_t(1023));
-  float* partial = reinterpret_cast<float*>((reinterpret_cast<uintptr_t>(kt + B * C * ipad) + 1023) & ~uintptr_t(1023));
-  if (g_feat) {
-    const int64_t total = B * C * ipad;
-    transpose_pad_h_kernel<<<(unsigned)std::min<int64_t>(ceil_div(total, 256), 1024), 256, 0, st>>>(
-        reinterpret_cast<const uint16_t*>(kernels), reinterpret_cast<uint16_t*>(kt), (int)I, (int)C, (int)ipad, total);
-    // out[b, c, p] = sum_i kT[b, c, i] * g[b, i, p]: "C" := I (zero-filled up to the k-block), "I" := C
-    int rc = dynconv_forward_h<T>(g_out, I, kt, g_feat, B, ipad, P, C, st);
-    if (rc != BXS_OK) return rc;
-  }
-  if (g_kernels) {
-    const int chunks = (int)ceil_div(I, 128), splits = wg_splits(B, P, I, H_BLOCK_K);
-    const int kb_total = (int)ceil_div(P, H_BLOCK_K), kb_per = (int)ceil_div(kb_total, splits);
-    CUtensorMap tm_g, tm_f;
-    if (!make_map3_h(&tm_g, Half16<T>::tma, g_out, B, I, P, 128) || !make_map3_h(&tm_f, Half16<T>::tma, feat, B, C, P, (int)C)) {
-      set_last_error(cudaErrorNotSupported);
-      return BXS_ERR_LAUNCH;
-    }
-    int rc = C <= 32    ? launch_wgrad_h<T, 32>(tm_g, tm_f, partial, B, C, P, I, chunks, splits, kb_per, st)
-             : C <= 64  ? launch_wgrad_h<T, 64>(tm_g, tm_f, partial, B, C, P, I, chunks, splits, kb_per, st)
-             : C <= 128 ? launch_wgrad_h<T, 128>(tm_g, tm_f, partial, B, C, P, I, chunks, splits, kb_per, st)
-                        : launch_wgrad_h<T, 256>(tm_g, tm_f, partial, B, C, P, I, chunks, splits, kb_per, st);
-    if (rc != BXS_OK) return rc;
-    const int64_t total = B * I * C;
-    dynconv_h_wgrad_reduce<T><<<(unsigned)std::min<int64_t>(ceil_div(total, 256), 1024), 256, 0, st>>>(
-        partial, g_kernels, splits, I * C, total);
-    rc = check_launch();
-    if (rc != BXS_OK) return rc;
-  }
-  return BXS_OK;
-}
-
-inline bool misaligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) != 0; }
-inline bool known_half(int dtype) { return dtype == BXS_F16 || dtype == BXS_BF16; }
 // the envelope of the 16-bit kernels: TMA needs 16-byte row strides (P % 8) and bases; the output tile is written in
 // 16-byte pieces
 inline bool half_shape_ok(int64_t B, int64_t C, int64_t P, int64_t I) {
   return C % 32 == 0 && C <= H_BLOCK_K * H_MAX_KBLOCKS && P % 8 == 0 && B * C < (int64_t(1) << 31) &&
          B * I < (int64_t(1) << 31);
 }
+inline bool known_half(int dtype) { return dtype == BXS_F16 || dtype == BXS_BF16; }
+
+// =====================================================================================================================
+// The dense products for every operand dtype: float runs the TF32 kernels, __half and __nv_bfloat16 the 16-bit ones.
+//   forward    [B,I,P] = K . F
+//   d/d feat   [B,C,P] = K^T . G : the FORWARD kernel with the roles swapped -- "feat" := g_out [B,I,P] (its rows beyond
+//       I read as zeros through the 3-D tensor map), "kernels" := K^T zero-padded to a multiple of 32 instances
+//       (transpose_pad_kernel, in the workspace).  I <= 256.
+//   d/d kernel [B,I,C] = G . F^T : the split-K wgrad kernel + dynconv_wgrad_reduce.
+// (the autograd of box_solov2_head.py:209-211, discobox_head.py:1219, box2mask_head.py:345; the reference gets it from
+// cuDNN / cuBLAS)
+// =====================================================================================================================
+
+// the kernels of operand dtype T
+template <typename T>
+struct Kernels {
+  template <int BN> static constexpr auto fwd = dynconv_h_kernel<T, BN>;
+  template <int BN> static constexpr auto wgrad = dynconv_h_wgrad_kernel<T, BN>;
+  static constexpr size_t fwd_smem = sizeof(HSmem) + 1024;
+  static constexpr int kmap_rank = 3;                 // dynconv_h_kernel loads B with 3-D TMA
+};
+template <>
+struct Kernels<float> {
+  template <int BN> static constexpr auto fwd = dynconv_tf32_kernel<BN>;
+  template <int BN> static constexpr auto wgrad = dynconv_wgrad_kernel<BN>;
+  static constexpr size_t fwd_smem = sizeof(SmemLayout) + 1024;
+  static constexpr int kmap_rank = 2;                 // dynconv_tf32_body loads B with 2-D TMA
+};
+
+// out[b, i, p] = sum_c kern[b, i, c] * feat3[b, c, p] for c < C; rows c >= feat_rows of feat3 read as zeros
+template <typename T>
+int dynconv_forward(const T* feat3, int64_t feat_rows, const T* kern, T* out, int64_t B, int64_t C, int64_t P, int64_t I,
+                    cudaStream_t st) {
+  using K = Kernels<T>;
+  const int bn = forward_bn(I), n_chunks = (int)ceil_div(I, bn);
+  CUtensorMap tm_feat, tm_kern;
+  if (!make_map(&tm_feat, 3, feat3, B, feat_rows, P, KBLOCK<T>) || !make_map(&tm_kern, K::kmap_rank, kern, 1, B * I, C, bn))
+    return BXS_ERR_LAUNCH;
+  const int64_t groups = B * n_chunks;
+  if (groups > 65535) return BXS_ERR_UNSUPPORTED;
+  const dim3 grid = persistent_grid(groups, (int)ceil_div(P, BLOCK_M));
+  auto go = [&](auto kernel) {
+    return launch(kernel, grid, K::fwd_smem, st, tm_feat, tm_kern, out, (int)C, (int)P, (int)I, n_chunks);
+  };
+  return bn == 32 ? go(K::template fwd<32>) : bn == 64 ? go(K::template fwd<64>) : go(K::template fwd<128>);
+}
+
+// d/d kernel split count: about 2 CTAs per SM, at least 256 pixels per CTA
+inline int wg_splits(int64_t B, int64_t P, int64_t I, int block_k) {
+  const int64_t chunks = ceil_div(I, 128), kb_total = ceil_div(P, block_k);
+  int64_t s = std::max<int64_t>(1, (2 * (int64_t)sm_count()) / (B * chunks));
+  s = std::min<int64_t>(s, std::max<int64_t>(1, kb_total / (256 / block_k)));   // at least 256 pixels per CTA
+  return (int)s;
+}
+
+// the workspace of dynconv_backward<T>: K^T padded to 32 instances, then the FP32 partials of the split-K d/d kernel
+template <typename T>
+int64_t backward_workspace_bytes(int64_t B, int64_t C, int64_t P, int64_t I) {
+  const int64_t ipad = ceil_div(I, 32) * 32;
+  return (int64_t)sizeof(T) * B * C * ipad + 1024 + 4 * B * (int64_t)wg_splits(B, P, I, KBLOCK<T>) * I * C + 1024;
+}
+
+template <typename T>
+int dynconv_backward(const T* feat, const T* kernels, const T* g_out, T* g_feat, T* g_kernels, void* workspace, int64_t B,
+                     int64_t C, int64_t P, int64_t I, cudaStream_t st) {
+  const int64_t ipad = ceil_div(I, 32) * 32;
+  T* kt = align1k<T>(workspace);
+  float* partial = align1k<float>(kt + B * C * ipad);
+  if (g_feat) {
+    const int64_t total = B * C * ipad;
+    transpose_pad_kernel<<<stride_grid(total), 256, 0, st>>>(kernels, kt, (int)I, (int)C, (int)ipad, total);
+    // out[b, c, p] = sum_i kT[b, c, i] * g[b, i, p]: "C" := I (zero-filled up to the K-block), "I" := C
+    const int rc = dynconv_forward(g_out, I, kt, g_feat, B, ipad, P, C, st);
+    if (rc != BXS_OK) return rc;
+  }
+  if (g_kernels) {
+    const int chunks = (int)ceil_div(I, 128), splits = wg_splits(B, P, I, KBLOCK<T>);
+    const int kb_per = (int)ceil_div(ceil_div(P, KBLOCK<T>), splits);
+    CUtensorMap tm_g, tm_f;
+    if (!make_map(&tm_g, 3, g_out, B, I, P, 128) || !make_map(&tm_f, 3, feat, B, C, P, (int)C)) return BXS_ERR_LAUNCH;
+    using K = Kernels<T>;
+    const dim3 grid((unsigned)splits, (unsigned)(B * chunks));
+    auto go = [&](auto kernel) {
+      return launch(kernel, grid, sizeof(WgSmem) + 1024, st, tm_g, tm_f, partial, (int)C, (int)P, (int)I, chunks, splits,
+                    kb_per);
+    };
+    int rc = C <= 32    ? go(K::template wgrad<32>)
+             : C <= 64  ? go(K::template wgrad<64>)
+             : C <= 128 ? go(K::template wgrad<128>)
+                        : go(K::template wgrad<256>);
+    if (rc != BXS_OK) return rc;
+    const int64_t total = B * I * C;
+    dynconv_wgrad_reduce<<<stride_grid(total), 256, 0, st>>>(partial, g_kernels, splits, I * C, total);
+    if ((rc = check_launch()) != BXS_OK) return rc;
+  }
+  return BXS_OK;
+}
 }  // namespace
 }  // namespace bxs
+
+// feat [B,C,P], kernels [B,I,C] -> out [B,I,P] (all float32, contiguous).  Requirements of the TMA/wgmma path:
+// C % 32 == 0, C <= 256, P % 4 == 0, 16-byte aligned bases.  BXS_ERR_UNSUPPORTED otherwise.
+extern "C" int bxs_dynconv1x1_forward(const float* feat, const float* kernels, float* out, int64_t B, int64_t C, int64_t P,
+                                      int64_t I, bxs_stream_t stream) {
+  if (!feat || !kernels || !out || B <= 0 || C <= 0 || P <= 0 || I <= 0) return BXS_ERR_INVALID_ARG;
+  if (C % BLOCK_K || C > BLOCK_K * MAX_KBLOCKS || P % 4 || !aligned16(feat) || !aligned16(kernels) ||
+      B * C >= (int64_t(1) << 31) || B * I >= (int64_t(1) << 31))
+    return BXS_ERR_UNSUPPORTED;
+  return dynconv_forward(feat, C, kernels, out, B, C, P, I, as_stream(stream));
+}
+
+// workspace: bxs_dynconv1x1_backward_workspace_bytes(B, C, P, I) bytes
+extern "C" int64_t bxs_dynconv1x1_backward_workspace_bytes(int64_t B, int64_t C, int64_t P, int64_t I) {
+  if (B <= 0 || C <= 0 || P <= 0 || I <= 0) return 0;
+  return backward_workspace_bytes<float>(B, C, P, I);
+}
+
+extern "C" int bxs_dynconv1x1_backward(const float* feat, const float* kernels, const float* g_out, float* g_feat,
+                                       float* g_kernels, void* workspace, int64_t B, int64_t C, int64_t P, int64_t I,
+                                       bxs_stream_t stream) {
+  if (!feat || !kernels || !g_out || (!g_feat && !g_kernels) || !workspace || B <= 0 || C <= 0 || P <= 0 || I <= 0)
+    return BXS_ERR_INVALID_ARG;
+  if (C % BLOCK_K || C > BLOCK_K * MAX_KBLOCKS || P % 4 || (g_feat && I > 256) || !aligned16(feat) || !aligned16(g_out) ||
+      !aligned16(kernels))
+    return BXS_ERR_UNSUPPORTED;
+  return dynconv_backward(feat, kernels, g_out, g_feat, g_kernels, workspace, B, C, P, I, as_stream(stream));
+}
 
 extern "C" int bxs_dynconv1x1_half_forward(const void* feat, const void* kernels, void* out, int64_t B, int64_t C,
                                            int64_t P, int64_t I, int dtype, bxs_stream_t stream) {
   if (!feat || !kernels || !out || B <= 0 || C <= 0 || P <= 0 || I <= 0 || !known_half(dtype)) return BXS_ERR_INVALID_ARG;
-  if (!half_shape_ok(B, C, P, I) || misaligned16(feat) || misaligned16(kernels) || misaligned16(out))
-    return BXS_ERR_UNSUPPORTED;
+  if (!half_shape_ok(B, C, P, I) || !aligned16(feat) || !aligned16(kernels) || !aligned16(out)) return BXS_ERR_UNSUPPORTED;
   cudaStream_t st = as_stream(stream);
   if (dtype == BXS_F16)
-    return dynconv_forward_h(static_cast<const __half*>(feat), C, static_cast<const __half*>(kernels),
-                             static_cast<__half*>(out), B, C, P, I, st);
-  return dynconv_forward_h(static_cast<const __nv_bfloat16*>(feat), C, static_cast<const __nv_bfloat16*>(kernels),
-                           static_cast<__nv_bfloat16*>(out), B, C, P, I, st);
+    return dynconv_forward(static_cast<const __half*>(feat), C, static_cast<const __half*>(kernels),
+                           static_cast<__half*>(out), B, C, P, I, st);
+  return dynconv_forward(static_cast<const __nv_bfloat16*>(feat), C, static_cast<const __nv_bfloat16*>(kernels),
+                         static_cast<__nv_bfloat16*>(out), B, C, P, I, st);
 }
 
+// the same for both 16-bit dtypes
 extern "C" int64_t bxs_dynconv1x1_half_backward_workspace_bytes(int64_t B, int64_t C, int64_t P, int64_t I, int dtype) {
   if (B <= 0 || C <= 0 || P <= 0 || I <= 0 || !known_half(dtype)) return 0;
-  const int64_t ipad = ceil_div(I, 32) * 32;
-  return 2 * B * C * ipad + 1024 + 4 * B * (int64_t)wg_splits(B, P, I, H_BLOCK_K) * I * C + 1024;
+  return backward_workspace_bytes<__half>(B, C, P, I);
 }
 
 extern "C" int bxs_dynconv1x1_half_backward(const void* feat, const void* kernels, const void* g_out, void* g_feat,
@@ -1620,15 +1452,15 @@ extern "C" int bxs_dynconv1x1_half_backward(const void* feat, const void* kernel
   if (!feat || !kernels || !g_out || (!g_feat && !g_kernels) || !workspace || B <= 0 || C <= 0 || P <= 0 || I <= 0 ||
       !known_half(dtype))
     return BXS_ERR_INVALID_ARG;
-  if (!half_shape_ok(B, C, P, I) || (g_feat && I > 256) || misaligned16(feat) || misaligned16(kernels) ||
-      misaligned16(g_out) || misaligned16(g_feat))
+  if (!half_shape_ok(B, C, P, I) || (g_feat && I > 256) || !aligned16(feat) || !aligned16(kernels) || !aligned16(g_out) ||
+      !aligned16(g_feat))
     return BXS_ERR_UNSUPPORTED;
   cudaStream_t st = as_stream(stream);
   if (dtype == BXS_F16)
-    return dynconv_backward_h(static_cast<const __half*>(feat), static_cast<const __half*>(kernels),
-                              static_cast<const __half*>(g_out), static_cast<__half*>(g_feat),
-                              static_cast<__half*>(g_kernels), workspace, B, C, P, I, st);
-  return dynconv_backward_h(static_cast<const __nv_bfloat16*>(feat), static_cast<const __nv_bfloat16*>(kernels),
-                            static_cast<const __nv_bfloat16*>(g_out), static_cast<__nv_bfloat16*>(g_feat),
-                            static_cast<__nv_bfloat16*>(g_kernels), workspace, B, C, P, I, st);
+    return dynconv_backward(static_cast<const __half*>(feat), static_cast<const __half*>(kernels),
+                            static_cast<const __half*>(g_out), static_cast<__half*>(g_feat),
+                            static_cast<__half*>(g_kernels), workspace, B, C, P, I, st);
+  return dynconv_backward(static_cast<const __nv_bfloat16*>(feat), static_cast<const __nv_bfloat16*>(kernels),
+                          static_cast<const __nv_bfloat16*>(g_out), static_cast<__nv_bfloat16*>(g_feat),
+                          static_cast<__nv_bfloat16*>(g_kernels), workspace, B, C, P, I, st);
 }
