@@ -3,7 +3,7 @@ dynamic-conv call sites (a2-a4), on the kernels of libboxseg_b200:
 
   ``BoxSOLOv2Head``       mmdet/models/dense_heads/box_solov2_head.py:204-217 (dynamic conv), :334-367 (loss)
   ``DiscoBoxSOLOv2Head``  mmdet/models/dense_heads/discobox_head.py:1206-1300 (per-image conv, MIL dice, mean-field teacher)
-  ``Box2MaskHead``        mmdet/models/dense_heads/box2mask_head.py:338-359 (mask_pred einsum), :269-335 (loss_single)
+  ``Box2MaskHead``        mmdet/models/dense_heads/box2mask_head.py:338-359 (mask_pred einsum), :192-335 (loss, loss_single)
 
 The mask-loss hot path and its immediate callers are implemented here: the SOLO target builders live in
 ``solo_targets.py`` / ``disco_targets.py`` (f2), the Hungarian front half in ``core/assigner.py`` (f1), DiscoBox's
@@ -513,15 +513,20 @@ def _disco_dice(x, t):
 
 @register(HEADS, partial=True)
 class Box2MaskHead(nn.Module):
-    """Box2Mask head: mask-loss path only."""
+    """Box2Mask head: ``forward`` / ``loss`` / ``loss_single`` with the reference's signatures, and the mask-loss path
+    (``mask_loss_single``, ``mask_loss_layers``).  The decoder modules are the reference constructor's (mmdet installed, or
+    attached by the caller); the standalone constructor builds only the losses and the matcher."""
 
     def __init__(self, in_channels=None, feat_channels=256, out_channels=256, num_things_classes=80, num_stuff_classes=0,
-                 num_queries=100, loss_box=None, loss_mask=None, train_cfg=None, **cfg):
+                 num_queries=100, loss_cls=None, loss_box=None, loss_mask=None, train_cfg=None, **cfg):
         super().__init__()
         self.num_queries = num_queries
         self.num_classes = num_things_classes + num_stuff_classes
         self.train_cfg = train_cfg
         self.cfg = cfg
+        # configs/box2mask/box2mask_r50_lsj_8x2_50e_coco.py:92-97
+        self.loss_cls_cfg = loss_cls or dict(type='CrossEntropyLoss', use_sigmoid=False, loss_weight=2.0, reduction='mean',
+                                             class_weight=[1.0] * self.num_classes + [0.1])
         self.loss_box = build_loss(loss_box or dict(type='BoxProjectionLoss', loss_weight=5.0))
         self.loss_mask = build_loss(loss_mask or dict(type='LevelsetLoss', loss_weight=1.0))
         self.mst = MinimumSpanningTree(TreeFilter2D.norm2_distance)
@@ -530,11 +535,27 @@ class Box2MaskHead(nn.Module):
 
     def _bxs_post_init(self):
         """Also runs after the REFERENCE class's ``__init__`` when mmdet is importable: the matcher of ``get_targets`` is
-        this package's MaskHungarianAssigner, built from the same ``train_cfg['assigner']`` (box2mask_head.py:95-97)."""
+        this package's MaskHungarianAssigner, built from the same ``train_cfg['assigner']`` (box2mask_head.py:95-97), and the
+        classification loss is read from the CrossEntropyLoss module and ``class_weight`` that constructor built (:99-100)."""
         from ...core.assigner import MaskHungarianAssigner      # core imports models.builder: not at module level
         cfg = (getattr(self, 'train_cfg', None) or {}).get('assigner')
         self.hungarian = MaskHungarianAssigner(**{k: v for k, v in cfg.items() if k != 'type'}) if cfg else None
         self.lsap_status = None
+        ref = getattr(self, 'loss_cls', None)
+        if isinstance(ref, nn.Module):
+            cls_cfg = dict(use_sigmoid=ref.use_sigmoid, use_mask=getattr(ref, 'use_mask', False), reduction=ref.reduction,
+                           loss_weight=ref.loss_weight, avg_non_ignore=getattr(ref, 'avg_non_ignore', False),
+                           class_weight=getattr(self, 'class_weight', ref.class_weight))
+        else:
+            cls_cfg = self.loss_cls_cfg
+        if (cls_cfg.get('use_sigmoid', False) or cls_cfg.get('use_mask', False) or cls_cfg.get('reduction', 'mean') != 'mean'
+                or cls_cfg.get('avg_non_ignore', False)):
+            raise NotImplementedError('Box2MaskHead: the classification loss is the softmax cross-entropy with reduction '
+                                      f"'mean' only, got {cls_cfg}")
+        cw = cls_cfg.get('class_weight')
+        self.cls_loss_weight = float(cls_cfg.get('loss_weight', 1.0))
+        self.cls_class_weight = None if cw is None else [float(v) for v in cw]
+        self._class_weight_on = {}                               # device -> [K] tensor, copied once per device
 
     # f1 -- box2mask_head.py:135-189 (get_targets + _get_target_single with MaskPseudoSampler), the reference's signature
     @torch.no_grad()
@@ -549,17 +570,49 @@ class Box2MaskHead(nn.Module):
         An image whose cost matrix holds a NaN (NaN predictions) cannot raise without a synchronisation: its queries come
         back as background (labels = num_classes, mask_weights = 0), its min(Q, G_b) mask_targets rows are placeholders,
         and ``self.lsap_status`` (int32 [B] on the device, 1 for such an image, else 0) keeps the per-image status."""
+        costs = self._costs(cls_scores_list, mask_preds_list, gt_labels_list, gt_masks_list)
+        matches, self.lsap_status = solve_batched(costs)
+        return self._targets_of_matches(matches, mask_preds_list, gt_labels_list, gt_masks_list)[0]
+
+    # f1 -- get_targets of every decoder layer (box2mask_head.py:203-205, 238-241), the matching in one launch
+    @torch.no_grad()
+    def get_targets_layers(self, all_cls_scores, all_mask_preds, gt_labels_list, gt_masks_list, img_metas):
+        """``get_targets`` of every decoder layer: a list with one 6-tuple per layer, each bit for bit what
+        ``get_targets(all_cls_scores[l], all_mask_preds[l], ...)`` returns.  all_cls_scores[l] [B,Q,C+1] (or a list of
+        per-image tensors), all_mask_preds[l] [B,Q,h,w] likewise.  The L*B cost matrices are matched in ONE launch, whose
+        problems (one dependent chain on one warp each) run side by side; nothing is read back to the host.
+        ``self.lsap_status`` becomes int32 [L, B]."""
+        return self._targets_layers(all_cls_scores, all_mask_preds, gt_labels_list, gt_masks_list)[0]
+
+    def _targets_layers(self, all_cls_scores, all_mask_preds, gt_labels_list, gt_masks_list):
+        """(per-layer 6-tuples of ``get_targets``, per-layer lists of the images' positive query indices)."""
+        n_layers, B = len(all_cls_scores), len(gt_labels_list)
+        costs = []
+        for cls_scores, mask_preds in zip(all_cls_scores, all_mask_preds):
+            costs += self._costs([cls_scores[b] for b in range(B)], [mask_preds[b] for b in range(B)], gt_labels_list,
+                                 gt_masks_list)
+        matches, status = solve_batched(costs)
+        self.lsap_status = status.view(n_layers, B)
+        out = [self._targets_of_matches(matches[l * B:(l + 1) * B], [mask_preds[b] for b in range(B)], gt_labels_list,
+                                        gt_masks_list) for l, mask_preds in enumerate(all_mask_preds)]
+        return [o[0] for o in out], [o[1] for o in out]
+
+    def _costs(self, cls_scores_list, mask_preds_list, gt_labels_list, gt_masks_list):
+        """The [Q, G_b] cost matrix of every image (mask_hungarian_assigner.py:92-111 on the low-resolution prediction)."""
         if self.hungarian is None:
             raise RuntimeError('Box2MaskHead.get_targets needs train_cfg with an assigner')
-        Q = self.num_queries
         costs = []
         for cls_score, mask_pred, gt_labels, gt_masks in zip(cls_scores_list, mask_preds_list, gt_labels_list, gt_masks_list):
             if gt_labels.shape[0] and mask_pred.shape[0]:
                 costs.append(self.hungarian.cost_matrix(cls_score, mask_pred, gt_labels, gt_masks, lowres=True))
             else:
                 costs.append(mask_pred.new_zeros((mask_pred.shape[0], gt_labels.shape[0])))
-        matches, self.lsap_status = solve_batched(costs)
-        labels_list, label_weights_list, mask_targets_list, mask_weights_list = [], [], [], []
+        return costs
+
+    def _targets_of_matches(self, matches, mask_preds_list, gt_labels_list, gt_masks_list):
+        """(``get_targets``' 6-tuple, the positive query indices of every image) from one layer's matches."""
+        Q = self.num_queries
+        labels_list, label_weights_list, mask_targets_list, mask_weights_list, pos_inds_list = [], [], [], [], []
         num_total_pos = num_total_neg = 0
         for match, mask_pred, gt_labels, gt_masks in zip(matches, mask_preds_list, gt_labels_list, gt_masks_list):
             m = match.long()
@@ -575,9 +628,11 @@ class Box2MaskHead(nn.Module):
             label_weights_list.append(gt_labels.new_ones((Q,)))
             mask_targets_list.append(gt_masks.unsqueeze(1)[pos_gt])
             mask_weights_list.append(pos.to(mask_pred.dtype))
+            pos_inds_list.append(pos_inds)
             num_total_pos += k
             num_total_neg += mask_pred.shape[0] - k
-        return labels_list, label_weights_list, mask_targets_list, mask_weights_list, num_total_pos, num_total_neg
+        return ((labels_list, label_weights_list, mask_targets_list, mask_weights_list, num_total_pos, num_total_neg),
+                pos_inds_list)
 
     # a4 -- box2mask_head.py:343-345
     @staticmethod
@@ -684,17 +739,87 @@ class Box2MaskHead(nn.Module):
         """``mask_loss_single`` of every decoder layer (the reference's ``multi_apply(self.loss_single, ...)`` over the layers,
         box2mask_head.py:214-227): the layers are independent, so each one runs on its own lane stream.  ``mask_preds_per_layer``
         : list of [n,h,w] tensors or of callables producing them (e.g. the layer's einsum + matching, run inside the lane).
-        Returns the list of (loss_project, loss_levelset) pairs."""
+        ``mask_targets`` and ``lst_feat``: one tensor for every layer, or a list with one per layer (each decoder layer has
+        its own matching and its own level-set feature, :203-205).  Returns the list of (loss_project, loss_levelset) pairs."""
+        n_layers = len(mask_preds_per_layer)
+        targets = list(mask_targets) if isinstance(mask_targets, (list, tuple)) else [mask_targets] * n_layers
+        lst_feats = list(lst_feat) if isinstance(lst_feat, (list, tuple)) else [lst_feat] * n_layers
         if trees is None:
             first = mask_preds_per_layer[0]
             shape = (first() if callable(first) else first).shape[-2:]
             trees = self.image_trees(norm_img, shape)
 
-        def layer(mp):
+        def layer(mp, tg, lf):
             mp = mp() if callable(mp) else mp
-            return self.mask_loss_single(mp, mask_targets, num_per_img, norm_img, lst_feat, trees=trees)
+            return self.mask_loss_single(mp, tg, num_per_img, norm_img, lf, trees=trees)
 
-        return run_concurrently([lambda mp=mp: layer(mp) for mp in mask_preds_per_layer], norm_img.device)
+        return run_concurrently([lambda w=w: layer(*w) for w in zip(mask_preds_per_layer, targets, lst_feats)],
+                                norm_img.device)
+
+    def _class_weight(self, device):
+        """The class weights as a [K] float32 tensor on ``device`` (copied once per device, so that later calls read nothing
+        from the host and can be captured in a CUDA graph), or None."""
+        if self.cls_class_weight is None:
+            return None
+        cw = self._class_weight_on.get(device)
+        if cw is None:
+            cw = self._class_weight_on[device] = torch.tensor(self.cls_class_weight, dtype=torch.float32, device=device)
+        return cw
+
+    # box2mask_head.py:192-221, the reference's signature
+    def loss(self, all_cls_scores, all_mask_preds, all_lst_feats, gt_labels_list, gt_masks_list, img_metas, norm_img):
+        """The reference's dict: ``loss_cls``, ``loss_project``, ``loss_levelset`` of the last decoder layer, then
+        ``d{i}.loss_*`` of the others.  all_cls_scores[l] [B,Q,C+1], all_mask_preds[l] [B,Q,h,w] (promoted to float32, the
+        reference's ``@force_fp32``), all_lst_feats[l] [B,1,h',w'] (each layer its own), gt_labels_list[b] [G_b],
+        gt_masks_list[b] [G_b,H,W], norm_img [B,3,H,W].
+        Every layer is matched in ONE launch (``get_targets_layers``), ``loss_cls`` of every layer is ONE kernel
+        (``softmax_cross_entropy_layers``), the matched rows are gathered with the min(Q, G_b) positive indices per image (known
+        from the shapes), the image trees are built once, and the mask losses of the layers run on lane streams.  Nothing is
+        read back to the host: after one eager call the loss can be captured in a CUDA graph.
+        An image whose costs hold a NaN cannot raise without a host read (the reference raises from scipy): its layer's
+        ``loss_cls`` is NaN and ``self.lsap_status[l, b]`` is non-zero.  A batch without ground truth gives zero
+        ``loss_project`` / ``loss_levelset`` attached to the graph (the reference's sum over no rows)."""
+        losses_cls, losses_project, losses_levelset = self._loss_layers(all_cls_scores, all_mask_preds, all_lst_feats,
+                                                                        gt_labels_list, gt_masks_list, norm_img)
+        loss_dict = dict(loss_cls=losses_cls[-1], loss_project=losses_project[-1], loss_levelset=losses_levelset[-1])
+        for i, (c, p, s) in enumerate(zip(losses_cls[:-1], losses_project[:-1], losses_levelset[:-1])):
+            loss_dict[f'd{i}.loss_cls'] = c
+            loss_dict[f'd{i}.loss_project'] = p
+            loss_dict[f'd{i}.loss_levelset'] = s
+        return loss_dict
+
+    # box2mask_head.py:224-335, the reference's signature
+    def loss_single(self, cls_scores, mask_preds, lst_feat, gt_labels_list, gt_masks_list, img_metas, norm_img):
+        """(loss_cls, loss_project, loss_levelset) of one decoder layer, as the reference returns them (``loss`` of one
+        layer)."""
+        c, p, s = self._loss_layers([cls_scores], [mask_preds], [lst_feat], gt_labels_list, gt_masks_list, norm_img)
+        return c[0], p[0], s[0]
+
+    def _loss_layers(self, all_cls_scores, all_mask_preds, all_lst_feats, gt_labels_list, gt_masks_list, norm_img):
+        """Lists of loss_cls, loss_project, loss_levelset, one entry per decoder layer."""
+        from ...ops.cross_entropy import softmax_cross_entropy_layers
+        cls_scores = [c.float() for c in all_cls_scores]
+        mask_preds = [m.float() for m in all_mask_preds]
+        lst_feats = [f.float() for f in all_lst_feats]
+        n_layers, B = len(cls_scores), len(gt_labels_list)
+        dev = cls_scores[0].device
+        with torch.no_grad():
+            targets, pos_inds = self._targets_layers(cls_scores, mask_preds, gt_labels_list, gt_masks_list)
+        labels = torch.stack([torch.stack(t[0]) for t in targets])                              # [L,B,Q]
+        losses_cls = softmax_cross_entropy_layers(cls_scores, labels, self._class_weight(dev), self.cls_loss_weight)
+        failed = (self.lsap_status != 0).any(1)                 # a layer with an unmatched (NaN) image: loss_cls is NaN
+        losses_cls = torch.where(failed, torch.full_like(losses_cls, float('nan')), losses_cls)
+        losses_cls = list(losses_cls.unbind(0))
+        num_per_img = [min(mask_preds[0].shape[1], int(g.shape[0])) for g in gt_labels_list]       # from the shapes
+        if sum(num_per_img) == 0:                               # zero match (:262-267): sums over no rows, on the graph
+            zeros = [m[:0].sum() for m in mask_preds]
+            return losses_cls, zeros, [z.clone() for z in zeros]
+        rows = [torch.cat([mp[b].index_select(0, pos_inds[l][b]) for b in range(B)])
+                for l, mp in enumerate(mask_preds)]                                                 # mask_preds[weights > 0]
+        mask_targets = [torch.cat(t[2]).squeeze(1) for t in targets]
+        pairs = self.mask_loss_layers(rows, mask_targets, num_per_img, norm_img.float(), lst_feats,
+                                      trees=self.image_trees(norm_img.float(), mask_preds[0].shape[-2:]))
+        return losses_cls, [p[0] for p in pairs], [p[1] for p in pairs]
 
     def image_trees(self, norm_img, pred_shape):
         """MST of every image at 96x96 (box2mask_head.py:232,269-272): identical for all decoder layers of a step."""

@@ -18,6 +18,16 @@ def _both(device, feature_fn, weight_fn):
     return gf, forked.join()
 
 
+def _sum_by_tree(gw, tree_of, num_trees):
+    """[n, ...] per-instance d/d edge_weight -> [num_trees, ...]: the rows of each tree summed in a fixed order (a torch
+    reduction over the instances, not an atomic scatter), so the gradient is bit-identical from run to run.  Rows of other
+    trees are selected away, not multiplied by 0: an Inf or NaN of one image cannot reach another."""
+    if num_trees == 1:
+        return gw.sum(0, keepdim=True)
+    trees = torch.arange(num_trees, device=gw.device).view((-1, 1) + (1,) * (gw.dim() - 1))
+    return torch.where(tree_of.long().view((1, -1) + (1,) * (gw.dim() - 1)) == trees, gw.unsqueeze(0), 0).sum(1)
+
+
 class _Refine(Function):
     """``tree_of`` (optional, [n] int32 -> tree): n instances share the G trees given.  The instances of one image share the
     image's tree in both heads that use the filter (box_solov2_head.py:300-305,353; box2mask_head.py:271-276), so the
@@ -45,7 +55,7 @@ class _Refine(Function):
         def d_weight():
             gw = _C.refine_backward_weight_grouped(w, idx, par, chd, (lvl, nlv), tree_of, out, aggr, aggr_up, wsum, wsum_up, g)
             if tree_of is not None:
-                gw = torch.zeros_like(w).index_add_(0, tree_of.long(), gw)
+                gw = _sum_by_tree(gw, tree_of, w.shape[0])
             return _C._to_theirs(gw, perm)
 
         if ctx.low_tree:

@@ -597,6 +597,32 @@ int bxs_sigmoid_focal_loss_levels_forward(const float* const* logits_host, const
                                           float* loss, void* workspace, int64_t n_levels, int64_t B, int64_t C, float gamma,
                                           float alpha, float loss_weight, bxs_stream_t stream);
 
+/* ---------------------------------------------------------------------------------------
+ * Box2Mask's classification loss over every decoder layer    replaces, per layer, mmdet's
+ *     CrossEntropyLoss(use_sigmoid=False, reduction='mean', class_weight=w)(cls_scores.flatten(0, 1), labels.flatten(0, 1),
+ *     avg_factor=w[labels].sum()) (box2mask_head.py:248-258, cross_entropy_loss.py, utils.py weight_reduce_loss).
+ * Layer l (L layers): scores_host[l] f32 [B,Q,K] in its own layout (K = num_classes + 1); labels i64 [L,B,Q] on the device;
+ * class_weight f32 [K] on the device (NULL: all ones).  loss f32 [L] on the device:
+ *   loss[l] = loss_weight * sum_i w[y_i] (logsumexp(x_i) - x_{i,y_i}) / (sum_i w[y_i] + FLT_EPSILON),
+ * with a max-subtracted logsumexp in float32.  avg_factor (the denominator's sum) is computed on the device from the labels.
+ * A label outside [0, K) adds nothing to the loss, to avg_factor or to the gradient (torch asserts on such a label; the
+ * head never produces one).  grad_host[l] f32 [B,Q,K] (grad_host NULL: not needed) = d loss[l] / d scores_host[l], written
+ * in the same pass: loss_weight * w[y_i] (softmax(x_i) - onehot(y_i)) / (avg_factor + FLT_EPSILON).
+ * Two launches: one CTA per (layer, 32 query rows) leaves an FP32 partial, a one-CTA-per-layer launch sums them in a fixed
+ * order: bit-identical from run to run, no atomics, no host synchronisation.  workspace:
+ * bxs_softmax_cross_entropy_layers_forward_workspace_bytes(L, B, Q) bytes (0 for invalid sizes).
+ * backward: g_loss f32 [L] on the device (upstream gradients); grad_host[l] is scaled IN PLACE by g_loss[l], and a layer
+ *   whose upstream gradient is exactly 1 returns at once.  Call it at most once per forward.
+ * The *_host arrays are HOST arrays, copied into kernel parameters.  BXS_ERR_INVALID_ARG: a NULL pointer the call needs,
+ * L, B, Q or K <= 0.  BXS_ERR_UNSUPPORTED: L > 16, B*Q or K above INT32_MAX.  All checks run before any device call.
+ * --------------------------------------------------------------------------------------- */
+int64_t bxs_softmax_cross_entropy_layers_forward_workspace_bytes(int64_t L, int64_t B, int64_t Q);
+int bxs_softmax_cross_entropy_layers_forward(const float* const* scores_host, const int64_t* labels, const float* class_weight,
+                                             float* const* grad_host, float* loss, void* workspace, int64_t L, int64_t B,
+                                             int64_t Q, int64_t K, float loss_weight, bxs_stream_t stream);
+int bxs_softmax_cross_entropy_layers_backward(float* const* grad_host, const float* g_loss, int64_t L, int64_t B, int64_t Q,
+                                              int64_t K, bxs_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
