@@ -148,6 +148,15 @@ def stream():
     return c_p(torch.cuda.current_stream().cuda_stream)
 
 
+def dense_aligned(t, align=16):
+    """``t`` as a dense row-major tensor whose base address is a multiple of ``align`` bytes: ``t`` itself when it already
+    is one, else one copy into a fresh allocation.  A dense view that starts inside another buffer (``flat[1:1 + n]``,
+    ``torch.cat(...)[a:b]`` with an odd row size) is ``is_contiguous()`` but only element-aligned; the kernels that read
+    through 8- or 16-byte vectors or a TMA tensor map take their operands through here."""
+    t = t.contiguous()
+    return t if t.data_ptr() % align == 0 else t.clone(memory_format=torch.contiguous_format)
+
+
 def require_cuda(*tensors):
     """Same error behaviour as the reference's CHECK_INPUT (pairwise.cu:7-13)."""
     for t in tensors:

@@ -989,6 +989,9 @@ extern "C" int bxs_mst_forward(const int32_t* edge_index, const float* edge_weig
   if (!edge_index || !edge_weight || !edge_out || !workspace || B <= 0 || B >= 65536 || E <= 0 || V <= 1 ||
       E >= (int64_t(1) << 31) || V >= (int64_t(1) << 31))
     return BXS_ERR_INVALID_ARG;
+  // both edge lists are read and written one int2 per edge
+  if ((reinterpret_cast<uintptr_t>(edge_index) & 7) || (reinterpret_cast<uintptr_t>(edge_out) & 7))
+    return BXS_ERR_UNSUPPORTED;
   cudaStream_t st = as_stream(stream);
   MstWs ws = carve_mst(workspace, B, E, V);
   int rounds = 0;
@@ -1030,6 +1033,9 @@ extern "C" int bxs_bfs_forward_rooted(const int32_t* tree_edges, int32_t* sorted
       B <= 0 || B >= 65536 || V <= 1 || root < 0 || root >= V)
     return BXS_ERR_INVALID_ARG;
   if (max_adj != 4) return BXS_ERR_UNSUPPORTED;             // the reference only ever passes 4 (tree_filter.py:137)
+  // the edges are read one int2 each, the child table is written one int4 per node
+  if ((reinterpret_cast<uintptr_t>(tree_edges) & 7) || (reinterpret_cast<uintptr_t>(sorted_child) & 15))
+    return BXS_ERR_UNSUPPORTED;
   cudaStream_t st = as_stream(stream);
   BfsWs ws = carve_bfs(workspace, B, V);
   int* err = (int*)((char*)workspace + ws.total_bytes);

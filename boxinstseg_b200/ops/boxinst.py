@@ -173,14 +173,13 @@ class _BoxInstMaskLoss(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, mask_logits, edge_bits, rects, inst_gt, gt_img, iter_buf, warmup_iters, dilation, plan=None):
-        logits = mask_logits.contiguous()
+        logits = L.dense_aligned(mask_logits)       # float4 / bulk-copy reads: one schedule whatever view the caller holds
         L.require_cuda(logits, edge_bits, rects, inst_gt, gt_img, iter_buf)
         N, _, H, W = logits.shape
         lib = L.lib()
         dev = logits.device
         out = torch.empty(4, dtype=torch.float32, device=dev)
-        fused = bool(ctx.needs_input_grad[0] and N > 0 and lib.bxs_boxinst_loss_fused_supported(N, H, W, dilation)
-                     and logits.data_ptr() % 16 == 0)
+        fused = bool(ctx.needs_input_grad[0] and N > 0 and lib.bxs_boxinst_loss_fused_supported(N, H, W, dilation))
         ctx.fused, ctx.dilation, ctx.calls = fused, dilation, 0
         ctx.set_materialize_grads(False)          # no zero-fill kernels for unused / non-differentiable outputs
         with torch.cuda.device(dev):

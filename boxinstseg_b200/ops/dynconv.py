@@ -21,10 +21,11 @@ _HALF = {torch.float16: 0, torch.bfloat16: 1}          # bxs_half_t
 _AUTOCAST_ELIGIBLE = (torch.float32, torch.float16, torch.bfloat16)
 
 
-def _half_native(*tensors):
-    """Inside the envelope of the 16-bit kernels: C % 32 == 0, C <= 256, h*w % 8 == 0, 16-byte aligned bases."""
-    B, C, h, w = tensors[0].shape
-    return C % 32 == 0 and C <= 256 and (h * w) % 8 == 0 and all(t.data_ptr() % 16 == 0 for t in tensors)
+def _half_native(f):
+    """Inside the envelope of the 16-bit kernels: C % 32 == 0, C <= 256, h*w % 8 == 0 (the operands are 16-byte aligned
+    by the time they get here: L.dense_aligned)."""
+    B, C, h, w = f.shape
+    return C % 32 == 0 and C <= 256 and (h * w) % 8 == 0
 
 
 def _forward(f, k):
@@ -73,13 +74,14 @@ class _DynConv1x1(torch.autograd.Function):
     @staticmethod
     def forward(ctx, feat, kernels):
         half = feat.dtype == kernels.dtype and feat.dtype in _HALF
-        f = feat.contiguous() if half else feat.contiguous().float()
-        k = kernels.contiguous() if half else kernels.contiguous().float()
+        # TMA tensor maps: dense and 16-byte aligned, whatever view the caller holds
+        f = L.dense_aligned(feat if half else feat.float())
+        k = L.dense_aligned(kernels if half else kernels.float())
         L.require_cuda(f, k)
         B, C, h, w = f.shape
         assert k.dim() == 3 and k.shape[0] == B and k.shape[2] == C, 'kernels must be [B,I,C]'
         ctx.save_for_backward(f, k)
-        if half and not _half_native(f, k):             # outside the 16-bit envelope: the FP32 kernels on promoted copies
+        if half and not _half_native(f):                # outside the 16-bit envelope: the FP32 kernels on promoted copies
             return _forward(f.float(), k.float()).to(f.dtype)
         return _forward(f, k)
 
@@ -91,8 +93,8 @@ class _DynConv1x1(torch.autograd.Function):
         need_f, need_k = ctx.needs_input_grad[0], ctx.needs_input_grad[1]
         if not (B and I) or not (need_f or need_k):
             return (torch.zeros_like(f) if need_f else None), (torch.zeros_like(k) if need_k else None)
-        g = g_out.contiguous().to(f.dtype)
-        if f.dtype != torch.float32 and not _half_native(f, k, g):
+        g = L.dense_aligned(g_out.to(f.dtype))
+        if f.dtype != torch.float32 and not _half_native(f):
             gf, gk = _backward(f.float(), k.float(), g.float(), need_f, need_k)
             return (None if gf is None else gf.to(f.dtype)), (None if gk is None else gk.to(f.dtype))
         return _backward(f, k, g, need_f, need_k)
@@ -166,7 +168,7 @@ class _SoloCells(torch.autograd.Function):
         B, C = ops[0].shape[:2]
         need_op = any(ctx.needs_input_grad[2:2 + n_ops])
         need_k = any(ctx.needs_input_grad[2 + n_ops:])
-        g = [torch.zeros((sum(n),) + ops[o].shape[2:], device=ops[0].device) if t is None else t.contiguous().float()
+        g = [torch.zeros((sum(n),) + ops[o].shape[2:], device=ops[0].device) if t is None else L.dense_aligned(t.float())
              for t, o, n in zip(g_outs, level_op, counts)]
         g_ops = [torch.empty_like(o) for o in ops] if need_op else None
         g_k = [torch.empty_like(k) for k in kerns] if need_k else None
@@ -178,13 +180,24 @@ class _SoloCells(torch.autograd.Function):
             call = lambda gop, gk: lib.bxs_dynconv1x1_cells_backward(      # noqa: E731
                 _ptrs(ops), sizes, kp, grid, lop, flat, L.ptr(cells), _ptrs(g), gop, gk, L.ptr(ws), len(kerns), n_ops, B, C,
                 L.stream())
-            rc = call(_ptrs(g_ops) if need_op else None, _ptrs(g_k) if need_k else None)
-            if rc == -3 and need_op:
+            if need_op and _cells_widest_problem(level_op, counts) > 256:
                 # more than 256 kernels in a problem: d/d operand through cuBLAS, as dynconv1x1 does beyond 256 kernels
                 g_ops = _cells_operand_grad_mm(ops, kerns, cells, g, level_op, counts)
                 rc = call(None, _ptrs(g_k)) if need_k else 0
+            else:
+                rc = call(_ptrs(g_ops) if need_op else None, _ptrs(g_k) if need_k else None)
             L.check(rc, 'dynconv1x1_cells_backward')
         return (None, None, *(g_ops if need_op else [None] * n_ops), *(g_k if need_k else [None] * len(kerns)))
+
+
+def _cells_widest_problem(level_op, counts):
+    """Kernels of the widest (operand, image) problem, each level's count padded to 32: what the d/d operand kernel reduces
+    over (cells_kp in csrc/dynconv_wgmma.cu), and what limits it to 256."""
+    widest = 0
+    for o in set(level_op):
+        per_image = zip(*[n for n, lo in zip(counts, level_op) if lo == o])
+        widest = max([widest] + [sum((c + 31) & ~31 for c in image) for image in per_image])
+    return widest
 
 
 def _cells_operand_grad_mm(ops, kerns, cells, g, level_op, counts):
@@ -212,7 +225,7 @@ def solo_cells_conv(feature_pred, kernel_preds, cells, out_sizes):
     ``bilinear_resize`` of it, shared by the consecutive levels of that size.  All levels and images run in one launch
     (TF32 operands, FP32 accumulation); other dtypes are promoted to float32.  Differentiable with respect to
     feature_pred and kernel_preds; gradients are deterministic.  C % 32 == 0, C <= 256, h_l*w_l % 4 == 0."""
-    f = feature_pred.contiguous().float()
+    f = L.dense_aligned(feature_pred.float())
     L.require_cuda(f)
     sizes = [(int(s[0]), int(s[1])) for s in out_sizes]
     level_op, op_sizes = [], []

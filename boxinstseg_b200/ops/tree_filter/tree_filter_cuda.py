@@ -16,8 +16,13 @@ def _f32(t):
     return t if t.dtype == torch.float32 and t.is_contiguous() else t.float().contiguous()
 
 
+def _edges(t):
+    """An edge list [B,E,2] as the kernels read it: int32, dense, and 8-byte aligned (one ``int2`` load per edge)."""
+    return L.dense_aligned(_i32(t), 8)
+
+
 def mst_forward(edge_index, edge_weight, vertex_count):
-    ei, ew = _i32(edge_index), _f32(edge_weight)
+    ei, ew = _edges(edge_index), _f32(edge_weight)
     L.require_cuda(ei, ew)
     B, E = ei.shape[0], ei.shape[1]
     V = int(vertex_count)
@@ -30,7 +35,7 @@ def mst_forward(edge_index, edge_weight, vertex_count):
 
 
 def bfs_forward(edge_index, max_adj_per_node, root=0):
-    te = _i32(edge_index)
+    te = _edges(edge_index)
     L.require_cuda(te)
     B, V = te.shape[0], te.shape[1] + 1
     dev = te.device
@@ -156,15 +161,17 @@ def refine_forward_grouped(feature_in, edge_weight, sorted_index, sorted_parent,
 
 def refine_backward_feature_grouped(edge_weight, sorted_index, sorted_parent, sorted_child, levels, tree_of, weight_sum,
                                     grad_out):
-    w, g = _f32(edge_weight), _f32(grad_out)
+    w, g, wsum = _f32(edge_weight), _f32(grad_out), _f32(weight_sum)
+    idx, par, chd = _i32(sorted_index), _i32(sorted_parent), _i32(sorted_child)
+    L.require_cuda(w, g, wsum, idx, par, chd, tree_of)
     lvl, nlv = levels
     n, C, V = g.shape
     G = w.shape[0]
     gf = torch.empty_like(g)
     with torch.cuda.device(g.device):
-        L.check(L.lib().bxs_refine_backward_feature_grouped(L.ptr(w), L.ptr(sorted_index), L.ptr(sorted_parent),
-                                                            L.ptr(sorted_child), L.ptr(lvl), L.ptr(nlv), L.ptr(tree_of),
-                                                            L.ptr(weight_sum), L.ptr(g), L.ptr(gf),
+        L.check(L.lib().bxs_refine_backward_feature_grouped(L.ptr(w), L.ptr(idx), L.ptr(par),
+                                                            L.ptr(chd), L.ptr(lvl), L.ptr(nlv), L.ptr(tree_of),
+                                                            L.ptr(wsum), L.ptr(g), L.ptr(gf),
                                                             L.ptr(_scratch(max(n, G), C, V, g.device)), n, G, C, V, L.stream()),
                 'refine_backward_feature_grouped')
     return gf
@@ -173,15 +180,19 @@ def refine_backward_feature_grouped(edge_weight, sorted_index, sorted_parent, so
 def refine_backward_weight_grouped(edge_weight, sorted_index, sorted_parent, sorted_child, levels, tree_of, feature_out,
                                    feature_aggr, feature_aggr_up, weight_sum, weight_sum_up, grad_out):
     w, g = _f32(edge_weight), _f32(grad_out)
+    idx, par, chd = _i32(sorted_index), _i32(sorted_parent), _i32(sorted_child)
+    out, aggr, aggr_up = _f32(feature_out), _f32(feature_aggr), _f32(feature_aggr_up)
+    wsum, wsum_up = _f32(weight_sum), _f32(weight_sum_up)
+    L.require_cuda(w, g, idx, par, chd, out, aggr, aggr_up, wsum, wsum_up, tree_of)
     lvl, nlv = levels
     n, C, V = g.shape
     G = w.shape[0]
     gw = torch.empty((n, V), dtype=torch.float32, device=g.device)
     with torch.cuda.device(g.device):
-        L.check(L.lib().bxs_refine_backward_weight_grouped(L.ptr(w), L.ptr(sorted_index), L.ptr(sorted_parent),
-                                                           L.ptr(sorted_child), L.ptr(lvl), L.ptr(nlv), L.ptr(tree_of),
-                                                           L.ptr(feature_out), L.ptr(feature_aggr), L.ptr(feature_aggr_up),
-                                                           L.ptr(weight_sum), L.ptr(weight_sum_up), L.ptr(g), L.ptr(gw),
+        L.check(L.lib().bxs_refine_backward_weight_grouped(L.ptr(w), L.ptr(idx), L.ptr(par),
+                                                           L.ptr(chd), L.ptr(lvl), L.ptr(nlv), L.ptr(tree_of),
+                                                           L.ptr(out), L.ptr(aggr), L.ptr(aggr_up),
+                                                           L.ptr(wsum), L.ptr(wsum_up), L.ptr(g), L.ptr(gw),
                                                            L.ptr(_scratch(max(n, G), C, V, g.device)), n, G, C, V, L.stream()),
                 'refine_backward_weight_grouped')
     return gw
