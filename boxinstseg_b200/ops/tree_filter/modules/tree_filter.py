@@ -157,7 +157,7 @@ class TreeFilter2D(nn.Module):
             shape = feature_in.shape
             sorted_index, sorted_parent, sorted_child = order if order is not None else bfs(tree, 4, self._root(shape))
             edge_weight = self.build_edge_weight(embed_in, sorted_index, sorted_parent, low_tree, sorted_child)
-            feat = feature_in.reshape(shape[0], shape[1], -1).contiguous()
+            feat = feature_in.reshape(shape[0], shape[1], shape[2] * shape[3]).contiguous()     # n may be 0
             t_of = tree_of if tree_of.dtype == torch.int32 else tree_of.to(torch.int32)
             return refine(feat, edge_weight, sorted_index, sorted_parent, sorted_child, low_tree,
                           t_of.contiguous()).reshape(shape)

@@ -74,16 +74,26 @@ def levels_of(sorted_index, sorted_parent):
 def _adopt(sorted_index, sorted_parent):
     """Any parent-before-child order (e.g. the reference's own racy bfs_forward output, bfs.cu:46-98) -> the
     deterministic level order of the SAME tree that the refine kernels need (levels contiguous, children of a node
-    adjacent): (idx, par, chd, (level_start, num_levels), perm) with perm[b, foreign position] = position here."""
+    adjacent): (idx, par, chd, (level_start, num_levels), perm) with perm[b, foreign position] = position here.
+    The adopted order keeps each tree's root (the foreign order's first vertex): a position's edge weight belongs to the
+    edge to ITS parent, and re-rooting would hand the weights of the edges between the two roots to the wrong edges."""
     idx, par = _i32(sorted_index), _i32(sorted_parent)
     B, V = idx.shape
     up = torch.gather(idx, 1, par[:, 1:].long())                       # vertex id of each non-root node's parent
     edges = torch.stack((idx[:, 1:], up), dim=2).contiguous()          # the tree as an edge list [B,V-1,2]
-    oidx, opar, ochd = bfs_forward(edges, 4)
+    roots = idx[:, 0].tolist()
+    if all(r == roots[0] for r in roots):
+        oidx, opar, ochd = bfs_forward(edges, 4, roots[0])
+        levels = _cached_levels(oidx)
+    else:                                                              # one BFS per tree
+        parts = [bfs_forward(edges[b:b + 1], 4, r) for b, r in enumerate(roots)]
+        oidx, opar, ochd = (torch.cat([p[k] for p in parts]) for k in range(3))
+        levels = tuple(torch.cat([_cached_levels(p[0])[k] for p in parts]) for k in range(2))
+        setattr(oidx, _LEVELS, (levels[0], levels[1], oidx._version))
     pos_of_vertex = torch.empty((B, V), dtype=torch.int64, device=idx.device)
     pos_of_vertex.scatter_(1, oidx.long(), torch.arange(V, device=idx.device).expand(B, V))
     perm = torch.gather(pos_of_vertex, 1, idx.long())
-    return oidx, opar, ochd, _cached_levels(oidx), perm
+    return oidx, opar, ochd, levels, perm
 
 
 def _resolve(edge_weight, sorted_index, sorted_parent, sorted_child):
@@ -151,6 +161,8 @@ def refine_forward_grouped(feature_in, edge_weight, sorted_index, sorted_parent,
     out, aggr, aggr_up = torch.empty_like(f), torch.empty_like(f), torch.empty_like(f)
     wsum = torch.empty((G, V), dtype=torch.float32, device=f.device)
     wsum_up = torch.empty_like(wsum)
+    if n == 0:                  # no instance: nothing to filter, and no backward reads the normaliser
+        return out, aggr, aggr_up, wsum.zero_(), wsum_up.zero_()
     with torch.cuda.device(f.device):
         L.check(L.lib().bxs_refine_forward_grouped(L.ptr(f), L.ptr(w), L.ptr(idx), L.ptr(par), L.ptr(chd), L.ptr(lvl), L.ptr(nlv),
                                                    L.ptr(tree_of), L.ptr(out), L.ptr(aggr), L.ptr(aggr_up), L.ptr(wsum),
@@ -168,6 +180,8 @@ def refine_backward_feature_grouped(edge_weight, sorted_index, sorted_parent, so
     n, C, V = g.shape
     G = w.shape[0]
     gf = torch.empty_like(g)
+    if n == 0:
+        return gf
     with torch.cuda.device(g.device):
         L.check(L.lib().bxs_refine_backward_feature_grouped(L.ptr(w), L.ptr(idx), L.ptr(par),
                                                             L.ptr(chd), L.ptr(lvl), L.ptr(nlv), L.ptr(tree_of),
@@ -188,6 +202,8 @@ def refine_backward_weight_grouped(edge_weight, sorted_index, sorted_parent, sor
     n, C, V = g.shape
     G = w.shape[0]
     gw = torch.empty((n, V), dtype=torch.float32, device=g.device)
+    if n == 0:                  # the callers sum the rows of a tree: a tree without instances gets a zero d/d w
+        return gw
     with torch.cuda.device(g.device):
         L.check(L.lib().bxs_refine_backward_weight_grouped(L.ptr(w), L.ptr(idx), L.ptr(par),
                                                            L.ptr(chd), L.ptr(lvl), L.ptr(nlv), L.ptr(tree_of),
