@@ -61,9 +61,6 @@ def run_concurrently(fns, device, max_lanes=10):
 def _tensors(obj):
     if isinstance(obj, torch.Tensor):
         yield obj
-        for extra in getattr(obj, '_bxs_levels', ()) or ():
-            if isinstance(extra, torch.Tensor):
-                yield extra
     elif isinstance(obj, (tuple, list)):
         for o in obj:
             yield from _tensors(o)

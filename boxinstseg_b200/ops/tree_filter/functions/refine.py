@@ -32,37 +32,46 @@ class _Refine(Function):
     """``tree_of`` (optional, [n] int32 -> tree): n instances share the G trees given.  The instances of one image share the
     image's tree in both heads that use the filter (box_solov2_head.py:300-305,353; box2mask_head.py:271-276), so the
     BFS order, the edge weights and the normaliser are computed once per image, and d/d edge_weight is summed over the
-    instances of a tree.  Without it instance i uses tree i, as in the reference.  An order that bfs_forward did not
-    produce is replaced by the equivalent canonical order of the same tree (tree_filter_cuda._resolve)."""
+    instances of a tree.  Without it instance i uses tree i, as in the reference.  The five tensors after ``edge_weight``
+    are a tree_filter_cuda.TreeOrder."""
 
     @staticmethod
-    def forward(ctx, feature_in, edge_weight, sorted_index, sorted_parent, sorted_child, low_tree, tree_of=None):
-        w, idx, par, chd, levels, perm = _C._resolve(edge_weight, sorted_index, sorted_parent, sorted_child)
-        out, aggr, aggr_up, wsum, wsum_up = _C.refine_forward_grouped(feature_in, w, idx, par, chd, levels, tree_of)
-        ctx.save_for_backward(w, idx, par, chd, *levels, tree_of, perm, out, aggr, aggr_up, wsum, wsum_up)
+    def forward(ctx, feature_in, edge_weight, sorted_index, sorted_parent, sorted_child, level_start, num_levels, low_tree,
+                tree_of):
+        w = _C._f32(edge_weight)
+        order = _C.TreeOrder(sorted_index, sorted_parent, sorted_child, level_start, num_levels)
+        out, aggr, aggr_up, wsum, wsum_up = _C.refine_forward_grouped(feature_in, w, order, tree_of)
+        ctx.save_for_backward(w, *order, tree_of, out, aggr, aggr_up, wsum, wsum_up)
         ctx.low_tree = low_tree
         return out
 
     @staticmethod
     @once_differentiable
     def backward(ctx, grad_output):
-        (w, idx, par, chd, lvl, nlv, tree_of, perm, out, aggr, aggr_up, wsum, wsum_up) = ctx.saved_tensors
+        w, idx, par, chd, lvl, nlv, tree_of, out, aggr, aggr_up, wsum, wsum_up = ctx.saved_tensors
+        order = _C.TreeOrder(idx, par, chd, lvl, nlv)
         g = grad_output.contiguous()
 
         def d_feature():
-            return _C.refine_backward_feature_grouped(w, idx, par, chd, (lvl, nlv), tree_of, wsum, g)
+            return _C.refine_backward_feature_grouped(w, order, tree_of, wsum, g)
 
         def d_weight():
-            gw = _C.refine_backward_weight_grouped(w, idx, par, chd, (lvl, nlv), tree_of, out, aggr, aggr_up, wsum, wsum_up, g)
-            if tree_of is not None:
-                gw = _sum_by_tree(gw, tree_of, w.shape[0])
-            return _C._to_theirs(gw, perm)
+            gw = _C.refine_backward_weight_grouped(w, order, tree_of, out, aggr, aggr_up, wsum, wsum_up, g)
+            return gw if tree_of is None else _sum_by_tree(gw, tree_of, w.shape[0])
 
         if ctx.low_tree:
-            return d_feature(), None, None, None, None, None, None
-        grad_feature, grad_weight = _both(g.device, d_feature, d_weight)
-        return grad_feature, grad_weight, None, None, None, None, None
+            return (d_feature(),) + (None,) * 8
+        return _both(g.device, d_feature, d_weight) + (None,) * 7
+
+
+def refine_ordered(feature_in, edge_weight, order, low_tree, tree_of=None):
+    """``refine`` for a caller that holds the tree_filter_cuda.TreeOrder (``bfs_order``, ``TreeFilter2D.order``)."""
+    return _Refine.apply(feature_in, edge_weight, *order, low_tree, tree_of)
 
 
 def refine(feature_in, edge_weight, sorted_index, sorted_parent, sorted_child, low_tree, tree_of=None):
-    return _Refine.apply(feature_in, edge_weight, sorted_index, sorted_parent, sorted_child, low_tree, tree_of)
+    """The reference's signature.  An order that ``bfs`` did not produce is replaced by the equivalent canonical order of
+    the same tree, with the edge weights (and, through autograd, their gradient) carried over by vertex
+    (tree_filter_cuda._resolve)."""
+    w, order, _ = _C._resolve(edge_weight, sorted_index, sorted_parent, sorted_child)
+    return refine_ordered(feature_in, w, order, low_tree, tree_of)

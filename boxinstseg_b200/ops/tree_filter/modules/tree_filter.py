@@ -10,9 +10,9 @@ from torch import nn
 
 from .... import _lib as L
 
-from ..functions.bfs import bfs
+from .. import tree_filter_cuda as _C
 from ..functions.mst import mst
-from ..functions.refine import refine
+from ..functions.refine import refine_ordered
 
 
 def _squared_distance(a, b):
@@ -143,33 +143,27 @@ class TreeFilter2D(nn.Module):
         return torch.exp(-dist / self.sigma) if low_tree else torch.exp(-dist)
 
     def order(self, tree, shape):
-        """The BFS order ``forward`` would compute for ``tree`` (rooted at the centre pixel of ``shape``): lets a caller build
-        it ahead of time, e.g. on a side stream while another filter runs, and pass it back as ``order=``."""
-        return bfs(tree, 4, self._root(shape))
+        """The order ``forward`` would compute for ``tree`` (a TreeOrder rooted at the centre pixel of ``shape``): lets a
+        caller build it ahead of time, e.g. on a side stream while another filter runs, and pass it back as ``order=``."""
+        return _C.bfs_order(tree, 4, self._root(shape))
 
     def forward(self, feature_in, embed_in, tree, low_tree=True, tree_of=None, order=None):
         """``tree_of`` (optional, int32 [n]): feature_in holds n instances that share the G trees / embeddings given
         (embed_in [G,C,h,w], tree [G,V-1,2]); instance i uses tree ``tree_of[i]``.  Same result as repeating the trees
         and embeddings per instance (what the reference's heads do), computed once per tree.
-        ``order`` (optional): ``self.order(tree, feature_in.shape)`` computed by the caller."""
-        if tree_of is not None:
-            assert self.groups == 1
-            shape = feature_in.shape
-            sorted_index, sorted_parent, sorted_child = order if order is not None else bfs(tree, 4, self._root(shape))
-            edge_weight = self.build_edge_weight(embed_in, sorted_index, sorted_parent, low_tree, sorted_child)
-            feat = feature_in.reshape(shape[0], shape[1], shape[2] * shape[3]).contiguous()     # n may be 0
-            t_of = tree_of if tree_of.dtype == torch.int32 else tree_of.to(torch.int32)
-            return refine(feat, edge_weight, sorted_index, sorted_parent, sorted_child, low_tree,
-                          t_of.contiguous()).reshape(shape)
+        ``order`` (optional): ``self.order(tree, feature_in.shape)`` computed by the caller, or the three tensors of
+        ``bfs(tree, 4, root)`` for any root."""
+        assert tree_of is None or self.groups == 1
         shape = feature_in.shape
-        sorted_index, sorted_parent, sorted_child = order if order is not None else bfs(tree, 4, self._root(shape))
-        edge_weight = self.build_edge_weight(embed_in, sorted_index, sorted_parent, low_tree, sorted_child)
-        feat = feature_in.reshape(shape[0] * self.groups, shape[1] // self.groups, -1).contiguous()
+        if order is None:
+            order = self.order(tree, shape)
+        elif not isinstance(order, _C.TreeOrder):
+            order = _C._own(*order)[0]
+        edge_weight = self.build_edge_weight(embed_in, order.sorted_index, order.sorted_parent, low_tree, order.sorted_child)
+        # n may be 0, so the last extent is spelled out
+        feat = feature_in.reshape(shape[0] * self.groups, shape[1] // self.groups, shape[2] * shape[3]).contiguous()
         if self.groups > 1:                                  # tree_filter.py:110-120 (split_group)
-            from .. import tree_filter_cuda as _C
-            levels = _C.levels_of(sorted_index, sorted_parent)
-            rep = lambda t: t.repeat_interleave(self.groups, dim=0).contiguous()   # noqa: E731
-            sorted_index, sorted_parent, sorted_child = rep(sorted_index), rep(sorted_parent), rep(sorted_child)
-            setattr(sorted_index, '_bxs_levels', (rep(levels[0]), rep(levels[1])))
-        out = refine(feat, edge_weight, sorted_index, sorted_parent, sorted_child, low_tree)
-        return out.reshape(shape)
+            order = _C.TreeOrder(*(t.repeat_interleave(self.groups, dim=0).contiguous() for t in order))
+        if tree_of is not None:
+            tree_of = tree_of.to(torch.int32).contiguous()
+        return refine_ordered(feat, edge_weight, order, low_tree, tree_of).reshape(shape)

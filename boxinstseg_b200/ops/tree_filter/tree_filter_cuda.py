@@ -1,11 +1,22 @@
 """Stand-in for the reference's pybind module ``tree_filter_cuda``
 (mmdet/ops/tree_filter/src/tree_filter.cpp:7-13): the same five functions with the same argument
 order and return values, implemented on the C ABI of libboxseg_b200."""
+from typing import NamedTuple
+
 import torch
 
 from ... import _lib as L
 
-_LEVELS = '_bxs_levels'        # (level_start, num_levels) riding on the sorted_index tensor object
+_LEVELS = '_bxs_levels'        # the attribute _remember / _recall keep on a sorted_index tensor object
+
+
+class TreeOrder(NamedTuple):
+    """A batch of trees in BFS order, with the level table the level-by-level refine kernels walk (all int32)."""
+    sorted_index: torch.Tensor      # [B,V]    vertex at each position
+    sorted_parent: torch.Tensor     # [B,V]    position of each position's parent
+    sorted_child: torch.Tensor      # [B,V,4]  positions of each position's children, 0-padded
+    level_start: torch.Tensor       # [B,V+1]  first position of each level
+    num_levels: torch.Tensor        # [B]
 
 
 def _i32(t):
@@ -34,7 +45,8 @@ def mst_forward(edge_index, edge_weight, vertex_count):
     return out
 
 
-def bfs_forward(edge_index, max_adj_per_node, root=0):
+def bfs_order(edge_index, max_adj_per_node, root=0):
+    """The deterministic level order of each tree, rooted at vertex ``root``, as a TreeOrder."""
     te = _edges(edge_index)
     L.require_cuda(te)
     B, V = te.shape[0], te.shape[1] + 1
@@ -49,32 +61,44 @@ def bfs_forward(edge_index, max_adj_per_node, root=0):
     with torch.cuda.device(dev):
         L.check(lib.bxs_bfs_forward_rooted(L.ptr(te), L.ptr(idx), L.ptr(par), L.ptr(chd), L.ptr(lvl), L.ptr(nlv), L.ptr(ws), B, V,
                                            int(max_adj_per_node), int(root), L.stream()), 'bfs_forward')
-    setattr(idx, _LEVELS, (lvl, nlv, idx._version))
-    return idx, par, chd
+    return TreeOrder(idx, par, chd, lvl, nlv)
 
 
-def _cached_levels(sorted_index):
-    """(level_start, num_levels) produced by bfs_forward for exactly this tensor in its current state, else None.
-    The cache rides on the tensor object; it is trusted only while the tensor has not been written since
-    (same `_version`), so a buffer that was modified in place or reused as an output is treated as foreign."""
-    cached = getattr(sorted_index, _LEVELS, None)
-    if cached is None or cached[2] != sorted_index._version:
+# The reference's five functions pass an order as three bare tensors, with no place for its level table.  So that code
+# written against them stays free of host synchronisation, bfs_forward remembers the table on the sorted_index it
+# returns and the refine_* functions recall it; everything else in the package carries a TreeOrder instead.
+def _remember(sorted_index, level_start, num_levels):
+    setattr(sorted_index, _LEVELS, (level_start, num_levels, sorted_index._version))
+
+
+def _recall(sorted_index):
+    """(level_start, num_levels) remembered for exactly this tensor object in its current state, else None: a tensor
+    written since (another `_version`), e.g. a buffer modified in place or reused as an output, counts as foreign."""
+    memo = getattr(sorted_index, _LEVELS, None)
+    if memo is None or memo[2] != sorted_index._version:
         return None
-    return cached[0], cached[1]
+    return memo[0], memo[1]
+
+
+def bfs_forward(edge_index, max_adj_per_node, root=0):
+    order = bfs_order(edge_index, max_adj_per_node, root)
+    _remember(order.sorted_index, order.level_start, order.num_levels)
+    return order.sorted_index, order.sorted_parent, order.sorted_child
 
 
 def levels_of(sorted_index, sorted_parent):
-    """level boundaries of an order produced by bfs_forward (cached), else of the equivalent canonical order."""
-    cached = _cached_levels(sorted_index)
-    if cached is not None:
-        return cached
-    return _adopt(sorted_index, sorted_parent)[3]
+    """level boundaries of an order produced by bfs_forward (remembered), else of the equivalent canonical order."""
+    levels = _recall(sorted_index)
+    if levels is not None:
+        return levels
+    order = _adopt(sorted_index, sorted_parent)[0]
+    return order.level_start, order.num_levels
 
 
 def _adopt(sorted_index, sorted_parent):
     """Any parent-before-child order (e.g. the reference's own racy bfs_forward output, bfs.cu:46-98) -> the
     deterministic level order of the SAME tree that the refine kernels need (levels contiguous, children of a node
-    adjacent): (idx, par, chd, (level_start, num_levels), perm) with perm[b, foreign position] = position here.
+    adjacent): (order, perm) with perm[b, foreign position] = position here.
     The adopted order keeps each tree's root (the foreign order's first vertex): a position's edge weight belongs to the
     edge to ITS parent, and re-rooting would hand the weights of the edges between the two roots to the wrong edges."""
     idx, par = _i32(sorted_index), _i32(sorted_parent)
@@ -83,28 +107,30 @@ def _adopt(sorted_index, sorted_parent):
     edges = torch.stack((idx[:, 1:], up), dim=2).contiguous()          # the tree as an edge list [B,V-1,2]
     roots = idx[:, 0].tolist()
     if all(r == roots[0] for r in roots):
-        oidx, opar, ochd = bfs_forward(edges, 4, roots[0])
-        levels = _cached_levels(oidx)
+        order = bfs_order(edges, 4, roots[0])
     else:                                                              # one BFS per tree
-        parts = [bfs_forward(edges[b:b + 1], 4, r) for b, r in enumerate(roots)]
-        oidx, opar, ochd = (torch.cat([p[k] for p in parts]) for k in range(3))
-        levels = tuple(torch.cat([_cached_levels(p[0])[k] for p in parts]) for k in range(2))
-        setattr(oidx, _LEVELS, (levels[0], levels[1], oidx._version))
+        parts = [bfs_order(edges[b:b + 1], 4, r) for b, r in enumerate(roots)]
+        order = TreeOrder(*(torch.cat(ts) for ts in zip(*parts)))
     pos_of_vertex = torch.empty((B, V), dtype=torch.int64, device=idx.device)
-    pos_of_vertex.scatter_(1, oidx.long(), torch.arange(V, device=idx.device).expand(B, V))
+    pos_of_vertex.scatter_(1, order.sorted_index.long(), torch.arange(V, device=idx.device).expand(B, V))
     perm = torch.gather(pos_of_vertex, 1, idx.long())
-    return oidx, opar, ochd, levels, perm
+    return order, perm
+
+
+def _own(sorted_index, sorted_parent, sorted_child):
+    """-> (order, perm): the caller's tensors with their remembered level table when bfs_forward produced them (perm
+    None), else the adopted order."""
+    levels = _recall(sorted_index)
+    if levels is not None:
+        return TreeOrder(_i32(sorted_index), _i32(sorted_parent), _i32(sorted_child), *levels), None
+    return _adopt(sorted_index, sorted_parent)
 
 
 def _resolve(edge_weight, sorted_index, sorted_parent, sorted_child):
-    """-> (w, idx, par, chd, levels, perm): the caller's order when it came from bfs_forward (perm None), else the
-    adopted order with the per-position edge weights carried over by vertex."""
-    w, idx, par, chd = _f32(edge_weight), _i32(sorted_index), _i32(sorted_parent), _i32(sorted_child)
-    levels = _cached_levels(sorted_index)
-    if levels is not None:
-        return w, idx, par, chd, levels, None
-    oidx, opar, ochd, levels, perm = _adopt(idx, par)
-    return torch.zeros_like(w).scatter_(1, perm, w), oidx, opar, ochd, levels, perm
+    """-> (w, order, perm): ``_own`` with the per-position edge weights carried over by vertex to an adopted order."""
+    order, perm = _own(sorted_index, sorted_parent, sorted_child)
+    w = _f32(edge_weight)
+    return (w if perm is None else torch.zeros_like(w).scatter_(1, perm, w)), order, perm
 
 
 def _to_ours(t, perm):      # position-ordered [B,V] or [B,C,V] tensor: foreign order -> adopted order
@@ -126,22 +152,22 @@ def _scratch(B, C, V, dev):
 
 
 def refine_forward(feature_in, edge_weight, sorted_index, sorted_parent, sorted_child):
-    w, idx, par, chd, levels, perm = _resolve(edge_weight, sorted_index, sorted_parent, sorted_child)
-    out, aggr, aggr_up, wsum, wsum_up = refine_forward_grouped(feature_in, w, idx, par, chd, levels, None)
+    w, order, perm = _resolve(edge_weight, sorted_index, sorted_parent, sorted_child)
+    out, aggr, aggr_up, wsum, wsum_up = refine_forward_grouped(feature_in, w, order, None)
     # out / aggr / wsum are vertex-ordered; the two *_up tensors are position-ordered (refine.cu:201-260)
     return out, aggr, _to_theirs(aggr_up, perm), wsum, _to_theirs(wsum_up, perm)
 
 
 def refine_backward_feature(feature_in, edge_weight, sorted_index, sorted_parent, sorted_child, feature_out,
                             feature_aggr, feature_aggr_up, weight_sum, weight_sum_up, grad_out):
-    w, idx, par, chd, levels, _ = _resolve(edge_weight, sorted_index, sorted_parent, sorted_child)
-    return refine_backward_feature_grouped(w, idx, par, chd, levels, None, _f32(weight_sum), grad_out)
+    w, order, _ = _resolve(edge_weight, sorted_index, sorted_parent, sorted_child)
+    return refine_backward_feature_grouped(w, order, None, _f32(weight_sum), grad_out)
 
 
 def refine_backward_weight(feature_in, edge_weight, sorted_index, sorted_parent, sorted_child, feature_out,
                            feature_aggr, feature_aggr_up, weight_sum, weight_sum_up, grad_out):
-    w, idx, par, chd, levels, perm = _resolve(edge_weight, sorted_index, sorted_parent, sorted_child)
-    gw = refine_backward_weight_grouped(w, idx, par, chd, levels, None, _f32(feature_out), _f32(feature_aggr),
+    w, order, perm = _resolve(edge_weight, sorted_index, sorted_parent, sorted_child)
+    gw = refine_backward_weight_grouped(w, order, None, _f32(feature_out), _f32(feature_aggr),
                                         _to_ours(_f32(feature_aggr_up), perm), _f32(weight_sum),
                                         _to_ours(_f32(weight_sum_up), perm), grad_out)
     return _to_theirs(gw, perm)
@@ -149,13 +175,12 @@ def refine_backward_weight(feature_in, edge_weight, sorted_index, sorted_parent,
 
 # ----------------------------------------------------------------------------------------------------------------
 # grouped forms (not part of the reference's pybind surface): n instances share G trees, tree_of [n] -> tree (None:
-# instance i uses tree i, n == G).  The order must come from bfs_forward (see _resolve); levels = its level table.
+# instance i uses tree i, n == G).  ``order`` is a TreeOrder: from bfs_order, or an adopted one (see _resolve).
 # ----------------------------------------------------------------------------------------------------------------
-def refine_forward_grouped(feature_in, edge_weight, sorted_index, sorted_parent, sorted_child, levels, tree_of):
+def refine_forward_grouped(feature_in, edge_weight, order, tree_of):
     f, w = _f32(feature_in), _f32(edge_weight)
-    idx, par, chd = _i32(sorted_index), _i32(sorted_parent), _i32(sorted_child)
-    L.require_cuda(f, w, idx, par, chd, tree_of)
-    lvl, nlv = levels
+    idx, par, chd, lvl, nlv = (_i32(t) for t in order)
+    L.require_cuda(f, w, idx, par, chd, lvl, nlv, tree_of)
     n, C, V = f.shape
     G = w.shape[0]
     out, aggr, aggr_up = torch.empty_like(f), torch.empty_like(f), torch.empty_like(f)
@@ -171,12 +196,10 @@ def refine_forward_grouped(feature_in, edge_weight, sorted_index, sorted_parent,
     return out, aggr, aggr_up, wsum, wsum_up
 
 
-def refine_backward_feature_grouped(edge_weight, sorted_index, sorted_parent, sorted_child, levels, tree_of, weight_sum,
-                                    grad_out):
+def refine_backward_feature_grouped(edge_weight, order, tree_of, weight_sum, grad_out):
     w, g, wsum = _f32(edge_weight), _f32(grad_out), _f32(weight_sum)
-    idx, par, chd = _i32(sorted_index), _i32(sorted_parent), _i32(sorted_child)
-    L.require_cuda(w, g, wsum, idx, par, chd, tree_of)
-    lvl, nlv = levels
+    idx, par, chd, lvl, nlv = (_i32(t) for t in order)
+    L.require_cuda(w, g, wsum, idx, par, chd, lvl, nlv, tree_of)
     n, C, V = g.shape
     G = w.shape[0]
     gf = torch.empty_like(g)
@@ -191,14 +214,13 @@ def refine_backward_feature_grouped(edge_weight, sorted_index, sorted_parent, so
     return gf
 
 
-def refine_backward_weight_grouped(edge_weight, sorted_index, sorted_parent, sorted_child, levels, tree_of, feature_out,
-                                   feature_aggr, feature_aggr_up, weight_sum, weight_sum_up, grad_out):
+def refine_backward_weight_grouped(edge_weight, order, tree_of, feature_out, feature_aggr, feature_aggr_up, weight_sum,
+                                   weight_sum_up, grad_out):
     w, g = _f32(edge_weight), _f32(grad_out)
-    idx, par, chd = _i32(sorted_index), _i32(sorted_parent), _i32(sorted_child)
+    idx, par, chd, lvl, nlv = (_i32(t) for t in order)
     out, aggr, aggr_up = _f32(feature_out), _f32(feature_aggr), _f32(feature_aggr_up)
     wsum, wsum_up = _f32(weight_sum), _f32(weight_sum_up)
-    L.require_cuda(w, g, idx, par, chd, out, aggr, aggr_up, wsum, wsum_up, tree_of)
-    lvl, nlv = levels
+    L.require_cuda(w, g, idx, par, chd, lvl, nlv, out, aggr, aggr_up, wsum, wsum_up, tree_of)
     n, C, V = g.shape
     G = w.shape[0]
     gw = torch.empty((n, V), dtype=torch.float32, device=g.device)

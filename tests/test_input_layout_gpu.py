@@ -551,8 +551,9 @@ def test_input_layout(name, shape, arg, kind):
     ref = _run(case, a)
     view = relayout(a[arg], kind)
     keep = view.clone()
-    if arg in ('index',):           # the level table rides on the tensor bfs_forward returned; a rebuilt one has none
-        assert not hasattr(view, '_bxs_levels')
+    if arg in ('index',):           # the level table is remembered for the tensor bfs_forward returned; a rebuilt one has none
+        from boxinstseg_b200.ops.tree_filter import tree_filter_cuda as C
+        assert C._recall(view) is None
     got = _run(case, {**a, arg: view})
     _compare(case, arg, ref, got)
     assert torch.equal(view, keep), 'the input is left as it was'

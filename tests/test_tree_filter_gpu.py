@@ -94,9 +94,13 @@ def test_bfs_valid_and_deterministic():
     lvl, nlv = _C.levels_of(idx, par)
     lvl2, nlv2 = _C.levels_of(idx.clone(), par)
     assert torch.equal(nlv, nlv2)
+    order = _C.bfs_order(tree, 4)                          # the same order as one value, level table included
+    assert all(torch.equal(a, b) for a, b in zip(order[:3], (idx, par, chd)))
+    assert torch.equal(order.num_levels, nlv)
     for b in range(3):
         L = int(nlv[b])
         assert torch.equal(lvl[b, :L + 1], lvl2[b, :L + 1])
+        assert torch.equal(order.level_start[b, :L + 1], lvl[b, :L + 1])
 
 
 def test_refine_golden_closed_form(golden):
@@ -149,6 +153,28 @@ def test_tree_filter_vs_oracle(B, C, h, w, low):
     assert rel_err(out.cpu(), out64.detach()) < 1e-4 and rel_err(gf.cpu(), gf64) < 1e-4
     err_ours, err_fp32_ref = rel_err(ge.cpu(), ge64), rel_err(ge_ref, ge64)
     assert err_ours <= max(1e-3, 1.5 * err_fp32_ref), (err_ours, err_fp32_ref)
+
+
+def test_channel_groups_equal_one_filter_per_group():
+    """groups=2 (tree_filter.py:110-120, split_group): each half of the channels is filtered with the edge weights of its
+    half of the embedding on the image's tree -- bit for bit what groups=1 gives for each half on its own."""
+    from boxinstseg_b200.ops.tree_filter import MinimumSpanningTree, TreeFilter2D
+    gen = torch.Generator().manual_seed(5)
+    guide = torch.randn(2, 3, 20, 12, generator=gen).to(DEV)
+    feat = torch.rand(2, 4, 20, 12, generator=gen).to(DEV)
+    embed = (torch.randn(2, 4, 20, 12, generator=gen) * 0.4).to(DEV)
+    gout = torch.randn(2, 4, 20, 12, generator=gen).to(DEV)
+    tree = MinimumSpanningTree(TreeFilter2D.norm2_distance)(guide)
+
+    def run(tf, f, e, g):
+        f, e = f.clone().requires_grad_(True), e.clone().requires_grad_(True)
+        out = tf(f, e, tree, low_tree=False)
+        return (out.detach(),) + torch.autograd.grad((out * g).sum(), [f, e])
+
+    both = run(TreeFilter2D(groups=2), feat, embed, gout)
+    halves = [run(TreeFilter2D(groups=1), feat[:, s], embed[:, s], gout[:, s]) for s in (slice(0, 2), slice(2, 4))]
+    for got, lo, hi in zip(both, *halves):
+        assert torch.equal(got, torch.cat((lo, hi), dim=1))
 
 
 def test_box2mask_call_pattern():

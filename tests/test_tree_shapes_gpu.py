@@ -74,6 +74,12 @@ def test_bfs_equals_canonical_order(name, kind):
     assert np.array_equal(par[0].cpu().numpy(), r_par)
     assert np.array_equal(chd[0].cpu().numpy(), r_chd)
     assert int(nlv[0]) == r_L and np.array_equal(lvl[0, :r_L + 1].cpu().numpy(), r_lvl)
+    order = _C.bfs_order(tree, 4, root)                    # the same order as one value, and a copy of it, which is adopted
+    lvl_c, nlv_c = _C.levels_of(idx.clone(), par)
+    assert all(torch.equal(a, b) for a, b in zip(order[:3], (idx, par, chd)))
+    assert torch.equal(order.num_levels, nlv) and torch.equal(nlv_c, nlv)
+    assert torch.equal(order.level_start[0, :r_L + 1], lvl[0, :r_L + 1])
+    assert torch.equal(lvl_c[0, :r_L + 1], lvl[0, :r_L + 1])
     # the path: the grid fast path is tried iff its shared memory fits, and keeps the tree iff the tree is 4-connected
     # on the pitch it infers and no level is wider than its frontier
     i2, p2, c2, l2, n2, flag = _bfs_with_path(tree, V, root)

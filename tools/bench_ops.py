@@ -90,6 +90,7 @@ gout = torch.randn_like(out)
 both(res, 'condinst_head_bwd', lambda: torch.autograd.grad(out, [feat, params], gout, retain_graph=True))
 
 from boxinstseg_b200.ops.tree_filter import MinimumSpanningTree, TreeFilter2D, bfs  # noqa: E402
+from boxinstseg_b200.ops.tree_filter.tree_filter_cuda import bfs_order  # noqa: E402
 mst, tf = MinimumSpanningTree(TreeFilter2D.norm2_distance), TreeFilter2D()
 for name, (n, h, w) in dict(levelset_D_200x256=(16, 200, 256), box2mask_E_96x96=(8, 96, 96)).items():
     guide = F.interpolate(torch.randn(n, 3, h // 8, w // 8, device=dev, generator=g), size=(h, w), mode='bilinear') + \
@@ -101,8 +102,7 @@ for name, (n, h, w) in dict(levelset_D_200x256=(16, 200, 256), box2mask_E_96x96=
     res[f'treefilter_fwd_{name}_us'] = timeit(lambda: tf(feat1, guide, tree), reps=5, warm=1)
     o = tf(feat1, guide, tree, low_tree=False)
     res[f'treefilter_bwd_{name}_us'] = timeit(lambda: torch.autograd.grad(o.sum(), feat1, retain_graph=True), reps=5, warm=1)
-    idx, par, chd = bfs(tree, 4)
-    res[f'tree_levels_{name}'] = int(getattr(idx, '_bxs_levels')[1].max())
+    res[f'tree_levels_{name}'] = int(bfs_order(tree, 4).num_levels.max())
 
 from boxinstseg_b200.models.losses import LCM, LevelsetLoss, projection_losses  # noqa: E402
 from boxinstseg_b200.models.losses.levelset_loss import levelset_assembly  # noqa: E402

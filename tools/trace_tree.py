@@ -10,8 +10,9 @@ import torch
 import torch.nn.functional as F
 
 from boxinstseg_b200 import _lib as L
-from boxinstseg_b200.ops.tree_filter import MinimumSpanningTree, TreeFilter2D, bfs
-from boxinstseg_b200.ops.tree_filter.functions.refine import refine
+from boxinstseg_b200.ops.tree_filter import MinimumSpanningTree, TreeFilter2D
+from boxinstseg_b200.ops.tree_filter.functions.refine import refine_ordered
+from boxinstseg_b200.ops.tree_filter.tree_filter_cuda import bfs_order
 
 dev = torch.device('cuda:0')
 g = torch.Generator(device=dev).manual_seed(0)
@@ -19,20 +20,20 @@ n, h, w = 2, 200, 256
 guide = F.interpolate(torch.randn(n, 3, h // 8, w // 8, device=dev, generator=g), size=(h, w), mode='bilinear') + 0.05 * torch.randn(n, 3, h, w, device=dev, generator=g)
 tree = MinimumSpanningTree(TreeFilter2D.norm2_distance)(guide)
 tf = TreeFilter2D()
-idx, par, chd = bfs(tree, 4)
+order = bfs_order(tree, 4)
 feat = torch.rand(n, 1, h * w, device=dev, generator=g)
-ew = tf.build_edge_weight(guide, idx, par, False, chd).detach()
+ew = tf.build_edge_weight(guide, order.sorted_index, order.sorted_parent, False, order.sorted_child).detach()
 for _ in range(3):
-    refine(feat, ew, idx, par, chd, False)
+    refine_ordered(feat, ew, order, False)
 torch.cuda.synchronize()
 handle = ctypes.CDLL(L.LIB_PATH)
 buf = np.zeros((6, 4096), dtype=np.int64)
 assert handle.bxs_debug_tree_trace(ctypes.c_void_p(buf.ctypes.data)) == 0
-levels = int(getattr(idx, '_bxs_levels')[1][0])
+levels = int(order.num_levels[0])
 m = min(levels, 4096) - 1
 c0, c1, c2, p0, p1, p2 = (buf[k][:m] for k in range(6))
 c0n, p0n = buf[0][1:m + 1], buf[3][1:m + 1]
-lvl = getattr(idx, '_bxs_levels')[0][0].cpu().numpy()
+lvl = order.level_start[0].cpu().numpy()
 width = (lvl[1:levels + 1] - lvl[:levels])[::-1][:m]        # the up pass starts at the deepest level
 
 
