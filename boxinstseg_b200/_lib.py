@@ -97,9 +97,15 @@ SIGNATURES = {
     'bxs_lsap_solve': [c_p] * 4 + [c_i64, c_int] + [c_p] * 4,
     'bxs_sigmoid_focal_loss_levels_forward_workspace_bytes': [c_p, c_i64, c_i64],
     'bxs_sigmoid_focal_loss_levels_forward': [c_p] * 7 + [c_i64] * 3 + [c_f] * 3 + [c_p],
+    'bxs_sigmoid_focal_loss_cells_forward_workspace_bytes': [c_p, c_i64, c_i64],
+    'bxs_sigmoid_focal_loss_cells_forward': [c_p] * 7 + [c_i64] * 3 + [c_f] * 3 + [c_p],
     'bxs_softmax_cross_entropy_layers_forward_workspace_bytes': [c_i64] * 3,
     'bxs_softmax_cross_entropy_layers_forward': [c_p] * 6 + [c_i64] * 4 + [c_f, c_p],
     'bxs_softmax_cross_entropy_layers_backward': [c_p] * 2 + [c_i64] * 4 + [c_p],
+    'bxs_fcos_loss_workspace_bytes': [c_p, c_p, c_i64, c_i64],
+    'bxs_fcos_loss_stats': [c_p] * 7 + [c_i64] * 3 + [c_p],
+    'bxs_fcos_loss_forward': [c_p] * 13 + [c_i64] * 3 + [c_f, c_f, c_p],
+    'bxs_fcos_loss_backward': [c_p, c_i64, c_p, c_p, c_i64, c_p, c_p],
 }
 _RESTYPE = {'bxs_mst_workspace_bytes': c_i64, 'bxs_bfs_workspace_bytes': c_i64, 'bxs_refine_scratch_bytes': c_i64, 'bxs_lcm_workspace_bytes': c_i64, 'bxs_meanfield_workspace_bytes': c_i64, 'bxs_projection_workspace_bytes': c_i64,'bxs_condinst_head_workspace_bytes': c_i64, 'bxs_last_error': ctypes.c_char_p, 'bxs_boxinst_loss_workspace_bytes': c_i64,
              'bxs_boxinst_loss_fused_workspace_bytes': c_i64, 'bxs_boxinst_loss_fused_sched_bytes': c_i64,
@@ -109,7 +115,8 @@ _RESTYPE = {'bxs_mst_workspace_bytes': c_i64, 'bxs_bfs_workspace_bytes': c_i64, 
              'bxs_discobox_loss_workspace_bytes': c_i64, 'bxs_dynconv1x1_cells_forward_workspace_bytes': c_i64,
              'bxs_dynconv1x1_cells_backward_workspace_bytes': c_i64,
              'bxs_sigmoid_focal_loss_levels_forward_workspace_bytes': c_i64,
-             'bxs_softmax_cross_entropy_layers_forward_workspace_bytes': c_i64}
+             'bxs_softmax_cross_entropy_layers_forward_workspace_bytes': c_i64,
+             'bxs_sigmoid_focal_loss_cells_forward_workspace_bytes': c_i64, 'bxs_fcos_loss_workspace_bytes': c_i64}
 
 _STATUS = {-1: 'invalid argument', -2: 'kernel launch failed', -3: 'unsupported shape', -4: 'no CUDA device'}
 

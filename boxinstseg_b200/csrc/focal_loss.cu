@@ -1,6 +1,7 @@
-// Sigmoid focal loss of BoxSOLOv2's category branch over every FPN level at once -- box_solov2_head.py:370-383
+// Sigmoid focal loss over every FPN level at once -- BoxSOLOv2's category branch (box_solov2_head.py:370-383)
 //     self.loss_cate(cat([cate_pred.permute(0,2,3,1).reshape(-1,C) for each level]), cat(labels), avg_factor=num_ins + 1)
-//     with mmdet's FocalLoss(use_sigmoid=True) (mmdet/models/losses/focal_loss.py, utils.py: weight_reduce_loss).
+//     and CondInstBoxHead's classification branch on the rectangular FCOS levels (condinst_head.py:404-445, avg_factor =
+//     num_pos), with mmdet's FocalLoss(use_sigmoid=True) (mmdet/models/losses/focal_loss.py, utils.py: weight_reduce_loss).
 //
 //     The logits stay in each level's own NCHW layout: a CTA owns FL_TILE cells of one (level, image), loads their labels once,
 //     walks the C class planes with reads coalesced along the cells, writes d loss / d logit in the same pass and leaves one
@@ -92,20 +93,21 @@ __global__ void __launch_bounds__(FL_RED_NT) focal_reduce_kernel(const float* __
   if (threadIdx.x == 0) *loss = loss_weight * ((float)acc / (*avg_factor + FLT_EPSILON));
 }
 
-// fills the level table; BXS_OK or the status of the first argument that is out of range
-int plan(FocalTable& tab, const int64_t* grid_host, int64_t n_levels, int64_t B, int64_t C) {
-  if (!grid_host || n_levels <= 0 || B <= 0 || C <= 0) return BXS_ERR_INVALID_ARG;
+// fills the level table from each level's cell count (H_l * W_l); BXS_OK or the status of the first argument that is out of
+// range
+int plan(FocalTable& tab, const int64_t* cells_host, int64_t n_levels, int64_t B, int64_t C) {
+  if (!cells_host || n_levels <= 0 || B <= 0 || C <= 0) return BXS_ERR_INVALID_ARG;
   if (n_levels > FL_MAX_LEVELS) return BXS_ERR_UNSUPPORTED;
   if (C > INT32_MAX) return BXS_ERR_UNSUPPORTED;
   tab = FocalTable{};
   tab.n_levels = (int)n_levels;
   int64_t total = 0;
   for (int64_t l = 0; l < n_levels; ++l) {
-    const int64_t S = grid_host[l];
-    if (S <= 0) return BXS_ERR_INVALID_ARG;
-    if (S > (1 << 15)) return BXS_ERR_UNSUPPORTED;                   // S2 * B * C stays far inside int64
-    tab.lv[l].S2 = S * S;
-    tab.lv[l].tiles = ceil_div(S * S, FL_TILE);
+    const int64_t n = cells_host[l];
+    if (n <= 0) return BXS_ERR_INVALID_ARG;
+    if (n > (int64_t(1) << 30)) return BXS_ERR_UNSUPPORTED;          // S2 * B * C stays far inside int64
+    tab.lv[l].S2 = n;
+    tab.lv[l].tiles = ceil_div(n, FL_TILE);
     tab.first[l] = total;
     total += B * tab.lv[l].tiles;
   }
@@ -113,25 +115,23 @@ int plan(FocalTable& tab, const int64_t* grid_host, int64_t n_levels, int64_t B,
   return total > INT32_MAX ? BXS_ERR_UNSUPPORTED : BXS_OK;
 }
 
-}  // namespace
-}  // namespace bxs
-
-using namespace bxs;
-
-extern "C" int64_t bxs_sigmoid_focal_loss_levels_forward_workspace_bytes(const int64_t* grid_host, int64_t n_levels, int64_t B) {
-  FocalTable tab;
-  if (plan(tab, grid_host, n_levels, B, 1) != BXS_OK) return 0;
-  return (int64_t)align_up((size_t)tab.first[n_levels] * sizeof(float));
+// the square-grid form: S_l <= 0 stays invalid, S_l > 2^15 (more than 2^30 cells) stays unsupported
+int plan_grid(FocalTable& tab, const int64_t* grid_host, int64_t n_levels, int64_t B, int64_t C) {
+  if (!grid_host || n_levels <= 0 || n_levels > FL_MAX_LEVELS) return plan(tab, grid_host, n_levels, B, C);
+  int64_t cells[FL_MAX_LEVELS];
+  for (int64_t l = 0; l < n_levels; ++l) {
+    const int64_t S = grid_host[l];
+    cells[l] = S <= 0 ? S : S > (1 << 15) ? (int64_t(1) << 31) : S * S;
+  }
+  return plan(tab, cells, n_levels, B, C);
 }
 
-extern "C" int bxs_sigmoid_focal_loss_levels_forward(const float* const* logits_host, const int64_t* const* labels_host,
-                                                     const int64_t* grid_host, float* const* grad_host,
-                                                     const float* avg_factor, float* loss, void* workspace, int64_t n_levels,
-                                                     int64_t B, int64_t C, float gamma, float alpha, float loss_weight,
-                                                     bxs_stream_t stream) {
-  FocalTable tab;
-  if (const int rc = plan(tab, grid_host, n_levels, B, C)) return rc;
+// fills the table's pointers and runs both launches
+int focal_forward(FocalTable& tab, const float* const* logits_host, const int64_t* const* labels_host,
+                  float* const* grad_host, const float* avg_factor, float* loss, void* workspace, int64_t C, float gamma,
+                  float alpha, float loss_weight, bxs_stream_t stream) {
   if (!logits_host || !labels_host || !avg_factor || !loss || !workspace || !(gamma >= 0.f)) return BXS_ERR_INVALID_ARG;
+  const int64_t n_levels = tab.n_levels;
   for (int64_t l = 0; l < n_levels; ++l) {
     if (!logits_host[l] || !labels_host[l] || (grad_host && !grad_host[l])) return BXS_ERR_INVALID_ARG;
     tab.lv[l].logits = logits_host[l];
@@ -145,4 +145,43 @@ extern "C" int bxs_sigmoid_focal_loss_levels_forward(const float* const* logits_
   if (const int rc = check_launch()) return rc;
   focal_reduce_kernel<<<1, FL_RED_NT, 0, st>>>(partials, ctas, avg_factor, loss_weight, loss);
   return check_launch();
+}
+
+}  // namespace
+}  // namespace bxs
+
+using namespace bxs;
+
+extern "C" int64_t bxs_sigmoid_focal_loss_levels_forward_workspace_bytes(const int64_t* grid_host, int64_t n_levels, int64_t B) {
+  FocalTable tab;
+  if (plan_grid(tab, grid_host, n_levels, B, 1) != BXS_OK) return 0;
+  return (int64_t)align_up((size_t)tab.first[n_levels] * sizeof(float));
+}
+
+extern "C" int bxs_sigmoid_focal_loss_levels_forward(const float* const* logits_host, const int64_t* const* labels_host,
+                                                     const int64_t* grid_host, float* const* grad_host,
+                                                     const float* avg_factor, float* loss, void* workspace, int64_t n_levels,
+                                                     int64_t B, int64_t C, float gamma, float alpha, float loss_weight,
+                                                     bxs_stream_t stream) {
+  FocalTable tab;
+  if (const int rc = plan_grid(tab, grid_host, n_levels, B, C)) return rc;
+  return focal_forward(tab, logits_host, labels_host, grad_host, avg_factor, loss, workspace, C, gamma, alpha, loss_weight,
+                       stream);
+}
+
+extern "C" int64_t bxs_sigmoid_focal_loss_cells_forward_workspace_bytes(const int64_t* cells_host, int64_t n_levels, int64_t B) {
+  FocalTable tab;
+  if (plan(tab, cells_host, n_levels, B, 1) != BXS_OK) return 0;
+  return (int64_t)align_up((size_t)tab.first[n_levels] * sizeof(float));
+}
+
+extern "C" int bxs_sigmoid_focal_loss_cells_forward(const float* const* logits_host, const int64_t* const* labels_host,
+                                                    const int64_t* cells_host, float* const* grad_host,
+                                                    const float* avg_factor, float* loss, void* workspace, int64_t n_levels,
+                                                    int64_t B, int64_t C, float gamma, float alpha, float loss_weight,
+                                                    bxs_stream_t stream) {
+  FocalTable tab;
+  if (const int rc = plan(tab, cells_host, n_levels, B, C)) return rc;
+  return focal_forward(tab, logits_host, labels_host, grad_host, avg_factor, loss, workspace, C, gamma, alpha, loss_weight,
+                       stream);
 }

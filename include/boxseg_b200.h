@@ -597,6 +597,16 @@ int bxs_sigmoid_focal_loss_levels_forward(const float* const* logits_host, const
                                           float* loss, void* workspace, int64_t n_levels, int64_t B, int64_t C, float gamma,
                                           float alpha, float loss_weight, bxs_stream_t stream);
 
+/* The same loss on rectangular levels (CondInstBoxHead's FCOS levels, condinst_head.py:404-445): cells_host[l] = H_l * W_l,
+ * logits_host[l] f32 [B,C,H_l,W_l], labels_host[l] i64 [B,H_l*W_l] (cell y*W_l + x).  Everything else as above; the
+ * square-grid form is this one with cells_host[l] = S_l^2.  BXS_ERR_INVALID_ARG: as above with a cell count <= 0;
+ * BXS_ERR_UNSUPPORTED: n_levels > 8, a cell count above 2^30. */
+int64_t bxs_sigmoid_focal_loss_cells_forward_workspace_bytes(const int64_t* cells_host, int64_t n_levels, int64_t B);
+int bxs_sigmoid_focal_loss_cells_forward(const float* const* logits_host, const int64_t* const* labels_host,
+                                         const int64_t* cells_host, float* const* grad_host, const float* avg_factor,
+                                         float* loss, void* workspace, int64_t n_levels, int64_t B, int64_t C, float gamma,
+                                         float alpha, float loss_weight, bxs_stream_t stream);
+
 /* ---------------------------------------------------------------------------------------
  * Box2Mask's classification loss over every decoder layer    replaces, per layer, mmdet's
  *     CrossEntropyLoss(use_sigmoid=False, reduction='mean', class_weight=w)(cls_scores.flatten(0, 1), labels.flatten(0, 1),
@@ -622,6 +632,44 @@ int bxs_softmax_cross_entropy_layers_forward(const float* const* scores_host, co
                                              int64_t Q, int64_t K, float loss_weight, bxs_stream_t stream);
 int bxs_softmax_cross_entropy_layers_backward(float* const* grad_host, const float* g_loss, int64_t L, int64_t B, int64_t Q,
                                               int64_t K, bxs_stream_t stream);
+
+/* ---------------------------------------------------------------------------------------
+ * CondInstBoxHead's regression and centerness losses over every FCOS level and image    replaces the permute / cat of
+ *     bbox_pred and centerness, nonzero(), the gathers, centerness_target, distance2bbox, GIoULoss(reduction='mean') with
+ *     weight = centerness targets and avg_factor = max(reduce_mean(sum ct), 1e-6), and CrossEntropyLoss(use_sigmoid=True)
+ *     with avg_factor = max(reduce_mean(num_pos), 1) (condinst_head.py:437-469).
+ * Level l (n_levels <= 8, H_l = height_host[l], W_l = width_host[l], P_l = H_l*W_l, stride_host[l] > 0): labels_host[l] i64
+ * [B*P_l] and targets_host[l] f32 [B*P_l,4] as bxs_fcos_targets writes them (point b*P_l + y*W_l + x; a label in [0, C) is
+ * a positive), pred_host[l] f32 [B,4,H_l,W_l] (l, t, r, b distances), ctr_host[l] f32 [B,1,H_l,W_l] (logits).  The point
+ * is ((x + 0.5) * stride, (y + 0.5) * stride); ct = sqrt(min(l,r)/max(l,r) * min(t,b)/max(t,b)) of the target.
+ * stats: stats f32 [2] on the device = (number of positives, sum of their ct).
+ * forward: den f32 [2] on the device = (max(reduce_mean(num_pos), 1), max(reduce_mean(sum ct), 1e-6));
+ *   loss_bbox = lw_bbox * sum ct (1 - GIoU) / (den[1] + FLT_EPSILON) and
+ *   loss_ctr = lw_ctr * sum BCE(ctr, ct) / (den[0] + FLT_EPSILON), f32 scalars on the device,
+ *   GIoU with eps 1e-6 in the reference's operation order.  g_pred_host[l] f32 [B,4,H_l,W_l] and g_ctr_host[l] f32
+ *   [B,1,H_l,W_l] (either array NULL: not needed) = d loss_bbox / d pred and d loss_ctr / d ctr, zero at every point that is
+ *   not a positive.  At ties the gradient is autograd's for the reference's lines: half to each side of an elementwise
+ *   max / min, clamp(min=0) passes at 0.
+ * backward: g_pred [n_pred] *= *g_loss_bbox and g_ctr [n_ctr] *= *g_loss_ctr IN PLACE (device scalars; a NULL buffer is
+ *   skipped, an upstream gradient of exactly 1 returns at once).  Call it at most once per forward.
+ * stats and forward launch one kernel of one thread per point and a one-CTA sum of its per-CTA partials in a fixed order:
+ * bit-identical from run to run, no atomics, no host synchronisation.  No vector loads: any 4-byte aligned base works.
+ * workspace: bxs_fcos_loss_workspace_bytes(height_host, width_host, n_levels, B) bytes (0 for invalid arguments), for
+ * stats and forward alike.  The *_host arrays are HOST arrays, copied into kernel parameters.  BXS_ERR_INVALID_ARG: a NULL
+ * pointer the call needs, n_levels, B, C, an H_l or W_l <= 0, a stride not positive and finite, a negative n.
+ * BXS_ERR_UNSUPPORTED: n_levels > 8, C or B * sum P_l above INT32_MAX.  All checks run before any device call.
+ * --------------------------------------------------------------------------------------- */
+int64_t bxs_fcos_loss_workspace_bytes(const int64_t* height_host, const int64_t* width_host, int64_t n_levels, int64_t B);
+int bxs_fcos_loss_stats(const int64_t* const* labels_host, const float* const* targets_host, const int64_t* height_host,
+                        const int64_t* width_host, const float* stride_host, float* stats, void* workspace, int64_t n_levels,
+                        int64_t B, int64_t C, bxs_stream_t stream);
+int bxs_fcos_loss_forward(const float* const* pred_host, const float* const* ctr_host, const int64_t* const* labels_host,
+                          const float* const* targets_host, float* const* g_pred_host, float* const* g_ctr_host,
+                          const int64_t* height_host, const int64_t* width_host, const float* stride_host, const float* den,
+                          float* loss_bbox, float* loss_ctr, void* workspace, int64_t n_levels, int64_t B, int64_t C, float lw_bbox, float lw_ctr,
+                          bxs_stream_t stream);
+int bxs_fcos_loss_backward(float* g_pred, int64_t n_pred, const float* g_loss_bbox, float* g_ctr, int64_t n_ctr,
+                           const float* g_loss_ctr, bxs_stream_t stream);
 
 #ifdef __cplusplus
 }
