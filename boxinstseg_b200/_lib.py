@@ -72,7 +72,9 @@ SIGNATURES = {
     'bxs_dynconv1x1_cells_forward': [c_p] * 9 + [c_i64] * 4 + [c_p],
     'bxs_dynconv1x1_cells_backward_workspace_bytes': [c_p] * 4 + [c_i64] * 4,
     'bxs_dynconv1x1_cells_backward': [c_p] * 11 + [c_i64] * 4 + [c_p],
-    'bxs_dynconv1x1_half_forward': [c_p] * 3 + [c_i64] * 4 + [c_int, c_p],
+    'bxs_disco_cells_pack': [c_p] * 4 + [c_i64] + [c_p] * 2 + [c_i64] * 4 + [c_int, c_p],
+    'bxs_disco_cells_unpack_grad': [c_p] * 4 + [c_i64] + [c_p] + [c_i64] * 4 + [c_int, c_p],
+    'bxs_dynconv1x1_half_forward':[c_p] * 3 + [c_i64] * 4 + [c_int, c_p],
     'bxs_dynconv1x1_half_backward_workspace_bytes': [c_i64] * 4 + [c_int],
     'bxs_dynconv1x1_half_backward': [c_p] * 6 + [c_i64] * 4 + [c_int, c_p],
     'bxs_upsampled_rowcol_max': [c_p] * 4 + [c_i64] * 5 + [c_int, c_p],

@@ -18,7 +18,7 @@ import torch.nn.functional as F
 
 from ...ops.box2mask import attention_mask
 from ...ops.discobox import HALF_DTYPES, discobox_mask_loss
-from ...ops.dynconv import box2mask_mask_pred, dynconv1x1, solo_cells_conv, solo_dynamic_conv
+from ...ops.dynconv import box2mask_mask_pred, disco_cells_conv, dynconv1x1, solo_cells_conv, solo_dynamic_conv
 from ...ops.focal import sigmoid_focal_loss_levels
 from ...ops.lsap import solve_batched
 from ...ops.resize import bilinear_resize, scale_target as _scale_target   # a18: F.interpolate / _scale_target as kernels
@@ -328,11 +328,13 @@ class DiscoBoxSOLOv2Head(nn.Module):
     """DiscoBox head: the mask-loss path (a3, a16, a17) and, with a ``loss_corr`` config (discobox_head.py:720-749), the
     semantic-correspondence loss on top of it (f4: ``corr_loss``, models/dense_heads/disco_corr.py)."""
 
-    def __init__(self, num_classes=80, in_channels=256, loss_ins=None, loss_ts=None, loss_corr=None, **cfg):
+    def __init__(self, num_classes=80, in_channels=256, loss_ins=None, loss_ts=None, loss_corr=None, loss_cate=None, **cfg):
         super().__init__()
         self.num_classes = num_classes
+        self.cate_out_channels = num_classes
         self.in_channels = in_channels
         self.cfg = cfg
+        self.loss_cate = dict(loss_cate or dict(type='FocalLoss', use_sigmoid=True, gamma=2.0, alpha=0.25, loss_weight=1.0))
         loss_ins = loss_ins or dict(loss_weight=1.0)
         loss_ts = loss_ts or dict(loss_weight=1.0, alpha0=2.0, theta0=0.5, theta1=30.0, theta2=20.0, kernel=3, base=0.10,
                                   max_iter=10)
@@ -348,7 +350,15 @@ class DiscoBoxSOLOv2Head(nn.Module):
 
     def _bxs_post_init(self):
         """Also runs after the REFERENCE class's ``__init__`` when mmdet is importable (``register(partial=True)``): the
-        correspondence state is then rebuilt from the attributes that constructor leaves behind (:720-749)."""
+        correspondence state is then rebuilt from the attributes that constructor leaves behind (:720-749), and the focal
+        parameters are read from the FocalLoss module it built.  Never raises: a ``loss_cate`` outside the envelope is
+        recorded, and ``loss`` then defers to the reference or raises."""
+        from .condinst_box_head import _loss_cfg
+        kind, c = _loss_cfg(getattr(self, 'loss_cate', None), 'FocalLoss')
+        if kind != 'FocalLoss' or not c.get('use_sigmoid', True) or c.get('activated', False) or c.get('reduction', 'mean') != 'mean':
+            self.focal = f'loss_cate {kind} {c}'
+        else:
+            self.focal = (float(c.get('gamma', 2.0)), float(c.get('alpha', 0.25)), float(c.get('loss_weight', 1.0)))
         self.corr = None
         solver, queues = getattr(self, 'semantic_corr_solver', None), getattr(self, 'object_queues', None)
         if solver is None or queues is None:
@@ -402,9 +412,16 @@ class DiscoBoxSOLOv2Head(nn.Module):
         cells gathered by ``grid_order``, one dynamic convolution per (level, image) with objects (a3: the wgmma kernel).
         ``*_kernel_preds_raw``: per level [B,C,g,g]; ``*_ins_pred`` [B,C,H,W]; ``gt_mask_list``: per image uint8 [G,H',W'] device
         tensors.  Returns (s_ins_pred_list, t_ins_pred_list, img_ind_list, ins_labels, kernel_label_list) with None for a level
-        without objects.  Plain torch around ``conv`` (default: ``self.dynamic_conv``)."""
+        without objects.  Without ``conv``, every level and image of a network is one ``disco_cells_conv`` call (one
+        dense wgmma launch on the packed kernels, the same values as one call per (level, image)); a given ``conv``
+        (mask_feat_img [C,h,w], kernels [C,I]) -> [I,h,w] runs once per (level, image) with objects, in plain torch."""
+        return self._corr_inputs(s_kernel_preds_raw, t_kernel_preds_raw, s_ins_pred, t_ins_pred, gt_bbox_list, gt_label_list,
+                                 gt_mask_list, use_ind_teacher, best, conv)[0]
+
+    def _corr_inputs(self, s_kernel_preds_raw, t_kernel_preds_raw, s_ins_pred, t_ins_pred, gt_bbox_list, gt_label_list,
+                     gt_mask_list, use_ind_teacher, best, conv):
+        """``corr_inputs`` and the per-image targets it was built from (``disco_target_single``'s four lists per image)."""
         from .disco_targets import disco_target_single
-        conv = conv or self.dynamic_conv
         scale_ranges, strides, grids, sigma = self._grid_cfg()
         fsize = tuple(s_ins_pred.shape[-2:])
         per_img = [disco_target_single(b, l, m, fsize, scale_ranges, strides, grids, sigma, self.num_classes, best=best)
@@ -412,6 +429,11 @@ class DiscoBoxSOLOv2Head(nn.Module):
         L_, B = len(grids), len(per_img)
         ins_labels = [torch.cat([per_img[b][0][lv] for b in range(B)], 0) for lv in range(L_)]
         klabels = [torch.cat([per_img[b][1][lv].reshape(-1)[per_img[b][3][lv]] for b in range(B)], 0) for lv in range(L_)]
+        if conv is None:
+            orders = [[per_img[b][3][lv] for b in range(B)] for lv in range(L_)]
+            s_list, img_list = disco_cells_conv(s_ins_pred, s_kernel_preds_raw, orders)
+            t_list = disco_cells_conv(t_ins_pred, t_kernel_preds_raw, orders)[0] if use_ind_teacher else [None] * L_
+            return (s_list, t_list, img_list, ins_labels, klabels), per_img
         s_list, t_list, img_list = [], [], []
         for lv in range(L_):
             s_lv, t_lv, i_lv = [], [], []
@@ -428,7 +450,7 @@ class DiscoBoxSOLOv2Head(nn.Module):
             s_list.append(torch.cat(s_lv, 0) if s_lv else None)
             t_list.append(torch.cat(t_lv, 0) if t_lv else None)
             img_list.append(torch.cat(i_lv, 0) if i_lv else None)
-        return s_list, t_list, img_list, ins_labels, klabels
+        return (s_list, t_list, img_list, ins_labels, klabels), per_img
 
     # f4 -- discobox_head.py:900-1139, the reference's signature
     def corr_loss(self, cate_preds, s_kernel_preds_raw, t_kernel_preds_raw, s_ins_pred, t_ins_pred, gt_bbox_list, gt_label_list,
@@ -446,6 +468,55 @@ class DiscoBoxSOLOv2Head(nn.Module):
         mf = MeanField(color_feats, alpha0=self.alpha0, theta0=self.theta0, theta1=self.theta1, theta2=self.theta2,
                        iter=self.crf_max_iter, kernel_size=self.mkernel, base=self.crf_base, gamma=gamma)
         return self.corr.levels(s_list, t_list, img_list, ins_labels, klabels, s_feat, t_feat, mf, use_ind_teacher)
+
+    # discobox_head.py:1142-1360, the reference's signature
+    def loss(self, cate_preds, s_kernel_preds_raw, t_kernel_preds_raw, s_ins_pred, t_ins_pred, gt_bbox_list, gt_label_list,
+             gt_mask_list, img_metas, cfg, img=None, gt_bboxes_ignore=None, use_loss_ts=False, use_ind_teacher=False,
+             use_corr=False, s_feat=None, t_feat=None):
+        """dict(loss_ins, loss_ts, loss_cate, loss_corr) as the reference computes them.  ``gt_mask_list``: per image uint8
+        [G,H,W] device tensors, or anything with mmdet's ``to_tensor(dtype, device)`` (BitmapMasks).
+
+        The SOLO targets are built on the device (``solov2_target_single``'s lists; their per-(level, image) cell counts are
+        the one host read), every level's and image's dynamic convolution of a network is one ``disco_cells_conv`` call, the
+        mask losses run as ``mask_loss`` (one mean field over the batch), ``loss_cate`` is the focal kernel on the [B,C,S,S]
+        levels as they lie with ``avg_factor = num_ins + 1`` on the device, and with ``use_loss_ts and use_corr`` the
+        correspondence loss is ``corr_loss_levels`` on the ``best_target_single`` targets, its dice terms joining
+        ``loss_ts``.  No loss value is read back to the host.  Autocast is the caller's: under ``torch.autocast('cuda')`` the
+        convolutions take the autocast dtype, as the reference's ``@autocast()`` does.  Only the student receives gradients
+        (the teacher's grids and mask features are detached); the teacher is convolved only with ``use_ind_teacher``.
+        Where the reference returns ``torch.zeros(1)`` (no instance with a non-empty target) this returns a 0-d zero."""
+        if isinstance(self.focal, str):
+            ref = getattr(type(self), '_bxs_reference_class', None)
+            if ref is not None:
+                return ref.loss(self, cate_preds, s_kernel_preds_raw, t_kernel_preds_raw, s_ins_pred, t_ins_pred, gt_bbox_list,
+                                gt_label_list, gt_mask_list, img_metas, cfg, img, gt_bboxes_ignore, use_loss_ts,
+                                use_ind_teacher, use_corr, s_feat, t_feat)
+            raise NotImplementedError(f'DiscoBoxSOLOv2Head.loss: unsupported {self.focal}')
+        dev = s_ins_pred.device
+        masks = [(m if torch.is_tensor(m) else m.to_tensor(dtype=torch.uint8, device=dev)).to(dev, torch.uint8)
+                 for m in gt_mask_list]
+        t_kern = [k.detach() for k in t_kernel_preds_raw] if use_ind_teacher else None
+        t_ins = t_ins_pred.detach() if use_ind_teacher else None
+        (s_list, t_list, img_list, ins_labels, _), per_img = self._corr_inputs(
+            s_kernel_preds_raw, t_kern, s_ins_pred, t_ins, gt_bbox_list, gt_label_list, masks, use_ind_teacher, False, None)
+        color_feats = bilinear_resize(img, tuple(s_ins_pred.shape[-2:]), align_corners=True)             # :1201
+        out = self.mask_loss(s_list, ins_labels, img_list, color_feats, t_list if use_ind_teacher else None, use_loss_ts)
+        loss_ins, loss_ts = out['loss_ins'], out['loss_ts']
+        zero = color_feats.new_zeros(())
+        if use_loss_ts and use_corr:                                                                       # :1309-1337
+            c_s, c_t, c_img, c_lab, c_kl = self.corr_inputs(s_kernel_preds_raw, t_kern, s_ins_pred, t_ins, gt_bbox_list,
+                                                            gt_label_list, masks, use_ind_teacher=use_ind_teacher, best=True)
+            loss_corr, corr_ts = self.corr_loss_levels(c_s, c_t, c_img, c_lab, c_kl, s_feat[0], t_feat[0], color_feats,
+                                                       use_ind_teacher)
+            kept = sum(((t.flatten(1) != 0).any(1).sum() for s, t in zip(s_list, ins_labels) if s is not None), zero)
+            loss_ts = torch.where(kept > 0, loss_ts + corr_ts * self.ts_loss_weight, zero)    # only with terms of its own
+        else:
+            loss_corr = zero
+        B, n_lv = len(per_img), len(cate_preds)
+        cate_labels = [torch.stack([per_img[b][1][lv] for b in range(B)]) for lv in range(n_lv)]
+        num_ins = torch.stack([per_img[b][2][lv].sum() for b in range(B) for lv in range(n_lv)]).sum()
+        loss_cate = sigmoid_focal_loss_levels(cate_preds, cate_labels, num_ins + 1, *self.focal)
+        return dict(loss_ins=loss_ins, loss_ts=loss_ts, loss_cate=loss_cate, loss_corr=loss_corr)
 
     # a3 -- discobox_head.py:1206-1246
     @staticmethod

@@ -241,6 +241,77 @@ def solo_cells_conv(feature_pred, kernel_preds, cells, out_sizes):
     return list(_SoloCells.apply((level_op, counts), flat, *ops, *kerns))
 
 
+_PACK_DTYPE = {torch.float32: 0, torch.float16: 1, torch.bfloat16: 2}
+
+
+class _DiscoPack(torch.autograd.Function):
+    """Raw kernel grids -> packed [B,I_pad,C] rows (bxs_disco_cells_pack); backward: bxs_disco_cells_unpack_grad."""
+
+    @staticmethod
+    def forward(ctx, counts, I_pad, cells, *grids):
+        B, C = grids[0].shape[:2]
+        args = (_i64([g.shape[-1] for g in grids]), _i64(counts), L.ptr(cells), cells.numel(), len(grids), B, C, I_pad,
+                _PACK_DTYPE[grids[0].dtype])
+        packed = grids[0].new_empty((B, I_pad, C))
+        with torch.cuda.device(cells.device):
+            L.check(L.lib().bxs_disco_cells_pack(_ptrs(grids), args[0], args[1], args[2], args[3], L.ptr(packed), None,
+                                                 *args[4:], L.stream()), 'disco_cells_pack')
+        ctx.save_for_backward(cells)
+        ctx.args = args
+        ctx.shapes = [g.shape for g in grids]
+        return packed
+
+    @staticmethod
+    def backward(ctx, g_packed):
+        (cells,) = ctx.saved_tensors
+        grid, counts, _, n_cells, n_levels, B, C, I_pad, dt = ctx.args
+        g = L.dense_aligned(g_packed.to(next(k for k, v in _PACK_DTYPE.items() if v == dt)))
+        g_grids = [g.new_empty(s) for s in ctx.shapes]
+        with torch.cuda.device(g.device):
+            L.check(L.lib().bxs_disco_cells_unpack_grad(L.ptr(g), grid, counts, L.ptr(cells), n_cells, _ptrs(g_grids),
+                                                        n_levels, B, C, I_pad, dt, L.stream()), 'disco_cells_unpack_grad')
+        return (None, None, None, *g_grids)
+
+
+def disco_cells_conv(ins_pred, kernel_preds_raw, grid_orders):
+    """Every (level, image) dynamic convolution of DiscoBox (discobox_head.py:1180-1246) in ONE ``dynconv1x1`` call.
+
+    ins_pred [B,C,h,w]; kernel_preds_raw: per level the raw grid [B,C,S,S]; grid_orders: per level a list of B int tensors,
+    the covered cells (gy*S + gx) of each image in the target builder's order, repeats included.  Every level convolves the
+    same ``ins_pred[b]``, so the kernels of all levels of image b are packed, in the grids' dtype, into one [B,I_pad,C]
+    operand (``bxs_disco_cells_pack``; I_pad the largest per-image total, zero rows past an image's own) and convolved by
+    ``dynconv1x1`` under its dtype and autocast rules.  Returns (per level [n_l,h,w] or None for a level without cells, per
+    level the int64 image of each row or None): the rows the reference concatenates.  Differentiable with respect to
+    ins_pred and kernel_preds_raw; d/d kernel_preds_raw sums repeated cells in row order (``bxs_disco_cells_unpack_grad``),
+    bit-identical from run to run.  The per-(level, image) counts are the cell tensors' shapes: nothing is read back."""
+    B = ins_pred.shape[0]
+    n_lv = len(kernel_preds_raw)
+    counts = [int(grid_orders[l][b].numel()) for l in range(n_lv) for b in range(B)]
+    totals = [sum(counts[l * B + b] for l in range(n_lv)) for b in range(B)]
+    I_pad = max(totals)
+    dev = ins_pred.device
+    if I_pad == 0:
+        return [None] * n_lv, [None] * n_lv
+    dt = kernel_preds_raw[0].dtype if kernel_preds_raw[0].dtype in _PACK_DTYPE else torch.float32
+    grids = [L.dense_aligned(k.to(dt)) for k in kernel_preds_raw]
+    L.require_cuda(*grids)
+    cells = torch.cat([grid_orders[l][b].reshape(-1) for l in range(n_lv) for b in range(B)]).to(dev, torch.int32)
+    packed = _DiscoPack.apply(counts, I_pad, cells, *grids)
+    rows = dynconv1x1(ins_pred, packed)                                                 # [B,I_pad,h,w]
+    preds, img_inds = [], []
+    row0 = [0] * B
+    for l in range(n_lv):
+        n = counts[l * B:(l + 1) * B]
+        if not sum(n):
+            preds.append(None)
+            img_inds.append(None)
+            continue
+        preds.append(torch.cat([rows[b, row0[b]:row0[b] + n[b]] for b in range(B) if n[b]], 0))
+        img_inds.append(torch.cat([torch.full((n[b],), b, dtype=torch.int64, device=dev) for b in range(B) if n[b]]))
+        row0 = [r + c for r, c in zip(row0, n)]
+    return preds, img_inds
+
+
 def box2mask_mask_pred(mask_embed, mask_feature):
     """Box2Mask call site (box2mask_head.py:345): einsum('bqc,bchw->bqhw')."""
     return dynconv1x1(mask_feature, mask_embed)

@@ -379,6 +379,29 @@ int bxs_dynconv1x1_cells_backward(const float* const* operands_host, const int64
                                   float* const* g_operands_host, float* const* g_kernels_host, void* workspace,
                                   int64_t n_levels, int64_t n_ops, int64_t B, int64_t C, bxs_stream_t stream);
 
+/* a3  DiscoBox's dynamic kernels of the covered cells, packed for one dense convolution per network
+ *     replaces the gather kernel_preds[l][b].view(C, -1)[:, grid_order] (discobox_head.py:1180-1189) of every (level, image):
+ *     all levels of image b convolve the same s_ins_pred[b], so bxs_dynconv1x1_forward / _half_forward on the packed
+ *     [B,I_pad,C] operand computes every (level, image) convolution of :1214-1227 in one call.
+ * grids_host[l] [B,C,S_l,S_l] (S_l = grid_host[l]) of the element type dtype (0 float32, 1 float16, 2 bfloat16);
+ * counts_host [n_levels*B]: rows of (level, image); cells i32 [n_cells] on the device: the cell (gy*S_l + gx) of every row,
+ * level-major, then image-major, each (level, image) in the order given (repeats allowed: DiscoBox appends a cell once per
+ * ground truth that covers it, :1511-1520).  packed [B,I_pad,C]: the rows of image b level by level, zeros past its total.
+ * status (device i32, may be NULL): set to BXS_ERR_INVALID_ARG when a cell lies outside [0, S_l^2); that row is packed as
+ * zeros and nothing outside the grids is read.  The caller zeroes it; the call never clears it.
+ * unpack_grad: g_packed [B,I_pad,C] -> g_grids_host[l] [B,C,S_l,S_l]: every (cell, channel) gets the sum over the rows of
+ * its (level, image) that name the cell, in row order, in FP32, rounded once to dtype; every other cell 0.  No atomics:
+ * bit-identical from run to run.  Neither needs a workspace.  No host synchronisation.
+ * Limits: n_levels <= 8, B <= 16, S_l <= 64, I_pad <= 2048 (BXS_ERR_UNSUPPORTED).  BXS_ERR_INVALID_ARG: a NULL pointer the
+ * shapes need, a non-positive size, an unknown dtype, a negative count, counts whose sum is not n_cells, an image whose
+ * rows exceed I_pad.  All checks run on the host before any device call. */
+int bxs_disco_cells_pack(const void* const* grids_host, const int64_t* grid_host, const int64_t* counts_host,
+                         const int32_t* cells, int64_t n_cells, void* packed, int32_t* status, int64_t n_levels, int64_t B,
+                         int64_t C, int64_t I_pad, int dtype, bxs_stream_t stream);
+int bxs_disco_cells_unpack_grad(const void* g_packed, const int64_t* grid_host, const int64_t* counts_host,
+                                const int32_t* cells, int64_t n_cells, void* const* g_grids_host, int64_t n_levels, int64_t B,
+                                int64_t C, int64_t I_pad, int dtype, bxs_stream_t stream);
+
 /* The same three products with 16-bit operands, for callers that run under torch.autocast (the reference's DiscoBox
  * configs train in FP16): feat, kernels, out, g_out, g_feat and g_kernels are all of the type `dtype` names, and the
  * tensor cores accumulate in FP32.  Each result is rounded to `dtype` once, at the end; d/d kernel keeps FP32 split-K
