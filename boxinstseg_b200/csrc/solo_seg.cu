@@ -1,0 +1,309 @@
+// SOLOv2 inference (get_seg_single of box_solov2_head.py:503-590 and discobox_head.py:1559-1660): per-row mask statistics,
+// batched Matrix NMS (mmdet/core/post_processing/matrix_nms.py) and the fused two-stage mask paste.
+//
+//   stats:  one CTA per distinct candidate row (a (level, image, cell) of the mask predictions): every warp takes 32 pixels
+//           at a time, compares them with the threshold and ballots the word of the packed mask; the area is the popcount,
+//           and the masked sum is accumulated per lane in float64 and reduced in a fixed order (one float32 rounding).
+//   nms:    inter[i, j] = popcount(m_i & m_j) over 32 x 32 tiles of candidate pairs (i < j, same label, both valid), the
+//           packed words staged through shared memory in 32-word chunks; a tile without such a pair returns at once.  The
+//           IoU goes to the workspace and its column maximum (compensate_iou) is an atomicMax on the bits of a non-negative
+//           float: exact and order-independent.  A second launch gives every column its decay coefficient (one warp per
+//           column, the minimum over every valid row i, NaN propagating as torch.min does) and the decayed, filtered score.
+//   paste:  one thread per output pixel: its four intermediate taps of the (4h, 4w) upsampling, each a lerp of four input
+//           pixels (sigmoid on the fly for logits), rounded to the row dtype between and after the stages as ATen rounds a
+//           16-bit tensor (or, under autocast, kept in float32: autocast runs upsample_bilinear2d in float32), then the
+//           threshold.  The [n, 4h, 4w] intermediate of the reference never exists.
+#include <cuda_fp16.h>
+
+#include <type_traits>
+
+#include "common.cuh"
+#include "half_math.cuh"
+#include "solo_seg_core.cuh"
+
+namespace bxs {
+namespace {
+
+constexpr int SS_MAX_SRC = 8;
+constexpr int SS_NT = 256;
+constexpr int NMS_TILE = 32;
+
+struct RowSources {                    // by value in the kernel parameters
+  const void* p[SS_MAX_SRC];
+  int64_t start[SS_MAX_SRC + 1];       // first row id of each source; start[n]: the total
+  int n;
+};
+
+int make_sources(RowSources& s, const void* const* src_host, const int64_t* src_rows_host, int64_t n_src) {
+  if (!src_host || !src_rows_host || n_src <= 0) return BXS_ERR_INVALID_ARG;
+  if (n_src > SS_MAX_SRC) return BXS_ERR_UNSUPPORTED;
+  s = RowSources{};
+  s.n = (int)n_src;
+  for (int64_t k = 0; k < n_src; ++k) {
+    if (src_rows_host[k] < 0 || (src_rows_host[k] && !src_host[k])) return BXS_ERR_INVALID_ARG;
+    s.p[k] = src_host[k];
+    s.start[k + 1] = s.start[k] + src_rows_host[k];
+  }
+  return BXS_OK;
+}
+
+// the row of id g, or nullptr for an id outside the sources
+template <typename T>
+__device__ __forceinline__ const T* row_ptr(const RowSources& s, int64_t g, int64_t hw) {
+  if (g < 0 || g >= s.start[s.n]) return nullptr;
+  int k = 0;
+  while (k + 1 < s.n && g >= s.start[k + 1]) ++k;
+  return static_cast<const T*>(s.p[k]) + (g - s.start[k]) * hw;
+}
+
+// a row element as the probability the reference thresholds and interpolates (widened to float, exact)
+__device__ __forceinline__ float prob(float v, bool logits) { return logits ? sigmoid_exact(v) : v; }
+__device__ __forceinline__ float prob(__half v, bool logits) { return logits ? sigmoid_rounded(v) : __half2float(v); }
+
+template <typename T>
+__device__ __forceinline__ float to_dtype(float v) {
+  if constexpr (std::is_same<T, __half>::value) return round_to<__half>(v);
+  return v;
+}
+
+template <typename T>
+__global__ void __launch_bounds__(SS_NT) solo_stats_kernel(RowSources src, const int64_t* __restrict__ rows, int64_t hw,
+                                                           int64_t words, int logits, float thr, uint32_t* __restrict__ bits,
+                                                           int32_t* __restrict__ area, float* __restrict__ masked_sum) {
+  __shared__ double s_sum[SS_NT / kWarp];
+  __shared__ int s_cnt[SS_NT / kWarp];
+  const int64_t r = blockIdx.x;
+  const T* p = row_ptr<T>(src, rows[r], hw);
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const float t = to_dtype<T>(thr);
+  double acc = 0.0;
+  int cnt = 0;
+#pragma unroll 4
+  for (int64_t w = warp; w < words; w += SS_NT / kWarp) {
+    const int64_t i = w * kWarp + lane;
+    float v = 0.f;
+    if (p && i < hw) v = prob(p[i], logits);
+    const bool on = v > t;
+    const unsigned m = __ballot_sync(kFull, on);
+    if (lane == 0) {
+      bits[r * words + w] = m;
+      cnt += __popc(m);
+    }
+    if (on) acc += (double)v;
+  }
+  acc = warp_sum(acc);
+  if (lane == 0) {
+    s_sum[warp] = acc;
+    s_cnt[warp] = cnt;
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double s = 0.0;
+    int c = 0;
+    for (int k = 0; k < SS_NT / kWarp; ++k) {
+      s += s_sum[k];
+      c += s_cnt[k];
+    }
+    area[r] = c;
+    masked_sum[r] = (float)s;
+  }
+}
+
+// Candidate pairs of one 32 x 32 tile: rows i0 + ty + 8k (k < 4), column j0 + tx.
+__global__ void __launch_bounds__(SS_NT) nms_inter_kernel(const uint32_t* __restrict__ bits, int64_t words,
+                                                          const int64_t* __restrict__ row, const int64_t* __restrict__ label,
+                                                          const float* __restrict__ area, const int64_t* __restrict__ n_valid,
+                                                          int64_t N, int half_inter, float* __restrict__ iou,
+                                                          unsigned* __restrict__ comp_bits) {
+  __shared__ uint32_t sa[NMS_TILE][NMS_TILE + 1], sb[NMS_TILE][NMS_TILE + 1];
+  const int64_t b = blockIdx.z, i0 = (int64_t)blockIdx.y * NMS_TILE, j0 = (int64_t)blockIdx.x * NMS_TILE;
+  const int64_t nv = min(n_valid[b], N);
+  if (i0 >= j0 + NMS_TILE - 1 || i0 >= nv || j0 >= nv) return;
+  const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
+  const int64_t base = b * N, j = j0 + tx;
+  const int64_t lj = j < nv ? label[base + j] : -1;
+  bool need[4];
+  int any = 0;
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    const int64_t i = i0 + ty + 8 * k;
+    need[k] = j < nv && i < j && label[base + i] == lj;
+    any |= need[k];
+  }
+  if (!__syncthreads_or(any)) return;
+  const uint32_t* ra[4];
+  const uint32_t* rb[4];
+#pragma unroll
+  for (int m = 0; m < 4; ++m) {
+    const int64_t gi = i0 + ty + 8 * m, gj = j0 + ty + 8 * m;
+    ra[m] = gi < nv ? bits + row[base + gi] * words : nullptr;
+    rb[m] = gj < nv ? bits + row[base + gj] * words : nullptr;
+  }
+  int acc[4] = {0, 0, 0, 0};
+  for (int64_t w0 = 0; w0 < words; w0 += NMS_TILE) {
+    const int64_t w = w0 + tx;
+#pragma unroll
+    for (int m = 0; m < 4; ++m) {
+      sa[ty + 8 * m][tx] = ra[m] && w < words ? __ldg(ra[m] + w) : 0u;
+      sb[ty + 8 * m][tx] = rb[m] && w < words ? __ldg(rb[m] + w) : 0u;
+    }
+    __syncthreads();
+#pragma unroll 8
+    for (int kw = 0; kw < NMS_TILE; ++kw) {
+      const uint32_t bj = sb[tx][kw];
+#pragma unroll
+      for (int k = 0; k < 4; ++k) acc[k] += __popc(sa[ty + 8 * k][kw] & bj);
+    }
+    __syncthreads();
+  }
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    if (!need[k]) continue;
+    const int64_t i = i0 + ty + 8 * k;
+    float inter = (float)acc[k];
+    if (half_inter) inter = round_to<__half>(inter);
+    const float v = nms_iou(inter, area[base + i], area[base + j]);
+    iou[(base + j) * N + i] = v;
+    atomicMax(comp_bits + base + j, __float_as_uint(v));
+  }
+}
+
+__global__ void __launch_bounds__(SS_NT) nms_decay_kernel(const int64_t* __restrict__ label, const float* __restrict__ score,
+                                                          const int64_t* __restrict__ n_valid, int64_t B, int64_t N,
+                                                          const float* __restrict__ iou, const unsigned* __restrict__ comp_bits,
+                                                          int kernel, float nsig, float filter_thr, float* __restrict__ out) {
+  const int64_t gw = (int64_t)blockIdx.x * (SS_NT / kWarp) + (threadIdx.x >> 5);
+  const int lane = threadIdx.x & 31;
+  if (gw >= B * N) return;
+  const int64_t b = gw / N, j = gw % N, base = b * N;
+  const int64_t nv = min(n_valid[b], N);
+  if (j >= nv) {
+    if (lane == 0) out[base + j] = -INFINITY;
+    return;
+  }
+  const int64_t lj = label[base + j];
+  float m = INFINITY;
+  for (int64_t i = lane; i < nv; i += kWarp) {
+    const float comp = __uint_as_float(comp_bits[base + i]);
+    const float v = (i < j && label[base + i] == lj) ? iou[(base + j) * N + i] : 0.f;
+    m = nan_min(m, nms_decay_ratio(v, comp, kernel, nsig));
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) m = nan_min(m, __shfl_xor_sync(kFull, m, o));
+  if (lane == 0) {
+    const float s = BXS_FMUL(score[base + j], m);
+    out[base + j] = (filter_thr > 0.f && !(s >= filter_thr)) ? -INFINITY : s;
+  }
+}
+
+// interp_f32: the probabilities of a 16-bit row are interpolated and thresholded in float32 without rounding (what
+// torch.autocast does to upsample_bilinear2d); else each stage is rounded to T.
+template <typename T, bool kRound>
+__device__ __forceinline__ float stage(float v) {
+  return kRound ? to_dtype<T>(v) : v;
+}
+
+template <typename T, bool kRound>
+__global__ void __launch_bounds__(SS_NT) solo_paste_kernel(RowSources src, const int64_t* __restrict__ rows, int64_t n, int h,
+                                                           int w, int H_img, int W_img, int H_ori, int W_ori, int logits,
+                                                           float thr, uint8_t* __restrict__ out) {
+  const float t = stage<T, kRound>(thr);
+  const int64_t npix = (int64_t)H_ori * W_ori;
+  for (int64_t k = blockIdx.y; k < n; k += gridDim.y) {
+    const T* p = row_ptr<T>(src, rows[k], (int64_t)h * w);
+    uint8_t* o = out + k * npix;
+    for (int64_t pix = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; pix < npix; pix += (int64_t)gridDim.x * blockDim.x) {
+      if (!p) {
+        o[pix] = 0;
+        continue;
+      }
+      const int y = (int)(pix / W_ori), x = (int)(pix % W_ori);
+      const PasteTaps pt = paste_taps(y, x, H_img, W_img, H_ori, W_ori);
+      float v[2][2];
+#pragma unroll
+      for (int a = 0; a < 2; ++a) {
+        const RsTap ty = paste_stage1_tap(pt.y1[a], h);
+#pragma unroll
+        for (int c = 0; c < 2; ++c) {
+          const RsTap tx = paste_stage1_tap(pt.x1[c], w);
+          const T* q = p + ty.i0 * w + tx.i0;
+          v[a][c] = stage<T, kRound>(rs_lerp2(ty, tx, prob(q[0], logits), prob(q[tx.ip], logits), prob(q[ty.ip * w], logits),
+                                         prob(q[ty.ip * w + tx.ip], logits)));
+        }
+      }
+      o[pix] = stage<T, kRound>(rs_lerp2(pt.ty2, pt.tx2, v[0][0], v[0][1], v[1][0], v[1][1])) > t;
+    }
+  }
+}
+
+}  // namespace
+}  // namespace bxs
+
+using namespace bxs;
+
+extern "C" int bxs_solo_mask_stats(const void* const* src_host, const int64_t* src_rows_host, int64_t n_src, int64_t hw,
+                                   int dtype, int logits, const int64_t* rows, int64_t n_rows, float mask_thr, uint32_t* bits,
+                                   int32_t* area, float* masked_sum, bxs_stream_t stream) {
+  RowSources src;
+  if (int rc = make_sources(src, src_host, src_rows_host, n_src)) return rc;
+  if (hw <= 0 || n_rows < 0 || (dtype != 0 && dtype != 1)) return BXS_ERR_INVALID_ARG;
+  if (n_rows > INT32_MAX) return BXS_ERR_UNSUPPORTED;
+  if (n_rows == 0) return BXS_OK;
+  if (!rows || !bits || !area || !masked_sum) return BXS_ERR_INVALID_ARG;
+  const int64_t words = ceil_div(hw, kWarp);
+  auto kern = dtype == 0 ? solo_stats_kernel<float> : solo_stats_kernel<__half>;
+  kern<<<(unsigned)n_rows, SS_NT, 0, as_stream(stream)>>>(src, rows, hw, words, logits, mask_thr, bits, area, masked_sum);
+  return check_launch();
+}
+
+extern "C" int64_t bxs_matrix_nms_workspace_bytes(int64_t B, int64_t N) {
+  if (B <= 0 || N <= 0) return 0;
+  Carver c(nullptr);
+  c.take((size_t)(B * N * N) * sizeof(float));
+  c.take((size_t)(B * N) * sizeof(unsigned));
+  return (int64_t)c.off;
+}
+
+extern "C" int bxs_matrix_nms(const uint32_t* bits, int64_t words, const int64_t* row, const int64_t* label, const float* area,
+                              const float* score, const int64_t* n_valid, int64_t B, int64_t N, int kernel, float sigma,
+                              float filter_thr, int half_inter, void* workspace, float* out_score, bxs_stream_t stream) {
+  if (B < 0 || N < 0 || words <= 0 || (kernel != kNmsGaussian && kernel != kNmsLinear)) return BXS_ERR_INVALID_ARG;
+  if (B == 0 || N == 0) return BXS_OK;
+  if (!bits || !row || !label || !area || !score || !n_valid || !workspace || !out_score) return BXS_ERR_INVALID_ARG;
+  if (B > 65535 || ceil_div(N, NMS_TILE) > 65535 || B * N > INT32_MAX) return BXS_ERR_UNSUPPORTED;
+  Carver c(workspace);
+  float* iou = reinterpret_cast<float*>(c.take((size_t)(B * N * N) * sizeof(float)));
+  unsigned* comp = reinterpret_cast<unsigned*>(c.take((size_t)(B * N) * sizeof(unsigned)));
+  cudaStream_t s = as_stream(stream);
+  if (cudaMemsetAsync(comp, 0, (size_t)(B * N) * sizeof(unsigned), s) != cudaSuccess) return check_launch();
+  const unsigned tiles = (unsigned)ceil_div(N, NMS_TILE);
+  nms_inter_kernel<<<dim3(tiles, tiles, (unsigned)B), SS_NT, 0, s>>>(bits, words, row, label, area, n_valid, N, half_inter, iou,
+                                                                     comp);
+  if (int rc = check_launch()) return rc;
+  const float nsig = -1.f * sigma;
+  nms_decay_kernel<<<(unsigned)ceil_div(B * N, SS_NT / kWarp), SS_NT, 0, s>>>(label, score, n_valid, B, N, iou, comp, kernel,
+                                                                              nsig, filter_thr, out_score);
+  return check_launch();
+}
+
+extern "C" int bxs_solo_paste_masks(const void* const* src_host, const int64_t* src_rows_host, int64_t n_src, int64_t h,
+                                    int64_t w, int dtype, int logits, int interp_f32, const int64_t* rows, int64_t n,
+                                    int64_t H_img, int64_t W_img, int64_t H_ori, int64_t W_ori, float mask_thr,
+                                    uint8_t* out, bxs_stream_t stream) {
+  RowSources src;
+  if (int rc = make_sources(src, src_host, src_rows_host, n_src)) return rc;
+  if (h <= 0 || w <= 0 || n < 0 || H_img <= 0 || W_img <= 0 || H_ori <= 0 || W_ori <= 0 || (dtype != 0 && dtype != 1))
+    return BXS_ERR_INVALID_ARG;
+  if (H_img > 4 * h || W_img > 4 * w) return BXS_ERR_INVALID_ARG;          // the crop lies inside the (4h, 4w) plane
+  if (4 * h > INT32_MAX || 4 * w > INT32_MAX || H_ori * W_ori > INT32_MAX || h * w > INT32_MAX) return BXS_ERR_UNSUPPORTED;
+  if (n == 0) return BXS_OK;
+  if (!rows || !out) return BXS_ERR_INVALID_ARG;
+  const int64_t npix = H_ori * W_ori;
+  const unsigned gx = (unsigned)std::min<int64_t>(ceil_div(npix, SS_NT), 1024);
+  const unsigned gy = (unsigned)std::min<int64_t>(n, 65535);
+  auto kern = dtype == 0 ? solo_paste_kernel<float, false>
+                         : (interp_f32 ? solo_paste_kernel<__half, false> : solo_paste_kernel<__half, true>);
+  kern<<<dim3(gx, gy), SS_NT, 0, as_stream(stream)>>>(src, rows, n, (int)h, (int)w, (int)H_img, (int)W_img, (int)H_ori,
+                                                      (int)W_ori, logits, mask_thr, out);
+  return check_launch();
+}

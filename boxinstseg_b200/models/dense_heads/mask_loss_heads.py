@@ -7,8 +7,9 @@ dynamic-conv call sites (a2-a4), on the kernels of libboxseg_b200:
 
 The mask-loss hot path and its immediate callers are implemented here: the SOLO target builders live in
 ``solo_targets.py`` / ``disco_targets.py`` (f2), the Hungarian front half in ``core/assigner.py`` (f1), DiscoBox's
-cross-image correspondence loss in ``disco_corr.py`` (f4; ``DiscoBoxSOLOv2Head.corr_inputs / corr_loss``).  The conv towers,
-category losses and inference are out of scope (SURVEY 2.1 row 3): the classes keep the reference's registry names and accept (and store) the reference's constructor kwargs so
+cross-image correspondence loss in ``disco_corr.py`` (f4; ``DiscoBoxSOLOv2Head.corr_inputs / corr_loss``).  The conv towers
+and category losses are out of scope (SURVEY 2.1 row 3); SOLOv2 inference (``get_seg`` of the two SOLOv2 heads) is in
+``solo_seg.py``.  The classes keep the reference's registry names and accept (and store) the reference's constructor kwargs so
 the configs build, and expose the hot-path pieces as methods with the tensors the reference passes between
 its own lines.
 """
@@ -222,6 +223,17 @@ class BoxSOLOv2Head(nn.Module):
         out = self.mask_loss(rows, ins_labels, [resized[s][0] for s in sizes], [resized[s][1] for s in sizes],
                              inst_imgs=inst_imgs)
         return dict(loss_boxpro=out['loss_boxpro'], loss_levelset=out['loss_levelset'], loss_cate=loss_cate)
+
+    # box_solov2_head.py:475-590, the reference's signature
+    def get_seg(self, seg_preds, cate_preds, levelset_feats, img_metas, cfg, rescale=None):
+        """Per image the reference's ``InstanceData`` (mmdet's when importable, else a namespace of the ``img_meta`` fields)
+        with ``masks`` bool [n, H_ori, W_ori], ``labels`` int64 and ``scores``: ``seg_preds`` / ``cate_preds`` as
+        ``forward(eval=True)`` returns them, every image of the batch at once (``solo_seg.box_solov2_get_seg``: each
+        distinct candidate row read in place once, Matrix NMS and the mask paste on the GPU, two host reads per call).  Where
+        Matrix NMS keeps nothing the reference raises (``F.interpolate`` of an empty batch); this returns ``empty_results``."""
+        from .solo_seg import box_solov2_get_seg
+        with torch.no_grad():
+            return box_solov2_get_seg(seg_preds, cate_preds, self.strides, img_metas, cfg)
 
     @staticmethod
     def _box_mask_rows(per_img, lv, loc, S, size, gt_label_list, dev):
@@ -517,6 +529,17 @@ class DiscoBoxSOLOv2Head(nn.Module):
         num_ins = torch.stack([per_img[b][2][lv].sum() for b in range(B) for lv in range(n_lv)]).sum()
         loss_cate = sigmoid_focal_loss_levels(cate_preds, cate_labels, num_ins + 1, *self.focal)
         return dict(loss_ins=loss_ins, loss_ts=loss_ts, loss_cate=loss_cate, loss_corr=loss_corr)
+
+    # discobox_head.py:1531-1660, the reference's signature
+    def get_seg(self, cate_preds, kernel_preds, seg_pred, img_metas, cfg, rescale=None, img=None):
+        """Per image the reference's ``InstanceData`` with ``masks`` bool [n, H_ori, W_ori], ``labels`` int64 and ``scores``,
+        every image of the batch at once under float16 autocast, as the reference's ``@autocast()`` get_seg_single runs:
+        each distinct candidate cell of ``kernel_preds`` is convolved with ``seg_pred`` once (``bxs_disco_cells_pack`` +
+        ``dynconv1x1``), then the statistics, Matrix NMS and the mask paste on the GPU, two host reads per call
+        (``solo_seg.discobox_get_seg``)."""
+        from .solo_seg import discobox_get_seg
+        with torch.no_grad():
+            return discobox_get_seg(cate_preds, kernel_preds, seg_pred, self._grid_cfg()[1], img_metas, cfg)
 
     # a3 -- discobox_head.py:1206-1246
     @staticmethod

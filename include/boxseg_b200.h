@@ -694,6 +694,44 @@ int bxs_fcos_loss_forward(const float* const* pred_host, const float* const* ctr
 int bxs_fcos_loss_backward(float* g_pred, int64_t n_pred, const float* g_loss_bbox, float* g_ctr, int64_t n_ctr,
                            const float* g_loss_ctr, bxs_stream_t stream);
 
+/* ---------------------------------------------------------------------------------------
+ * SOLOv2 inference    replaces the body of get_seg_single of BoxSOLOv2Head (box_solov2_head.py:503-590) and
+ *     DiscoBoxSOLOv2Head (discobox_head.py:1559-1660): thresholding, mask areas and scores, mask_matrix_nms
+ *     (mmdet/core/post_processing/matrix_nms.py:5-121) and the two F.interpolate passes of the mask paste.
+ * Rows: src_host[s] (n_src <= 8, a HOST array of device pointers) holds src_rows_host[s] rows of hw (h*w) elements of `dtype`
+ *   (0 float32, 1 float16), dense; a row id indexes the concatenation of the sources (BoxSOLOv2: the levels' [B*S_l^2, h, w]
+ *   probabilities of forward(eval=True) as they lie; DiscoBox: its candidate convolution).  logits != 0: an element is a logit
+ *   and p = sigmoid(x) as torch computes it for that dtype; else p is the element.  A row id outside the sources reads as
+ *   an all-zero row.  mask_thr is rounded to `dtype` first: torch compares a tensor with a Python float in the tensor's dtype.
+ * bxs_solo_mask_stats: for each of n_rows ids in rows i64 -> bits u32 [n_rows, ceil(hw/32)] (bit k of word w: p[32w+k] >
+ *   mask_thr), area i32 [n_rows] (its popcount), masked_sum f32 [n_rows] = sum of p over the set bits (accumulated in float64
+ *   in a fixed order, rounded once).  One CTA per row.
+ * bxs_matrix_nms: for B images of N candidate slots each, sorted by score (descending; the first min(n_valid[b], N) slots are
+ *   the valid ones): row i64 [B,N] (the slot's row of bits), label i64 [B,N], area f32 [B,N], score f32 [B,N], n_valid i64
+ *   [B] on the device -> out_score f32 [B,N] = score * decay coefficient (kernel 0 gaussian with sigma, 1 linear; the
+ *   reference's lines in its operation order), -inf for an invalid slot or, with filter_thr > 0, a score below filter_thr.
+ *   half_inter != 0 rounds each intersection count to float16 once (the reference's torch.mm under autocast).
+ *   workspace: bxs_matrix_nms_workspace_bytes(B, N) bytes (B*N*N IoUs and B*N column maxima).  Two launches and a memset.
+ * bxs_solo_paste_masks: for n row ids -> out u8 [n, H_ori, W_ori] (the bytes of a torch.bool tensor) =
+ *   interpolate(interpolate(p, (4h, 4w))[:H_img, :W_img], (H_ori, W_ori)) > mask_thr, bilinear with align_corners=False in
+ *   the arithmetic of bxs_bilinear_resize_forward; a float16 row is rounded to float16 after each stage and compared in
+ *   float16, as ATen computes on a float16 tensor, or with interp_f32 != 0 interpolated and compared in float32 without
+ *   rounding (torch.autocast runs upsample_bilinear2d in float32).  H_img <= 4h, W_img <= 4w.
+ * No host synchronisation, deterministic.  BXS_ERR_INVALID_ARG: a NULL pointer the call needs, a negative count, a
+ * non-positive size, an unknown dtype or kernel.  BXS_ERR_UNSUPPORTED: n_src > 8, more than INT32_MAX rows or pixels per
+ * plane, more than 65535 images or 65535 * 32 slots.  All checks run before any device call.
+ * --------------------------------------------------------------------------------------- */
+int bxs_solo_mask_stats(const void* const* src_host, const int64_t* src_rows_host, int64_t n_src, int64_t hw, int dtype,
+                        int logits, const int64_t* rows, int64_t n_rows, float mask_thr, uint32_t* bits, int32_t* area,
+                        float* masked_sum, bxs_stream_t stream);
+int64_t bxs_matrix_nms_workspace_bytes(int64_t B, int64_t N);
+int bxs_matrix_nms(const uint32_t* bits, int64_t words, const int64_t* row, const int64_t* label, const float* area,
+                   const float* score, const int64_t* n_valid, int64_t B, int64_t N, int kernel, float sigma, float filter_thr,
+                   int half_inter, void* workspace, float* out_score, bxs_stream_t stream);
+int bxs_solo_paste_masks(const void* const* src_host, const int64_t* src_rows_host, int64_t n_src, int64_t h, int64_t w,
+                         int dtype, int logits, int interp_f32, const int64_t* rows, int64_t n, int64_t H_img, int64_t W_img,
+                         int64_t H_ori, int64_t W_ori, float mask_thr, uint8_t* out, bxs_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
