@@ -112,6 +112,12 @@ SIGNATURES = {
     'bxs_matrix_nms_workspace_bytes': [c_i64, c_i64],
     'bxs_matrix_nms': [c_p, c_i64] + [c_p] * 5 + [c_i64, c_i64, c_int, c_f, c_f, c_int, c_p, c_p, c_p],
     'bxs_solo_paste_masks': [c_p, c_p, c_i64, c_i64, c_i64, c_int, c_int, c_int, c_p] + [c_i64] * 5 + [c_f, c_p, c_p],
+    'bxs_condinst_point_scores': [c_p] * 6 + [c_i64] * 4 + [c_p, c_p],
+    'bxs_condinst_decode': [c_p] * 10 + [c_i64] * 3 + [c_p, c_i64, c_p, c_p, c_f] + [c_p] * 7,
+    'bxs_condinst_gather': [c_p] * 6 + [c_i64] * 3 + [c_p, c_p, c_i64] + [c_p] * 4,
+    'bxs_box_nms_workspace_bytes': [c_p, c_i64],
+    'bxs_box_nms': [c_p] * 3 + [c_i64] * 3 + [c_f, c_p, c_p, c_p],
+    'bxs_condinst_paste_masks': [c_p] + [c_i64] * 8 + [c_int, c_p, c_p],
 }
 _RESTYPE = {'bxs_mst_workspace_bytes': c_i64, 'bxs_bfs_workspace_bytes': c_i64, 'bxs_refine_scratch_bytes': c_i64, 'bxs_lcm_workspace_bytes': c_i64, 'bxs_meanfield_workspace_bytes': c_i64, 'bxs_projection_workspace_bytes': c_i64,'bxs_condinst_head_workspace_bytes': c_i64, 'bxs_last_error': ctypes.c_char_p, 'bxs_boxinst_loss_workspace_bytes': c_i64,
              'bxs_boxinst_loss_fused_workspace_bytes': c_i64, 'bxs_boxinst_loss_fused_sched_bytes': c_i64,
@@ -123,7 +129,7 @@ _RESTYPE = {'bxs_mst_workspace_bytes': c_i64, 'bxs_bfs_workspace_bytes': c_i64, 
              'bxs_sigmoid_focal_loss_levels_forward_workspace_bytes': c_i64,
              'bxs_softmax_cross_entropy_layers_forward_workspace_bytes': c_i64,
              'bxs_sigmoid_focal_loss_cells_forward_workspace_bytes': c_i64, 'bxs_fcos_loss_workspace_bytes': c_i64,
-             'bxs_matrix_nms_workspace_bytes': c_i64}
+             'bxs_matrix_nms_workspace_bytes': c_i64, 'bxs_box_nms_workspace_bytes': c_i64}
 
 _STATUS = {-1: 'invalid argument', -2: 'kernel launch failed', -3: 'unsupported shape', -4: 'no CUDA device'}
 

@@ -15,7 +15,7 @@ and the GIoU + centerness losses (``bxs_fcos_loss_forward``).  Nothing is read b
 backward can be captured in a CUDA graph.
 
 Registered as a *partial* head: with mmdet importable the registered class inherits everything else (layers, forward,
-get_bboxes) from the reference's own ``CondInstBoxHead``.
+simple_test) from the reference's own ``CondInstBoxHead``; ``get_bboxes`` runs on csrc/condinst_infer.cu (condinst_infer.py).
 """
 import ctypes
 
@@ -131,7 +131,7 @@ class CondInstBoxHead:
     def __init__(self, num_classes, in_channels=256, regress_ranges=((-1, 64), (64, 128), (128, 256), (256, 512), (512, INF)),
                  strides=(8, 16, 32, 64, 128), center_sampling=True, center_sample_radius=1.5, norm_on_bbox=True,
                  loss_cls=_DEFAULT_LOSS_CLS, loss_bbox=_DEFAULT_LOSS_BBOX, loss_centerness=_DEFAULT_LOSS_CENTERNESS,
-                 **kwargs):
+                 test_cfg=None, **kwargs):
         self.num_classes = num_classes
         self.in_channels = in_channels
         self.regress_ranges = regress_ranges
@@ -140,6 +140,7 @@ class CondInstBoxHead:
         self.center_sample_radius = center_sample_radius
         self.norm_on_bbox = norm_on_bbox
         self.loss_cls, self.loss_bbox, self.loss_centerness = dict(loss_cls), dict(loss_bbox), dict(loss_centerness)
+        self.test_cfg = test_cfg
         self._bxs_post_init()
 
     def _bxs_post_init(self):
@@ -185,3 +186,13 @@ class CondInstBoxHead:
         flatten_level_inds = torch.cat([torch.full((B * h * w,), i, device=dev).long() for i, (h, w) in enumerate(sizes)])
         losses = dict(loss_cls=loss_cls, loss_bbox=loss_bbox, loss_centerness=loss_centerness)
         return losses, flatten_points, flatten_level_inds, flatten_img_inds, torch.cat(gt_inds)
+
+    def get_bboxes(self, cls_scores, bbox_preds, centernesses, param_preds, img_metas, cfg=None, rescale=False, with_nms=True):
+        """condinst_head.py:640-853, same arguments and return value: per image (det_bboxes [n,5], det_labels int64,
+        det_params [n,P], det_coors [n,2], det_level_inds int64), or with ``with_nms=False`` the reference's 6-tuple of
+        every kept point.  ``cfg=None`` means ``self.test_cfg``.  Every image at once on the kernels of
+        csrc/condinst_infer.cu (``condinst_infer.get_bboxes``), with two host reads per call; equal top-k keys keep the
+        lower point and equal scores the candidate order (INTEGRATION.md section 11)."""
+        from .condinst_infer import get_bboxes
+        return get_bboxes(cls_scores, bbox_preds, centernesses, param_preds, img_metas,
+                          self.test_cfg if cfg is None else cfg, self.strides, rescale, with_nms)

@@ -120,6 +120,15 @@ class CondInstMaskHead(nn.Module):
             sel = torch.arange(P, device=params.device)
         return params[sel], coors[sel], level_inds[sel], img_inds[sel], gt_inds[sel]
 
+    def simple_test(self, mask_feat, det_labels, det_params, det_coors, det_level_inds, img_metas, num_classes,
+                    rescale=False):
+        """condinst_head.py:1234-1286, same arguments and return value (per image, per class, uint8 numpy masks): the
+        dynamic head once for the batch and the fused paste ``ops.condinst.paste_masks`` per image.  An image without a
+        detection in a batch with some gets one entry of empty class lists (INTEGRATION.md section 11)."""
+        from .condinst_infer import simple_test
+        return simple_test(self, mask_feat, det_labels, det_params, det_coors, det_level_inds, img_metas, num_classes,
+                           rescale)
+
     # ------------------------------------------------------------------ a5
     def get_targets(self, gt_bboxes, gt_masks, img, img_metas):
         """BoxInst: returns a BoxInstTargets (per-image similarity bits + per-GT rectangles) instead of

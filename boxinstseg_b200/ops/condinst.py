@@ -57,3 +57,19 @@ def dynamic_mask_head(feat, params, coors, level_inds, img_inds, sizes_of_intere
     coors = coors.to(device=dev, dtype=torch.float32).contiguous() if rel_coors else None
     img32 = img_inds.to(device=dev, dtype=torch.int32).contiguous()
     return _DynamicMaskHead.apply(feat, params, coors, soi, img32, in_stride, in_stride // out_stride, rel_coors)
+
+
+def paste_masks(mask_logits, factor, img_shape, ori_shape=None):
+    """The mask lines of CondInstMaskHead.simple_test (condinst_head.py:1261-1281) in one pass: mask_logits [n,1,h,w] ->
+    bool [n, H, W] = aligned_bilinear(sigmoid(mask_logits), factor)[:, :, :H_img, :W_img] > 0.5, resized bilinearly
+    (align_corners=False) to ``ori_shape[:2]`` before the threshold when ``ori_shape`` is given (``rescale=True``)."""
+    n, _, h, w = mask_logits.shape
+    logits = mask_logits.detach().float().contiguous()
+    L.require_cuda(logits)
+    H_img, W_img = [int(v) for v in img_shape[:2]]
+    H, W = [int(v) for v in ori_shape[:2]] if ori_shape is not None else (H_img, W_img)
+    out = torch.empty((n, H, W), dtype=torch.bool, device=logits.device)
+    with torch.cuda.device(logits.device):
+        L.check(L.lib().bxs_condinst_paste_masks(L.ptr(logits), n, h, w, int(factor), H_img, W_img, H, W,
+                                                 int(ori_shape is not None), L.ptr(out), L.stream()), 'condinst_paste_masks')
+    return out

@@ -732,6 +732,56 @@ int bxs_solo_paste_masks(const void* const* src_host, const int64_t* src_rows_ho
                          int dtype, int logits, int interp_f32, const int64_t* rows, int64_t n, int64_t H_img, int64_t W_img,
                          int64_t H_ori, int64_t W_ori, float mask_thr, uint8_t* out, bxs_stream_t stream);
 
+/* ---------------------------------------------------------------------------------------
+ * CondInst inference   replaces the level loop of CondInstBoxHead._get_bboxes (condinst_head.py:762-813), the NMS of
+ *     nms_with_others (:18-83: mmcv's batched_nms with type 'nms') and the mask lines of CondInstMaskHead.simple_test
+ *     (:1261-1281: sigmoid, aligned_bilinear, crop, F.interpolate, > 0.5).
+ * Level table: for each of n_levels <= 8 levels, cls_host[l] / ctr_host[l] / bbox_host[l] / param_host[l] (HOST arrays of
+ *   device pointers) are float32 [B,C,H,W] / [B,1,H,W] / [B,4,H,W] / [B,P,H,W] read in place with the element strides
+ *   *_strides_host[4l .. 4l+3] (any layout); height_host / width_host / stride_host give H_l, W_l and the level's stride.
+ *   k_host[l] is the number of points the level keeps (H_l*W_l: all, in point order; less: the first k_host[l] of the
+ *   level's row of `order`).  The slots of an image are the kept points, level after level: S = sum k_host.  B <= 32.
+ * bxs_condinst_point_scores -> key f32 [B, n_levels, P_max] = max_c sigmoid(cls_c) * sigmoid(ctr) (a NaN wins), -inf past
+ *   H_l*W_l.  P_max >= every H_l*W_l.
+ * bxs_condinst_decode: order i64 [B, n_levels, P_max] (the per-level ranking of the keys; may be NULL when no level is cut),
+ *   img_hw_host f32 [B,2] (img_shape[:2]), scale_host f32 [B,4] (scale_factor, or NULL: no rescale) -> for each slot g of
+ *   [B,S]: box f32 [B,S,4] (distance2bbox with the per-image clamp, then / scale_factor), ctr f32 [B,S] = sigmoid(ctr),
+ *   point i64 [B,S] (y*W_l + x), and per class cand u8 [B,S,C] = sigmoid(cls) > score_thr, score f32 [B,S,C] =
+ *   sigmoid(cls) * sigmoid(ctr), sig f32 [B,S,C] = sigmoid(cls) (optional).
+ * bxs_condinst_gather: for n slot ids rows i64 (b*S + s) -> params f32 [n,P], coors f32 [n,2] (the point), level i64 [n].
+ * bxs_box_nms: N boxes f32 [N,4] (16-byte aligned; batched_nms's offset boxes) sorted into n_seg segments, segment s being
+ *   the rows seg_start[s] .. seg_start[s+1]-1 (i64 [n_seg+1] on the device) in descending score order; mask_off i64 [n_seg]
+ *   = the exclusive prefix sum of n_s * ceil(n_s / 64); max_seg >= every n_s -> keep u8 [N]: greedy NMS within every
+ *   segment with mmcv's test interS > iou_thr * (Sa + Sb - interS).  workspace: bxs_box_nms_workspace_bytes(n_s host
+ *   array, n_seg) bytes, 8-byte aligned.  Two launches.
+ * bxs_condinst_paste_masks: logits f32 [n, h, w] (dense) -> out u8 [n, H_out, W_out] (the bytes of a torch.bool tensor) =
+ *   aligned_bilinear(sigmoid(logits), factor)[:H_img, :W_img] > 0.5, or with rescale != 0 that crop resized to
+ *   (H_out, W_out) (bilinear, align_corners=False) first; in the arithmetic of bxs_bilinear_resize_forward.  H_img <=
+ *   factor*h, W_img <= factor*w; without rescale (H_out, W_out) == (H_img, W_img).
+ * No host synchronisation, no atomics: deterministic.  BXS_ERR_INVALID_ARG: a NULL pointer the call needs, a negative count,
+ *   a non-positive size, k_host[l] outside [0, H_l*W_l], P_max below a level's size.  BXS_ERR_UNSUPPORTED: more than 8
+ *   levels or 32 images, more than INT32_MAX points per level or pixels per plane, a segment of more than 393216 boxes.
+ *   All checks run before any device call.
+ * --------------------------------------------------------------------------------------- */
+int bxs_condinst_point_scores(const float* const* cls_host, const int64_t* cls_strides_host, const float* const* ctr_host,
+                              const int64_t* ctr_strides_host, const int64_t* height_host, const int64_t* width_host,
+                              int64_t n_levels, int64_t B, int64_t C, int64_t P_max, float* key, bxs_stream_t stream);
+int bxs_condinst_decode(const float* const* cls_host, const int64_t* cls_strides_host, const float* const* ctr_host,
+                        const int64_t* ctr_strides_host, const float* const* bbox_host, const int64_t* bbox_strides_host,
+                        const int64_t* height_host, const int64_t* width_host, const float* stride_host, const int64_t* k_host,
+                        int64_t n_levels, int64_t B, int64_t C, const int64_t* order, int64_t P_max, const float* img_hw_host,
+                        const float* scale_host, float score_thr, float* box, float* ctr, int64_t* point, uint8_t* cand,
+                        float* score, float* sig, bxs_stream_t stream);
+int bxs_condinst_gather(const float* const* param_host, const int64_t* param_strides_host, const int64_t* height_host,
+                        const int64_t* width_host, const float* stride_host, const int64_t* k_host, int64_t n_levels, int64_t B,
+                        int64_t P, const int64_t* point, const int64_t* rows, int64_t n, float* params, float* coors,
+                        int64_t* level, bxs_stream_t stream);
+int64_t bxs_box_nms_workspace_bytes(const int64_t* seg_count_host, int64_t n_seg);
+int bxs_box_nms(const float* boxes, const int64_t* seg_start, const int64_t* mask_off, int64_t N, int64_t n_seg, int64_t max_seg,
+                float iou_thr, void* workspace, uint8_t* keep, bxs_stream_t stream);
+int bxs_condinst_paste_masks(const float* logits, int64_t n, int64_t h, int64_t w, int64_t factor, int64_t H_img, int64_t W_img,
+                             int64_t H_out, int64_t W_out, int rescale, uint8_t* out, bxs_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
