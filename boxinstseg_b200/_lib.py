@@ -5,11 +5,13 @@ exception is raised.  Build with ``python -m boxinstseg_b200.build`` (or ``__gra
 """
 import ctypes
 import os
+import re
 
 import torch
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get('BXS_LIB_PATH') or os.path.join(_HERE, 'lib', 'libboxseg_b200.so')   # BXS_LIB_PATH: A/B builds (tools/)
+HEADER_PATH = os.path.join(os.path.dirname(_HERE), 'include', 'boxseg_b200.h')
 
 _lib = None
 
@@ -18,118 +20,41 @@ c_i64 = ctypes.c_int64
 c_int = ctypes.c_int
 c_f = ctypes.c_float
 
-# name -> argtypes (all return int unless listed in _RESTYPE)
-SIGNATURES = {
-    'bxs_version': [],
-    'bxs_last_error': [],
-    'bxs_device_sm_count': [],
-    'bxs_pairwise_nlog_forward': [c_p, c_p, c_i64, c_i64, c_i64, c_int, c_int, c_int, c_p],
-    'bxs_pairwise_nlog_backward': [c_p, c_p, c_p, c_i64, c_i64, c_i64, c_int, c_int, c_int, c_p],
-    'bxs_boxinst_bitmasks': [c_p, c_p, c_i64, c_i64, c_i64, c_p],
-    'bxs_boxinst_targets_forward': [c_p] * 13 + [c_i64] * 3 + [c_int] * 3 + [c_f, c_p],
-    'bxs_rgb_u8_to_lab': [c_p, c_p, c_i64, c_p],
-    'bxs_boxinst_loss_workspace_bytes': [c_i64, c_i64, c_i64],
-    'bxs_boxinst_loss_forward': [c_p, c_p, c_p, c_p, c_p, c_p, c_f, c_p, c_p, c_i64, c_i64, c_i64, c_int, c_p],
-    'bxs_boxinst_loss_backward': [c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_i64, c_i64, c_i64, c_int, c_p],
-    'bxs_boxinst_loss_fused_supported': [c_i64, c_i64, c_i64, c_int],
-    'bxs_boxinst_loss_fused_workspace_bytes': [c_i64, c_i64, c_i64],
-    'bxs_boxinst_loss_fused_sched_bytes': [],
-    'bxs_boxinst_loss_fused_forward': [c_p] * 6 + [c_f] + [c_p] * 4 + [c_i64] * 3 + [c_int, c_p],
-    'bxs_boxinst_loss_fused_backward': [c_p] * 4 + [c_i64] * 3 + [c_p],
-    'bxs_boxinst_loss_plan_bytes': [c_i64, c_i64, c_i64, c_int],
-    'bxs_boxinst_loss_plan': [c_p] * 5 + [c_i64] * 3 + [c_int, c_p],
-    'bxs_boxinst_loss_fused_forward_planned': [c_p] * 4 + [c_f] + [c_p] * 4 + [c_i64] * 3 + [c_int, c_p],
-    'bxs_condinst_head_forward': [c_p] * 6 + [c_i64] * 6 + [c_int] * 3 + [c_p],
-    'bxs_condinst_head_workspace_bytes': [c_i64] * 5,
-    'bxs_condinst_head_backward': [c_p] * 9 + [c_i64] * 6 + [c_int] * 3 + [c_p],
-    'bxs_projection_workspace_bytes': [c_i64] * 3,
-    'bxs_projection_loss_forward': [c_p] * 4 + [c_i64] * 3 + [c_f, c_f, c_p],
-    'bxs_projection_loss_backward': [c_p] * 3 + [c_i64] * 3 + [c_p],
-    'bxs_length_reg_forward': [c_p] * 3 + [c_i64] * 4 + [c_p],
-    'bxs_length_reg_backward': [c_p] * 3 + [c_i64] * 4 + [c_p],
-    'bxs_lcm_workspace_bytes': [c_i64] * 3,
-    'bxs_lcm_forward': [c_p] * 5 + [c_i64] * 4 + [c_int, c_int, c_p],
-    'bxs_lcm_backward': [c_p] * 5 + [c_i64] * 3 + [c_int, c_int, c_p],
-    'bxs_meanfield_kernel': [c_p, c_p] + [c_i64] * 4 + [c_int, c_f, c_f, c_f, c_p],
-    'bxs_meanfield_workspace_bytes': [c_i64] * 3,
-    'bxs_meanfield_forward_inter': [c_p] * 5 + [c_f] + [c_p] * 4 + [c_i64] * 3 + [c_int, c_int, c_p],
-    'bxs_meanfield_forward_logits': [c_p] * 5 + [c_int] + [c_p] * 3 + [c_i64] * 3 + [c_int, c_int, c_p],
-    'bxs_discobox_loss_workspace_bytes': [c_i64] * 3,
-    'bxs_discobox_loss_forward': [c_p] * 3 + [c_int] + [c_p] * 2 + [c_i64] * 3 + [c_p],
-    'bxs_discobox_loss_backward': [c_p] * 3 + [c_int] + [c_p] * 3 + [c_i64] * 3 + [c_p],
-    'bxs_mst_workspace_bytes': [c_i64] * 3,
-    'bxs_mst_forward': [c_p] * 4 + [c_i64] * 3 + [c_p],
-    'bxs_bfs_workspace_bytes': [c_i64] * 2,
-    'bxs_bfs_forward_rooted': [c_p] * 7 + [c_i64] * 2 + [c_int, c_i64, c_p],
-    'bxs_refine_scratch_bytes': [c_i64] * 3,
-    'bxs_refine_forward_grouped': [c_p] * 14 + [c_i64] * 4 + [c_p],
-    'bxs_refine_backward_feature_grouped': [c_p] * 11 + [c_i64] * 4 + [c_p],
-    'bxs_refine_backward_weight_grouped': [c_p] * 15 + [c_i64] * 4 + [c_p],
-    'bxs_dynconv1x1_forward': [c_p] * 3 + [c_i64] * 4 + [c_p],
-    'bxs_dynconv1x1_backward_workspace_bytes': [c_i64] * 4,
-    'bxs_dynconv1x1_backward': [c_p] * 6 + [c_i64] * 4 + [c_p],
-    'bxs_dynconv1x1_cells_forward_workspace_bytes': [c_p] + [c_i64] * 3,
-    'bxs_dynconv1x1_cells_forward': [c_p] * 9 + [c_i64] * 4 + [c_p],
-    'bxs_dynconv1x1_cells_backward_workspace_bytes': [c_p] * 4 + [c_i64] * 4,
-    'bxs_dynconv1x1_cells_backward': [c_p] * 11 + [c_i64] * 4 + [c_p],
-    'bxs_disco_cells_pack': [c_p] * 4 + [c_i64] + [c_p] * 2 + [c_i64] * 4 + [c_int, c_p],
-    'bxs_disco_cells_unpack_grad': [c_p] * 4 + [c_i64] + [c_p] + [c_i64] * 4 + [c_int, c_p],
-    'bxs_dynconv1x1_half_forward':[c_p] * 3 + [c_i64] * 4 + [c_int, c_p],
-    'bxs_dynconv1x1_half_backward_workspace_bytes': [c_i64] * 4 + [c_int],
-    'bxs_dynconv1x1_half_backward': [c_p] * 6 + [c_i64] * 4 + [c_int, c_p],
-    'bxs_upsampled_rowcol_max': [c_p] * 4 + [c_i64] * 5 + [c_int, c_p],
-    'bxs_bilinear_resize_forward': [c_p, c_p] + [c_i64] * 5 + [c_int, c_p],
-    'bxs_bilinear_resize_backward': [c_p, c_p] + [c_i64] * 5 + [c_int, c_p],
-    'bxs_box2mask_attn_mask': [c_p, c_p] + [c_i64] * 7 + [c_int, c_int, c_p],
-    'bxs_tree_edge_weight_forward': [c_p] * 4 + [c_i64] * 4 + [c_f, c_p],
-    'bxs_tree_edge_weight_backward': [c_p] * 7 + [c_i64] * 4 + [c_f, c_p],
-    'bxs_levelset_fused_workspace_bytes': [c_i64],
-    'bxs_levelset_fused_forward': [c_p] * 6 + [c_i64] * 4 + [c_f, c_int, c_p],
-    'bxs_levelset_fused_backward': [c_p] * 7 + [c_i64] * 4 + [c_f, c_int, c_p],
-    'bxs_corr_solve': [c_p, c_p] + [c_i64] * 3 + [c_int] * 3 + [c_p],
-    'bxs_corr_solve_batched': [c_p] * 3 + [c_i64] * 4 + [c_int] * 3 + [c_p],
-    'bxs_corr_transfer_workspace_bytes': [c_i64] * 3,
-    'bxs_corr_transfer': [c_p] * 7 + [c_i64] * 5 + [c_p],
-    'bxs_corr_transfer_batched': [c_p] * 8 + [c_i64] * 6 + [c_p],
-    'bxs_corr_retrieve': [c_p] * 19 + [c_i64] * 8 + [c_f] * 6 + [c_int] * 2 + [c_p],
-    'bxs_corr_paste': [c_p] * 5 + [c_i64] * 5 + [c_p],
-    'bxs_corr_bank_append': [c_p] * 12 + [c_i64] * 5 + [c_p],
-    'bxs_fcos_targets': [c_p] * 7 + [c_i64] * 2 + [c_p] * 5 + [c_int, c_int, c_i64, c_p],
-    'bxs_lsap_workspace_bytes': [c_p, c_p, c_i64],
-    'bxs_lsap_solve': [c_p] * 4 + [c_i64, c_int] + [c_p] * 4,
-    'bxs_sigmoid_focal_loss_levels_forward_workspace_bytes': [c_p, c_i64, c_i64],
-    'bxs_sigmoid_focal_loss_levels_forward': [c_p] * 7 + [c_i64] * 3 + [c_f] * 3 + [c_p],
-    'bxs_sigmoid_focal_loss_cells_forward_workspace_bytes': [c_p, c_i64, c_i64],
-    'bxs_sigmoid_focal_loss_cells_forward': [c_p] * 7 + [c_i64] * 3 + [c_f] * 3 + [c_p],
-    'bxs_softmax_cross_entropy_layers_forward_workspace_bytes': [c_i64] * 3,
-    'bxs_softmax_cross_entropy_layers_forward': [c_p] * 6 + [c_i64] * 4 + [c_f, c_p],
-    'bxs_softmax_cross_entropy_layers_backward': [c_p] * 2 + [c_i64] * 4 + [c_p],
-    'bxs_fcos_loss_workspace_bytes': [c_p, c_p, c_i64, c_i64],
-    'bxs_fcos_loss_stats': [c_p] * 7 + [c_i64] * 3 + [c_p],
-    'bxs_fcos_loss_forward': [c_p] * 13 + [c_i64] * 3 + [c_f, c_f, c_p],
-    'bxs_fcos_loss_backward': [c_p, c_i64, c_p, c_p, c_i64, c_p, c_p],
-    'bxs_solo_mask_stats': [c_p, c_p, c_i64, c_i64, c_int, c_int, c_p, c_i64, c_f, c_p, c_p, c_p, c_p],
-    'bxs_matrix_nms_workspace_bytes': [c_i64, c_i64],
-    'bxs_matrix_nms': [c_p, c_i64] + [c_p] * 5 + [c_i64, c_i64, c_int, c_f, c_f, c_int, c_p, c_p, c_p],
-    'bxs_solo_paste_masks': [c_p, c_p, c_i64, c_i64, c_i64, c_int, c_int, c_int, c_p] + [c_i64] * 5 + [c_f, c_p, c_p],
-    'bxs_condinst_point_scores': [c_p] * 6 + [c_i64] * 4 + [c_p, c_p],
-    'bxs_condinst_decode': [c_p] * 10 + [c_i64] * 3 + [c_p, c_i64, c_p, c_p, c_f] + [c_p] * 7,
-    'bxs_condinst_gather': [c_p] * 6 + [c_i64] * 3 + [c_p, c_p, c_i64] + [c_p] * 4,
-    'bxs_box_nms_workspace_bytes': [c_p, c_i64],
-    'bxs_box_nms': [c_p] * 3 + [c_i64] * 3 + [c_f, c_p, c_p, c_p],
-    'bxs_condinst_paste_masks': [c_p] + [c_i64] * 8 + [c_int, c_p, c_p],
-}
-_RESTYPE = {'bxs_mst_workspace_bytes': c_i64, 'bxs_bfs_workspace_bytes': c_i64, 'bxs_refine_scratch_bytes': c_i64, 'bxs_lcm_workspace_bytes': c_i64, 'bxs_meanfield_workspace_bytes': c_i64, 'bxs_projection_workspace_bytes': c_i64,'bxs_condinst_head_workspace_bytes': c_i64, 'bxs_last_error': ctypes.c_char_p, 'bxs_boxinst_loss_workspace_bytes': c_i64,
-             'bxs_boxinst_loss_fused_workspace_bytes': c_i64, 'bxs_boxinst_loss_fused_sched_bytes': c_i64,
-             'bxs_boxinst_loss_plan_bytes': c_i64, 'bxs_levelset_fused_workspace_bytes': c_i64,
-             'bxs_dynconv1x1_backward_workspace_bytes': c_i64, 'bxs_corr_transfer_workspace_bytes': c_i64,
-             'bxs_dynconv1x1_half_backward_workspace_bytes': c_i64, 'bxs_lsap_workspace_bytes': c_i64,
-             'bxs_discobox_loss_workspace_bytes': c_i64, 'bxs_dynconv1x1_cells_forward_workspace_bytes': c_i64,
-             'bxs_dynconv1x1_cells_backward_workspace_bytes': c_i64,
-             'bxs_sigmoid_focal_loss_levels_forward_workspace_bytes': c_i64,
-             'bxs_softmax_cross_entropy_layers_forward_workspace_bytes': c_i64,
-             'bxs_sigmoid_focal_loss_cells_forward_workspace_bytes': c_i64, 'bxs_fcos_loss_workspace_bytes': c_i64,
-             'bxs_matrix_nms_workspace_bytes': c_i64, 'bxs_box_nms_workspace_bytes': c_i64}
+# The by-value C types the header uses.  Every pointer binds as c_void_p.  A type outside this table is an error, never a
+# guess: on x86-64 a wrong scalar type is not caught by ctypes, the call just receives a wrong value.
+_BY_VALUE = {'int64_t': c_i64, 'int': c_int, 'float': c_f, 'bxs_stream_t': c_p}
+
+
+def _ctype(c_type, where):
+    if '*' in c_type:
+        return c_p
+    if c_type not in _BY_VALUE:
+        raise TypeError(f'{where}: no ctypes mapping for the C type {c_type!r}')
+    return _BY_VALUE[c_type]
+
+
+def parse_header(text):
+    """(argtypes, restypes): name -> ctypes argument list and name -> ctypes result type of every ``bxs_*`` prototype in
+    the C header ``text``.  A ``const char*`` result is a ``c_char_p``; ``(void)`` is no argument."""
+    text = re.sub(r'/\*.*?\*/', ' ', text, flags=re.S)
+    argtypes, restypes = {}, {}
+    for stmt in text.split(';'):
+        if not re.search(r'\bbxs_\w+\s*\(', stmt):
+            continue
+        m = re.fullmatch(r'\s*([\w\s*]+?)\s*\b(bxs_\w+)\s*\(([^()]*)\)\s*', stmt)
+        if m is None:
+            raise ValueError(f'not a prototype: {" ".join(stmt.split())!r}')
+        ret, name, params = m.groups()
+        ret = ' '.join(ret.replace('*', ' * ').split())
+        restypes[name] = ctypes.c_char_p if ret == 'const char *' else _ctype(ret, name)
+        params = [] if params.strip() == 'void' else params.split(',')
+        argtypes[name] = [_ctype(' '.join(re.sub(r'\w+\s*$', '', p).split()), name) for p in params]   # drop the name
+    return argtypes, restypes
+
+
+# name -> argtypes and name -> restype of every entry point, from the prototypes the library is compiled against
+with open(HEADER_PATH) as _f:
+    SIGNATURES, RESTYPES = parse_header(_f.read())
 
 _STATUS = {-1: 'invalid argument', -2: 'kernel launch failed', -3: 'unsupported shape', -4: 'no CUDA device'}
 
@@ -149,7 +74,7 @@ def lib():
         for name, args in SIGNATURES.items():
             fn = getattr(handle, name)          # AttributeError if the .so does not export it
             fn.argtypes = args
-            fn.restype = _RESTYPE.get(name, c_int)
+            fn.restype = RESTYPES[name]
         _lib = handle
     return _lib
 

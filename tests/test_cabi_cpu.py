@@ -1,5 +1,5 @@
 """CPU: the C-ABI shared library loads without a GPU and exports every symbol include/boxseg_b200.h
-declares; the ctypes table binds exactly that set; host-side argument validation works."""
+declares; the ctypes types read from the header are the C types; host-side argument validation works."""
 import ctypes
 import os
 import re
@@ -7,12 +7,16 @@ import re
 import pytest
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+c_p, c_i64, c_int, c_f = ctypes.c_void_p, ctypes.c_int64, ctypes.c_int, ctypes.c_float
+
+
+def _header():
+    with open(os.path.join(ROOT, 'include', 'boxseg_b200.h')) as f:
+        return re.sub(r'/\*.*?\*/', '', f.read(), flags=re.S)
 
 
 def _declared():
-    text = open(os.path.join(ROOT, 'include', 'boxseg_b200.h')).read()
-    text = re.sub(r'/\*.*?\*/', '', text, flags=re.S)
-    return sorted(set(re.findall(r'\b(bxs_\w+)\s*\(', text)))
+    return sorted(set(re.findall(r'\b(bxs_\w+)\s*\(', _header())))
 
 
 @pytest.fixture(scope='module')
@@ -29,8 +33,47 @@ def test_every_declared_symbol_is_exported_and_bound(lib):
     handle = ctypes.CDLL(lib.LIB_PATH)
     missing = [n for n in names if not hasattr(handle, n)]
     assert not missing, f'declared in the header but not exported: {missing}'
-    assert sorted(lib.SIGNATURES) == names, (set(names) ^ set(lib.SIGNATURES))
-    lib.lib()           # resolves + types every symbol
+    h = lib.lib()           # resolves + types every symbol
+    for n in names:
+        fn = getattr(h, n)
+        assert fn.argtypes == lib.SIGNATURES[n] and fn.restype is lib.RESTYPES[n], n
+
+
+@pytest.mark.parametrize('name, argtypes, restype', [
+    ('bxs_boxinst_targets_forward', [c_p] * 13 + [c_i64] * 3 + [c_int] * 3 + [c_f, c_p], c_int),
+    ('bxs_corr_retrieve', [c_p] * 19 + [c_i64] * 8 + [c_f] * 6 + [c_int] * 2 + [c_p], c_int),
+    ('bxs_dynconv1x1_cells_forward', [c_p] * 9 + [c_i64] * 4 + [c_p], c_int),            # const float* const*
+    ('bxs_lsap_workspace_bytes', [c_p, c_p, c_i64], c_i64),
+    ('bxs_version', [], c_int),
+    ('bxs_last_error', [], ctypes.c_char_p),
+])
+def test_header_signatures(name, argtypes, restype):
+    from boxinstseg_b200 import _lib as lib
+    assert lib.SIGNATURES[name] == argtypes and lib.RESTYPES[name] is restype
+
+
+def test_every_int64_result_is_bound_as_int64():
+    """A size query left at ctypes' default c_int would truncate a workspace of 2 GiB or more."""
+    from boxinstseg_b200 import _lib as lib
+    wide = set(re.findall(r'\bint64_t\s+(bxs_\w+)\s*\(', _header()))
+    assert len(wide) >= 25
+    assert {n for n, r in lib.RESTYPES.items() if r is c_i64} == wide
+    assert {n for n, r in lib.RESTYPES.items() if r is c_int} == set(lib.SIGNATURES) - wide - {'bxs_last_error'}
+
+
+def test_parse_header_on_text():
+    from boxinstseg_b200 import _lib as lib
+    text = '''/* bxs_in_a_comment(double x); */
+    typedef void* bxs_stream_t;
+    int64_t bxs_a(const void* const* p, int64_t n, int k, float x, bxs_stream_t s);
+    int bxs_b(void);'''
+    argtypes, restypes = lib.parse_header(text)
+    assert argtypes == {'bxs_a': [c_p, c_i64, c_int, c_f, c_p], 'bxs_b': []}
+    assert restypes == {'bxs_a': c_i64, 'bxs_b': c_int}
+    with pytest.raises(TypeError):
+        lib.parse_header('int bxs_c(const void* p, double x);')
+    with pytest.raises(TypeError):
+        lib.parse_header('double bxs_d(int n);')
 
 
 def test_identity_and_no_device(lib):
