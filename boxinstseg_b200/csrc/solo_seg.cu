@@ -13,6 +13,8 @@
 //           pixels (sigmoid on the fly for logits), rounded to the row dtype between and after the stages as ATen rounds a
 //           16-bit tensor (or, under autocast, kept in float32: autocast runs upsample_bilinear2d in float32), then the
 //           threshold.  The [n, 4h, 4w] intermediate of the reference never exists.
+//   maskformer paste: the same per-pixel function (paste_value) on Box2Mask's logit rows, with a first stage of any size
+//           and stages that may be skipped, plus each mask's area, masked sum and box folded in the pass that writes it.
 #include <cuda_fp16.h>
 
 #include <type_traits>
@@ -218,23 +220,71 @@ __global__ void __launch_bounds__(SS_NT) solo_paste_kernel(RowSources src, const
         continue;
       }
       const int y = (int)(pix / W_ori), x = (int)(pix % W_ori);
-      const PasteTaps pt = paste_taps(y, x, H_img, W_img, H_ori, W_ori);
-      float v[2][2];
-#pragma unroll
-      for (int a = 0; a < 2; ++a) {
-        const RsTap ty = paste_stage1_tap(pt.y1[a], h);
-#pragma unroll
-        for (int c = 0; c < 2; ++c) {
-          const RsTap tx = paste_stage1_tap(pt.x1[c], w);
-          const T* q = p + ty.i0 * w + tx.i0;
-          v[a][c] = stage<T, kRound>(rs_lerp2(ty, tx, prob(q[0], logits), prob(q[tx.ip], logits), prob(q[ty.ip * w], logits),
-                                         prob(q[ty.ip * w + tx.ip], logits)));
-        }
-      }
-      o[pix] = stage<T, kRound>(rs_lerp2(pt.ty2, pt.tx2, v[0][0], v[0][1], v[1][0], v[1][1])) > t;
+      const PasteGeom g{h, w, 4 * h, 4 * w, H_img, W_img, H_ori, W_ori, false, false};
+      o[pix] = paste_value<false>(
+                   g, y, x, [&](int q, int d) { return prob((p + q)[d], logits); },
+                   [](float v) { return stage<T, kRound>(v); }) > t;
     }
   }
 }
+
+// MaskFormer's instance masks (maskformer_fusion_head.py:112-241 after box2mask_head.py:445-459): the same per-pixel paste
+// of logit rows, thresholded at 0, a float16 row rounded after each stage; each CTA also folds its set pixels into a
+// MaskStats (sigmoid as torch computes it for T) and writes it to part[k * gridDim.x + blockIdx.x], reduced in a fixed order
+// (lanes by the butterfly, warps in index order) so that the float64 sum is the same from run to run.
+template <typename T>
+__global__ void __launch_bounds__(SS_NT) maskformer_paste_kernel(RowSources src, const int64_t* __restrict__ rows, int64_t n,
+                                                                 PasteGeom g, uint8_t* __restrict__ out,
+                                                                 MaskStats* __restrict__ part) {
+  constexpr bool kRound = std::is_same<T, __half>::value;
+  __shared__ MaskStats s_part[SS_NT / kWarp];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int64_t npix = (int64_t)g.H_out * g.W_out;
+  for (int64_t k = blockIdx.y; k < n; k += gridDim.y) {
+    const T* p = row_ptr<T>(src, rows[k], (int64_t)g.h * g.w);
+    uint8_t* o = out + k * npix;
+    MaskStats st = mask_stats_empty();
+    for (int64_t pix = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; pix < npix; pix += (int64_t)gridDim.x * blockDim.x) {
+      const int y = (int)(pix / g.W_out), x = (int)(pix % g.W_out);
+      const float v = p ? paste_value<true>(
+                              g, y, x, [&](int q, int d) { return prob((p + q)[d], false); },
+                              [](float u) { return stage<T, kRound>(u); })
+                        : 0.f;
+      const bool on = v > 0.f;
+      o[pix] = on;
+      if (on) mask_stats_add(st, y, x, kRound ? prob(__float2half_rn(v), true) : prob(v, true));
+    }
+    st.sum = warp_sum(st.sum);
+    st.area = __reduce_add_sync(kFull, st.area);
+    st.x0 = __reduce_min_sync(kFull, st.x0);
+    st.y0 = __reduce_min_sync(kFull, st.y0);
+    st.x1 = __reduce_max_sync(kFull, st.x1);
+    st.y1 = __reduce_max_sync(kFull, st.y1);
+    if (lane == 0) s_part[warp] = st;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      MaskStats s = s_part[0];
+      for (int i = 1; i < SS_NT / kWarp; ++i) mask_stats_merge(s, s_part[i]);
+      part[k * gridDim.x + blockIdx.x] = s;
+    }
+    __syncthreads();
+  }
+}
+
+// the n_part partials of every row, in index order -> area, masked_sum (one float32 rounding), box
+__global__ void __launch_bounds__(SS_NT) maskformer_stats_kernel(const MaskStats* __restrict__ part, int64_t n, int n_part,
+                                                                 int32_t* __restrict__ area, float* __restrict__ masked_sum,
+                                                                 float* __restrict__ box) {
+  const int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= n) return;
+  MaskStats s = part[k * n_part];
+  for (int i = 1; i < n_part; ++i) mask_stats_merge(s, part[k * n_part + i]);
+  area[k] = s.area;
+  masked_sum[k] = (float)s.sum;
+  mask_stats_box(s, box + 4 * k);
+}
+
+constexpr int MF_MAX_PARTS = 64;       // CTAs per row of the maskformer paste: 256-thread CTAs, one partial each
 
 }  // namespace
 }  // namespace bxs
@@ -305,5 +355,38 @@ extern "C" int bxs_solo_paste_masks(const void* const* src_host, const int64_t* 
                          : (interp_f32 ? solo_paste_kernel<__half, false> : solo_paste_kernel<__half, true>);
   kern<<<dim3(gx, gy), SS_NT, 0, as_stream(stream)>>>(src, rows, n, (int)h, (int)w, (int)H_img, (int)W_img, (int)H_ori,
                                                       (int)W_ori, logits, mask_thr, out);
+  return check_launch();
+}
+
+extern "C" int64_t bxs_maskformer_paste_workspace_bytes(int64_t n) {
+  if (n <= 0) return 0;
+  return n * MF_MAX_PARTS * (int64_t)sizeof(MaskStats);
+}
+
+extern "C" int bxs_maskformer_paste_masks(const void* const* src_host, const int64_t* src_rows_host, int64_t n_src, int64_t h,
+                                          int64_t w, int dtype, const int64_t* rows, int64_t n, int64_t H_pad, int64_t W_pad,
+                                          int64_t H_img, int64_t W_img, int rescale, int64_t H_out, int64_t W_out,
+                                          void* workspace, uint8_t* out, int32_t* area, float* masked_sum, float* box,
+                                          bxs_stream_t stream) {
+  RowSources src;
+  if (int rc = make_sources(src, src_host, src_rows_host, n_src)) return rc;
+  if (h <= 0 || w <= 0 || n < 0 || H_img <= 0 || W_img <= 0 || H_out <= 0 || W_out <= 0 || (dtype != 0 && dtype != 1))
+    return BXS_ERR_INVALID_ARG;
+  if (h > H_pad || w > W_pad || H_img > H_pad || W_img > W_pad) return BXS_ERR_INVALID_ARG;
+  if (!rescale && (H_out != H_img || W_out != W_img)) return BXS_ERR_INVALID_ARG;
+  if (H_pad > INT32_MAX || W_pad > INT32_MAX || h * w > INT32_MAX || H_out * W_out > INT32_MAX || n > INT32_MAX)
+    return BXS_ERR_UNSUPPORTED;
+  if (n == 0) return BXS_OK;
+  if (!rows || !workspace || !out || !area || !masked_sum || !box) return BXS_ERR_INVALID_ARG;
+  const PasteGeom g{(int)h, (int)w, (int)H_pad, (int)W_pad, (int)H_img, (int)W_img, (int)H_out, (int)W_out,
+                    h == H_pad && w == W_pad, !rescale};
+  const unsigned gx = (unsigned)std::min<int64_t>(ceil_div(H_out * W_out, SS_NT), MF_MAX_PARTS);
+  const unsigned gy = (unsigned)std::min<int64_t>(n, 65535);
+  MaskStats* part = static_cast<MaskStats*>(workspace);
+  cudaStream_t s = as_stream(stream);
+  auto kern = dtype == 0 ? maskformer_paste_kernel<float> : maskformer_paste_kernel<__half>;
+  kern<<<dim3(gx, gy), SS_NT, 0, s>>>(src, rows, n, g, out, part);
+  if (int rc = check_launch()) return rc;
+  maskformer_stats_kernel<<<(unsigned)ceil_div(n, SS_NT), SS_NT, 0, s>>>(part, n, (int)gx, area, masked_sum, box);
   return check_launch();
 }

@@ -791,6 +791,14 @@ class Box2MaskHead(nn.Module):
             lst_feat_list.append(lst_feat)
         return cls_pred_list, mask_pred_list, lst_feat_list
 
+    # box2mask_head.py:445-459, the reference's signature
+    def simple_test(self, feats, img_metas, **kwargs):
+        """(mask_cls [B,Q,K+1], mask_pred [B,Q,h,w]) of the last decoder layer.  Unlike the reference, the mask predictions
+        stay at the mask-feature resolution: MaskFormerFusionHead.simple_test upsamples them to batch_input_shape inside
+        its paste.  ``ops.resize.bilinear_resize(mask_pred, batch_input_shape)`` gives the reference's tensor bit for bit."""
+        all_cls_scores, all_mask_preds, _ = self(feats, img_metas)
+        return all_cls_scores[-1], all_mask_preds[-1]
+
     # a17 -- box2mask_head.py:229-233, 269-335
     def mask_loss_single(self, mask_preds, mask_targets, num_per_img, norm_img, lst_feat, trees=None):
         """mask_preds [n,h,w] matched logits (images concatenated), mask_targets [n,H,W] box masks,

@@ -1,5 +1,6 @@
 """SOLOv2 inference on the kernels of csrc/solo_seg.cu: per-row mask statistics, Matrix NMS (mmdet/core/post_processing/
-matrix_nms.py) and the fused mask paste of get_seg_single (box_solov2_head.py:576-585, discobox_head.py:1645-1653).
+matrix_nms.py) and the fused mask paste of get_seg_single (box_solov2_head.py:576-585, discobox_head.py:1645-1653); and
+Box2Mask's instance masks on the same paste (maskformer_fusion_head.py:112-241), with their statistics.
 
 Row sources: the mask rows the kernels read are given as a list of tensors [rows_s, h, w] (float32 or float16, any layout:
 made dense here) and addressed by a row id into their concatenation, so that BoxSOLOv2's per-level [B,S^2,h,w] predictions are
@@ -87,6 +88,29 @@ def paste_rows(src, rows, img_hw, ori_hw, mask_thr, logits=False, interp_f32=Fal
                                              int(logits), int(interp_f32), L.ptr(rows), n, H_img, W_img, H_ori, W_ori, float(mask_thr),
                                              L.ptr(out), L.stream()), 'solo_paste_masks')
     return out
+
+
+def maskformer_paste_rows(src, rows, pad_hw, img_hw, ori_hw=None):
+    """MaskFormer's instance masks of the LOGIT rows ``rows`` of ``src`` and their statistics, in one pass: masks bool
+    [n, H, W] = interpolate(interpolate(x, pad_hw)[:H_img, :W_img], ori_hw) > 0 (bilinear, align_corners=False; a stage
+    whose sizes match is skipped, so ``ori_hw=None`` gives the crop at ``img_hw``), area int32 [n], masked_sum float32 [n]
+    (the sum of sigmoid over the set pixels) and box float32 [n, 4] (mask2bbox).  Two launches, no host read."""
+    rows = rows.to(device=src.device, dtype=torch.int64).contiguous()
+    n = rows.numel()
+    (H_pad, W_pad), (H_img, W_img) = [int(v) for v in pad_hw[:2]], [int(v) for v in img_hw[:2]]
+    H_out, W_out = (H_img, W_img) if ori_hw is None else [int(v) for v in ori_hw[:2]]
+    dev = src.device
+    out = torch.empty((n, H_out, W_out), dtype=torch.bool, device=dev)
+    area = torch.empty(n, dtype=torch.int32, device=dev)
+    msum = torch.empty(n, dtype=torch.float32, device=dev)
+    box = torch.empty((n, 4), dtype=torch.float32, device=dev)
+    with torch.cuda.device(dev):
+        ws = torch.empty(L.lib().bxs_maskformer_paste_workspace_bytes(n), dtype=torch.uint8, device=dev)
+        L.check(L.lib().bxs_maskformer_paste_masks(src.ptrs, src.rows, len(src.tensors), src.h, src.w, _DTYPE[src.dtype],
+                                                   L.ptr(rows), n, H_pad, W_pad, H_img, W_img, int(ori_hw is not None),
+                                                   H_out, W_out, L.ptr(ws), L.ptr(out), L.ptr(area), L.ptr(msum),
+                                                   L.ptr(box), L.stream()), 'maskformer_paste_masks')
+    return out, area, msum, box
 
 
 def paste_masks(rows, featmap_size, img_shape, ori_shape, mask_thr):

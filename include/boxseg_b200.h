@@ -717,6 +717,15 @@ int bxs_fcos_loss_backward(float* g_pred, int64_t n_pred, const float* g_loss_bb
  *   the arithmetic of bxs_bilinear_resize_forward; a float16 row is rounded to float16 after each stage and compared in
  *   float16, as ATen computes on a float16 tensor, or with interp_f32 != 0 interpolated and compared in float32 without
  *   rounding (torch.autocast runs upsample_bilinear2d in float32).  H_img <= 4h, W_img <= 4w.
+ * bxs_maskformer_paste_masks (MaskFormerFusionHead.instance_postprocess after Box2MaskHead.simple_test's upsample): for n
+ *   row ids of LOGITS (no sigmoid before the resizes) -> out u8 [n, H_out, W_out] = interpolate(interpolate(x, (H_pad,
+ *   W_pad))[:H_img, :W_img], (H_out, W_out)) > 0, bilinear with align_corners=False in the arithmetic of
+ *   bxs_bilinear_resize_forward, a float16 row rounded to float16 after each stage.  The first stage is skipped when (h, w)
+ *   == (H_pad, W_pad), the second when rescale == 0 (then (H_out, W_out) == (H_img, W_img)): the value is read, as ATen
+ *   copies, not lerped.  In the same pass, per row: area i32 [n] = the set pixels, masked_sum f32 [n] = the sum of
+ *   sigmoid(v) over them (torch's sigmoid for the dtype, accumulated in float64 in a fixed order, rounded once), box f32
+ *   [n,4] = [x_min, y_min, x_max + 1, y_max + 1] of them (mask2bbox), zeros for an empty mask.  h <= H_pad, w <= W_pad,
+ *   H_img <= H_pad, W_img <= W_pad.  workspace: bxs_maskformer_paste_workspace_bytes(n) bytes, 8-byte aligned.  Two launches.
  * No host synchronisation, deterministic.  BXS_ERR_INVALID_ARG: a NULL pointer the call needs, a negative count, a
  * non-positive size, an unknown dtype or kernel.  BXS_ERR_UNSUPPORTED: n_src > 8, more than INT32_MAX rows or pixels per
  * plane, more than 65535 images or 65535 * 32 slots.  All checks run before any device call.
@@ -731,6 +740,11 @@ int bxs_matrix_nms(const uint32_t* bits, int64_t words, const int64_t* row, cons
 int bxs_solo_paste_masks(const void* const* src_host, const int64_t* src_rows_host, int64_t n_src, int64_t h, int64_t w,
                          int dtype, int logits, int interp_f32, const int64_t* rows, int64_t n, int64_t H_img, int64_t W_img,
                          int64_t H_ori, int64_t W_ori, float mask_thr, uint8_t* out, bxs_stream_t stream);
+int64_t bxs_maskformer_paste_workspace_bytes(int64_t n);
+int bxs_maskformer_paste_masks(const void* const* src_host, const int64_t* src_rows_host, int64_t n_src, int64_t h, int64_t w,
+                               int dtype, const int64_t* rows, int64_t n, int64_t H_pad, int64_t W_pad, int64_t H_img,
+                               int64_t W_img, int rescale, int64_t H_out, int64_t W_out, void* workspace, uint8_t* out,
+                               int32_t* area, float* masked_sum, float* box, bxs_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------
  * CondInst inference   replaces the level loop of CondInstBoxHead._get_bboxes (condinst_head.py:762-813), the NMS of
