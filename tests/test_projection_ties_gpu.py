@@ -9,9 +9,6 @@ time.  The generators below plant ties wherever a kernel merges partial maxima: 
 float64 oracle: oracle.boxinst.projection_losses_logit_argmax plus the pairwise term of oracle.boxinst.pairwise_nlog.
 """
 import functools
-import os
-import subprocess
-import sys
 
 import pytest
 import torch
@@ -20,7 +17,6 @@ from oracle import boxinst as ob
 
 pytestmark = pytest.mark.gpu
 DEV = 'cuda:0'
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 UPSTREAM = [(1.0, 1.0), (0.75, 2.5), (1.0, 0.0), (0.0, 1.0)]      # (g_prj, g_pair)
 
 
@@ -250,17 +246,6 @@ def test_two_call_no_grad_and_second_backward_ties(kind, shape):
         _check(p, r3, gp, gq, exact_support=kind != 'saturated')
         r4 = _second_backward(p, gp, gq)
         assert torch.equal(r3[2], r4[2])
-
-
-def test_single_pass_ties_on_the_cta_schedule():
-    """The CTA-granular single-pass schedule is chosen by BXS_ONEPASS_CTA=1, once per process: run the single-pass tie
-    cases again in a child process that selects it."""
-    env = dict(os.environ, BXS_ONEPASS_CTA='1')
-    r = subprocess.run([sys.executable, '-m', 'pytest', '-q', '-p', 'no:cacheprovider', '-m', 'gpu',
-                        os.path.join('tests', 'test_projection_ties_gpu.py') + '::test_single_pass_ties'],
-                       cwd=ROOT, env=env, capture_output=True, text=True, timeout=1200)
-    assert r.returncode == 0, r.stdout[-4000:] + r.stderr[-2000:]
-    assert f'{len(KINDS) * len(SHAPES)} passed' in r.stdout, r.stdout[-2000:]
 
 
 @pytest.mark.parametrize('kind', KINDS)

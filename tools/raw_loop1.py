@@ -18,13 +18,10 @@ inst_gt = case['gt_inds'].to(dev).to(torch.int32)
 ws = torch.empty(lib.bxs_boxinst_loss_fused_workspace_bytes(N_INST, H, W), dtype=torch.uint8, device=dev)
 sched = torch.zeros(int(lib.bxs_boxinst_loss_fused_sched_bytes()), dtype=torch.uint8, device=dev)
 out = torch.empty(4, device=dev); g = torch.ones(2, device=dev)
-plan = None if os.environ.get('BXS_ONEPASS_CTA') == '1' else boxinst_loss_plan(t, inst_gt, H, W, 2)
+plan = boxinst_loss_plan(t, inst_gt, H, W, 2)
 def raw(i, st):
     x, gl = xs[i % R], gls[i % R]
-    if plan is not None:
-        rc = lib.bxs_boxinst_loss_fused_forward_planned(L.ptr(x), L.ptr(t.edge_bits), L.ptr(plan), L.ptr(it), 10000.0, L.ptr(ws), L.ptr(sched), L.ptr(out), L.ptr(gl), N_INST, H, W, 2, st)
-    else:
-        rc = lib.bxs_boxinst_loss_fused_forward(L.ptr(x), L.ptr(t.edge_bits), L.ptr(t.rects), L.ptr(inst_gt), L.ptr(t.gt_img), L.ptr(it), 10000.0, L.ptr(ws), L.ptr(sched), L.ptr(out), L.ptr(gl), N_INST, H, W, 2, st)
+    rc = lib.bxs_boxinst_loss_fused_forward_planned(L.ptr(x), L.ptr(t.edge_bits), L.ptr(plan), L.ptr(it), 10000.0, L.ptr(ws), L.ptr(sched), L.ptr(out), L.ptr(gl), N_INST, H, W, 2, st)
     assert rc == 0, rc
     rc = lib.bxs_boxinst_loss_fused_backward(L.ptr(ws), L.ptr(g[0:1]), L.ptr(g[1:2]), L.ptr(gl), N_INST, H, W, st)
     assert rc == 0, rc
