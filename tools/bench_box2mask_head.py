@@ -17,24 +17,17 @@ import argparse
 import ctypes
 import json
 import os
-import statistics
-import subprocess
 import sys
 import time
-import warnings
 
 import torch
 import torch.nn.functional as F
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+from benchkit import card, kernel_launches, summary, syncs, time_call  # noqa: E402
 
 B, Q, C, HF, HEADS = 1, 100, 256, 256, 8
 SIZES = ((32, 32), (64, 64), (128, 128))
-
-
-def card():
-    q = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit', '--format=csv,noheader'], capture_output=True, text=True)
-    return {'torch_name': torch.cuda.get_device_name(0), 'nvidia_smi': q.stdout.strip().splitlines()[:1]}
 
 
 def ref_arm(embed, feat, size):
@@ -55,43 +48,22 @@ def new_arm(embed, feat, size):
 
 def layer_times(fn, embed, feat, iters):
     """(GPU ms, host ms) per layer: the mean over `iters` passes of the three target sizes."""
-    ev = [torch.cuda.Event(enable_timing=True) for _ in range(2)]
-    torch.cuda.synchronize()
+    def host_clock(size):
+        t0 = time.perf_counter()
+        fn(embed, feat, size)
+        return time.perf_counter() - t0
     host, gpu = 0.0, 0.0
     for _ in range(iters):
         for size in SIZES:
-            ev[0].record()
-            t0 = time.perf_counter()
-            fn(embed, feat, size)
-            host += time.perf_counter() - t0
-            ev[1].record()
-            ev[1].synchronize()
-            gpu += ev[0].elapsed_time(ev[1])
+            g, h = time_call(lambda: host_clock(size))
+            gpu += g
+            host += h
     n = iters * len(SIZES)
     return gpu / n, host * 1e3 / n
 
 
-def launches(fn, embed, feat):
-    with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
-        for size in SIZES:
-            fn(embed, feat, size)
-        torch.cuda.synchronize()
-    kern = [e for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA and 'Memcpy' not in e.name
-            and 'Memset' not in e.name]
-    return len(kern) / len(SIZES)
-
-
-def syncs(fn, embed, feat):
-    torch.cuda.synchronize()
-    torch.cuda.set_sync_debug_mode('warn')
-    try:
-        with warnings.catch_warnings(record=True) as w:
-            warnings.simplefilter('always')
-            for size in SIZES:
-                fn(embed, feat, size)
-    finally:
-        torch.cuda.set_sync_debug_mode('default')
-    return sum('synchroniz' in str(x.message) for x in w) / len(SIZES)
+def all_sizes(fn, embed, feat):
+    return lambda: [fn(embed, feat, size) for size in SIZES]
 
 
 def kernel_only(path, mask_pred, iters):
@@ -105,18 +77,8 @@ def kernel_only(path, mask_pred, iters):
         args = (L.ptr(mask_pred), L.ptr(attn), B, Q, HF, HF, h, w, HEADS, 0, 1, L.stream())
         for _ in range(3):
             L.check(f(*args), 'warm-up')
-        ev = [torch.cuda.Event(enable_timing=True) for _ in range(2)]
-        ev[0].record()
-        for _ in range(iters):
-            f(*args)
-        ev[1].record()
-        torch.cuda.synchronize()
-        out[f'{h}x{w}'] = ev[0].elapsed_time(ev[1]) / iters
+        out[f'{h}x{w}'] = time_call(lambda: f(*args), reps=iters)[0]
     return out
-
-
-def summary(xs):
-    return {'median': statistics.median(xs), 'min': min(xs), 'max': max(xs), 'all': xs}
 
 
 def main():
@@ -149,7 +111,8 @@ def main():
                 host[a].append(h)
         for a, fn in arms.items():
             res[a] = {'gpu_ms_per_layer': summary(gpu[a]), 'host_ms_per_layer': summary(host[a]),
-                      'launches_per_layer': launches(fn, embed, feat), 'syncs_per_layer': syncs(fn, embed, feat)}
+                      'launches_per_layer': kernel_launches(all_sizes(fn, embed, feat)) / len(SIZES),
+                      'syncs_per_layer': syncs(all_sizes(fn, embed, feat)) / len(SIZES)}
             r = res[a]
             print(f'{a:3s} GPU {r["gpu_ms_per_layer"]["median"]:.4f} ms [{r["gpu_ms_per_layer"]["min"]:.4f}, '
                   f'{r["gpu_ms_per_layer"]["max"]:.4f}]  host {r["host_ms_per_layer"]["median"]:.4f} ms '

@@ -18,26 +18,19 @@ run.  Prints one JSON document; `--out PATH` also writes it.
 import argparse
 import json
 import os
-import statistics
-import subprocess
 import sys
-import warnings
 
 import torch
 import torch.nn.functional as F
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
+from benchkit import card, ms_summary, peak_alloc, profile, syncs, time_call  # noqa: E402
 from oracle import box2mask_infer as obi  # noqa: E402
 
 HBM = 3.35e12
 Q, K, HW, PAD, IMG, ORI = 100, 80, (200, 272), (800, 1088), (800, 1067), ((480, 640), (427, 640))
 KERNELS = ('maskformer_paste_kernel', 'maskformer_stats_kernel')
-
-
-def card():
-    q = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit', '--format=csv,noheader'], capture_output=True, text=True)
-    return {'torch_name': torch.cuda.get_device_name(0), 'nvidia_smi': q.stdout.strip().splitlines()[:1]}
 
 
 def workload(B, seed=0):
@@ -67,35 +60,6 @@ def ref_arm(mask_cls, mask_pred, metas):
         binary = binary.bool()
         out.append((labels, torch.cat([obi.mask2bbox(binary), det[:, None]], -1), binary))
     return out
-
-
-def time_call(fn):
-    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    a.record()
-    out = fn()
-    b.record()
-    torch.cuda.synchronize()
-    return a.elapsed_time(b), out
-
-
-def count_syncs(fn):
-    torch.cuda.synchronize()
-    with warnings.catch_warnings(record=True) as rec:
-        warnings.simplefilter('always')
-        torch.cuda.set_sync_debug_mode('warn')
-        try:
-            fn()
-        finally:
-            torch.cuda.set_sync_debug_mode('default')
-    return sum('called a synchronizing' in str(r.message) for r in rec)
-
-
-def profile(fn):
-    from torch.profiler import ProfilerActivity, profile as prof
-    with prof(activities=[ProfilerActivity.CUDA]) as p:
-        fn()
-        torch.cuda.synchronize()
-    return {e.key: (e.count, e.device_time_total / 1e3) for e in p.key_averages() if e.device_type.name == 'CUDA' and e.count}
 
 
 def kernel_bytes(B):
@@ -128,14 +92,10 @@ def main():
                 t[k].append(time_call(f)[0])
         rec = {}
         for k, f in fns.items():
-            torch.cuda.synchronize()
-            torch.cuda.reset_peak_memory_stats()
-            base = torch.cuda.memory_allocated()
-            _, out = time_call(f)
-            peak = torch.cuda.max_memory_allocated() - base
+            peak, out = peak_alloc(f)
             kern = profile(f)
-            rec[k] = {'median_ms': statistics.median(t[k]), 'min_ms': min(t[k]), 'max_ms': max(t[k]),
-                      'launches': sum(c for c, _ in kern.values()), 'syncs': count_syncs(f), 'peak_bytes': peak,
+            rec[k] = {**ms_summary(t[k]), 'launches': sum(c for c, _ in kern.values()), 'syncs': syncs(f),
+                      'peak_bytes': peak,
                       'detections': [len(o[0]) for o in out]}
             if k == 'new':
                 need = kernel_bytes(B)

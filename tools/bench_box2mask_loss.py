@@ -18,23 +18,16 @@ card's name and power limit read in the same run.  Prints one JSON document; `--
 import argparse
 import json
 import os
-import statistics
-import subprocess
 import sys
-import warnings
 
 import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
+from benchkit import card, launches, ms_summary, peak_alloc, syncs, time_call  # noqa: E402
 from oracle import box2mask_loss as obl  # noqa: E402
 
 DEV = 'cuda:0'
-
-
-def card():
-    q = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit', '--format=csv,noheader'], capture_output=True, text=True)
-    return {'torch_name': torch.cuda.get_device_name(0), 'nvidia_smi': q.stdout.strip().splitlines()[:1]}
 
 
 def workload(seed=0, layers=10):
@@ -65,39 +58,6 @@ def arms(head, case):
     return {'ref': ref, 'new': new}
 
 
-def timed(fn):
-    torch.cuda.synchronize()
-    torch.cuda.reset_peak_memory_stats()
-    base = torch.cuda.memory_allocated()
-    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    a.record()
-    fn()
-    b.record()
-    torch.cuda.synchronize()
-    return a.elapsed_time(b), torch.cuda.max_memory_allocated() - base
-
-
-def syncs(fn):
-    torch.cuda.synchronize()
-    with warnings.catch_warnings(record=True) as seen:
-        warnings.simplefilter('always')
-        torch.cuda.set_sync_debug_mode('warn')
-        try:
-            fn()
-        finally:
-            torch.cuda.set_sync_debug_mode(0)
-    return sum('synchroniz' in str(w.message) for w in seen)
-
-
-def launches(fn):
-    from torch.profiler import ProfilerActivity, profile
-    torch.cuda.synchronize()
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        fn()
-        torch.cuda.synchronize()
-    return sum(1 for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA)
-
-
 def ce_alone(head, case, reps=100):
     """The 10 layers' classification losses, forward + backward: one kernel pair against the reference's torch lines."""
     from boxinstseg_b200.ops.cross_entropy import softmax_cross_entropy_layers
@@ -119,8 +79,8 @@ def ce_alone(head, case, reps=100):
     for name, fn in (('kernel', kernel), ('torch_lines', torch_lines)):
         for _ in range(5):
             fn()
-        ts = [timed(fn)[0] for _ in range(reps)]
-        out[name] = dict(median_ms=statistics.median(ts), min_ms=min(ts), max_ms=max(ts), launches=launches(fn))
+        ts = [time_call(fn)[0] for _ in range(reps)]
+        out[name] = dict(**ms_summary(ts), launches=launches(fn))
     out['bytes'] = dict(scores=sum(c.numel() * 4 for c in cls), grad=sum(c.numel() * 4 for c in cls))
     return out
 
@@ -141,15 +101,15 @@ def main():
     times, peaks = {k: [] for k in fns}, {k: 0 for k in fns}
     for r in range(args.rounds):                                   # alternate the arms, starting side swapped each round
         for name in (list(fns) if r % 2 == 0 else list(fns)[::-1]):
-            t, p = timed(fns[name])
+            p, t = peak_alloc(lambda: time_call(fns[name])[0])
             times[name].append(t)
             peaks[name] = max(peaks[name], p)
     res = dict(card=card(), workload='Box2MaskHead.loss at config E: 1 x 1024x1024, 8 GT, 10 decoder layers x 100 queries, '
                                      '256x256 mask logits, forward + backward to every layer\'s scores, logits and level-set '
                                      'feature', rounds=args.rounds)
     for name, fn in fns.items():
-        res[name] = dict(median_ms=statistics.median(times[name]), min_ms=min(times[name]), max_ms=max(times[name]),
-                         peak_alloc_bytes=peaks[name], launches=launches(fn), host_syncs=syncs(fn))
+        res[name] = dict(**ms_summary(times[name]), peak_alloc_bytes=peaks[name], launches=launches(fn),
+                         host_syncs=syncs(fn))
     res['speedup_median'] = res['ref']['median_ms'] / res['new']['median_ms']
     res['cross_entropy'] = ce_alone(head, case)
     text = json.dumps(res, indent=1)

@@ -18,24 +18,17 @@ and the card's name and power limit read in the same run.  Prints one JSON docum
 import argparse
 import json
 import os
-import statistics
-import subprocess
 import sys
-import warnings
 
 import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
+from benchkit import capture, card, launches, ms_summary, replay_ms, syncs, time_call  # noqa: E402
 from oracle import fcos_loss as ofl  # noqa: E402
 from oracle.make_golden_fcos_loss import STRIDES, case  # noqa: E402
 
 DEV = 'cuda:0'
-
-
-def card():
-    q = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit', '--format=csv,noheader'], capture_output=True, text=True)
-    return {'torch_name': torch.cuda.get_device_name(0), 'nvidia_smi': q.stdout.strip().splitlines()[:1]}
 
 
 def workload(seed=0):
@@ -59,58 +52,6 @@ def arms(head, leaves, boxes, labels):
         out = ofl.loss(*parts, boxes, labels, STRIDES, 80)
         return torch.autograd.grad(sum(out[0].values()), leaves)
     return {'ref': ref, 'new': new}
-
-
-def timed(fn):
-    torch.cuda.synchronize()
-    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    a.record()
-    fn()
-    b.record()
-    torch.cuda.synchronize()
-    return a.elapsed_time(b)
-
-
-def syncs(fn):
-    torch.cuda.synchronize()
-    with warnings.catch_warnings(record=True) as seen:
-        warnings.simplefilter('always')
-        torch.cuda.set_sync_debug_mode('warn')
-        try:
-            fn()
-        finally:
-            torch.cuda.set_sync_debug_mode(0)
-    return sum('synchroniz' in str(w.message) for w in seen)
-
-
-def launches(fn):
-    from torch.profiler import ProfilerActivity, profile
-    torch.cuda.synchronize()
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        fn()
-        torch.cuda.synchronize()
-    return sum(1 for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA)
-
-
-def graph_replay_ms(fn, reps=200):
-    s = torch.cuda.Stream()
-    s.wait_stream(torch.cuda.current_stream())
-    with torch.cuda.stream(s):
-        fn()
-    torch.cuda.current_stream().wait_stream(s)
-    g = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(g):
-        fn()
-    for _ in range(10):
-        g.replay()
-    torch.cuda.synchronize()
-    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    a.record()
-    for _ in range(reps):
-        g.replay()
-    b.record()
-    torch.cuda.synchronize()
-    return a.elapsed_time(b) / reps
 
 
 def algorithmic_bytes(leaves):
@@ -138,14 +79,13 @@ def main():
     times = {k: [] for k in fns}
     for r in range(args.rounds):                                   # alternate the arms, starting side swapped each round
         for name in (list(fns) if r % 2 == 0 else list(fns)[::-1]):
-            times[name].append(timed(fns[name]))
+            times[name].append(time_call(fns[name])[0])
     res = dict(card=card(), workload='CondInstBoxHead.loss at config A: 2 x 800x1024, 8 GT per image, 80 classes, five '
                                      'FCOS levels, forward + backward to cls_scores, bbox_preds and centernesses',
                rounds=args.rounds, bytes=algorithmic_bytes(leaves))
     for name, fn in fns.items():
-        res[name] = dict(median_ms=statistics.median(times[name]), min_ms=min(times[name]), max_ms=max(times[name]),
-                         launches=launches(fn), host_syncs=syncs(fn))
-    res['new']['graph_replay_ms'] = graph_replay_ms(fns['new'])
+        res[name] = dict(**ms_summary(times[name]), launches=launches(fn), host_syncs=syncs(fn))
+    res['new']['graph_replay_ms'] = replay_ms(capture(fns['new']), 200)
     res['speedup_median_eager'] = res['ref']['median_ms'] / res['new']['median_ms']
     text = json.dumps(res, indent=1)
     print(text)

@@ -22,10 +22,7 @@ same run.  Prints one JSON document; `--out PATH` also writes it.
 import argparse
 import json
 import os
-import statistics
-import subprocess
 import sys
-import warnings
 
 import numpy as np
 import torch
@@ -33,16 +30,12 @@ import torch.nn.functional as F
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
+from benchkit import card, ms_summary, peak_alloc, profile, syncs, time_call  # noqa: E402
 from oracle import condinst_infer as oci  # noqa: E402
 
 HBM = 3.35e12
 SOI = [64, 128, 256, 512, 1024]
 KERNELS = ('ci_key_kernel', 'ci_decode_kernel', 'nms_mask_kernel', 'nms_resolve_kernel', 'ci_gather_kernel', 'ci_paste_kernel')
-
-
-def card():
-    q = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit', '--format=csv,noheader'], capture_output=True, text=True)
-    return {'torch_name': torch.cuda.get_device_name(0), 'nvidia_smi': q.stdout.strip().splitlines()[:1]}
 
 
 def _tv_nms(boxes, scores, iou_threshold, stable=True):
@@ -76,35 +69,6 @@ def new_arm(box_head, mask_head, cls, bbox, ctr, prm, feat, metas):
     dets = box_head.get_bboxes(cls, bbox, ctr, prm, metas, rescale=True)
     segm = mask_head.simple_test(feat, *[[d[i] for d in dets] for i in (1, 2, 3, 4)], metas, 80, rescale=True)
     return dets, segm
-
-
-def time_call(fn):
-    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    a.record()
-    out = fn()
-    b.record()
-    torch.cuda.synchronize()
-    return a.elapsed_time(b), out
-
-
-def count_syncs(fn):
-    torch.cuda.synchronize()
-    with warnings.catch_warnings(record=True) as rec:
-        warnings.simplefilter('always')
-        torch.cuda.set_sync_debug_mode('warn')
-        try:
-            fn()
-        finally:
-            torch.cuda.set_sync_debug_mode('default')
-    return sum('called a synchronizing' in str(r.message) for r in rec)
-
-
-def profile(fn):
-    from torch.profiler import ProfilerActivity, profile as prof
-    with prof(activities=[ProfilerActivity.CUDA]) as p:
-        fn()
-        torch.cuda.synchronize()
-    return {e.key: (e.count, e.device_time_total / 1e3) for e in p.key_averages() if e.device_type.name == 'CUDA' and e.count}
 
 
 def kernel_bytes(box_head, cls, bbox, ctr, prm, metas, dets, B):
@@ -154,14 +118,10 @@ def main():
                     t[k].append(time_call(f)[0])
             rec = {}
             for k, f in fns.items():
-                torch.cuda.synchronize()
-                torch.cuda.reset_peak_memory_stats()
-                base = torch.cuda.memory_allocated()
-                _, out = time_call(f)
-                peak = torch.cuda.max_memory_allocated() - base
+                peak, out = peak_alloc(f)
                 kern = profile(f)
-                rec[k] = {'median_ms': statistics.median(t[k]), 'min_ms': min(t[k]), 'max_ms': max(t[k]),
-                          'launches': sum(c for c, _ in kern.values()), 'syncs': count_syncs(f), 'peak_bytes': peak,
+                rec[k] = {**ms_summary(t[k]), 'launches': sum(c for c, _ in kern.values()), 'syncs': syncs(f),
+                          'peak_bytes': peak,
                           'detections': [len(d[0]) for d in out[0]]}
                 if k == 'new':
                     need = kernel_bytes(box_head, *inputs[:4], inputs[5], out[0], B)

@@ -19,7 +19,8 @@ import os
 import statistics
 import subprocess
 import sys
-import time
+
+from benchkit import capture, card, host_ms, launches, replay_ms
 
 DEV = 'cuda:0'
 NS = (4, 16, 32)
@@ -53,7 +54,6 @@ def inputs(torch, n, seed, B=2, C=128, H=200, W=336):
 def worker(tree, iters):
     sys.path.insert(0, os.path.abspath(tree))
     import torch
-    from torch.profiler import ProfilerActivity, profile
     from boxinstseg_b200.models import build_head
     out = {}
     for n in NS:
@@ -63,49 +63,18 @@ def worker(tree, iters):
         with torch.no_grad():
             for _ in range(8):                                       # fills the bank: >= 5 similar objects per class
                 call()
-            torch.cuda.synchronize()
-            times = []
-            for _ in range(iters):
-                t0 = time.perf_counter()
-                call()
-                torch.cuda.synchronize()
-                times.append(time.perf_counter() - t0)
-            with profile(activities=[ProfilerActivity.CUDA]) as prof:
-                call()
-                torch.cuda.synchronize()
-            launches = sum(1 for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA)
+            times = [host_ms(call)[0] for _ in range(iters)]
+            n_launches = launches(call)
             graph_ms = None
             if not hasattr(head.corr, 'levels_masked'):               # a tree whose loss synchronises: no capture
-                out[n] = dict(eager_ms=statistics.median(times) * 1e3, graph_ms=None, launches=launches)
+                out[n] = dict(eager_ms=statistics.median(times), graph_ms=None, launches=n_launches)
                 continue
             try:
-                g = torch.cuda.CUDAGraph()
-                side = torch.cuda.Stream()
-                side.wait_stream(torch.cuda.current_stream())
-                with torch.cuda.stream(side):
-                    call()
-                torch.cuda.current_stream().wait_stream(side)
-                with torch.cuda.graph(g):
-                    call()
-                g.replay()
-                torch.cuda.synchronize()
-                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-                e0.record()
-                for _ in range(iters):
-                    g.replay()
-                e1.record()
-                torch.cuda.synchronize()
-                graph_ms = e0.elapsed_time(e1) / iters
+                graph_ms = replay_ms(capture(call), iters)
             except Exception as exc:                                  # a host synchronisation inside the call
-                graph_ms = None
                 out.setdefault('graph_error', str(exc).splitlines()[0][:200])
-        out[n] = dict(eager_ms=statistics.median(times) * 1e3, graph_ms=graph_ms, launches=launches)
+        out[n] = dict(eager_ms=statistics.median(times), graph_ms=graph_ms, launches=n_launches)
     print(json.dumps(out))
-
-
-def card():
-    q = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit', '--format=csv,noheader'], capture_output=True, text=True)
-    return q.stdout.strip().splitlines()[:1]
 
 
 def main():

@@ -16,20 +16,14 @@ import argparse
 import json
 import os
 import statistics
-import subprocess
 import sys
-import time
 
 import torch
 
 sys.path.insert(0, '.')
+from benchkit import capture, card, host_ms, kernel_launches, replay_ms, summary  # noqa: E402
 
 DEV = 'cuda:0'
-
-
-def card():
-    q = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit', '--format=csv,noheader'], capture_output=True, text=True)
-    return {'torch_name': torch.cuda.get_device_name(0), 'nvidia_smi': q.stdout.strip().splitlines()[:1]}
 
 
 def make_step(arm, dt):
@@ -59,57 +53,6 @@ def make_step(arm, dt):
     return step
 
 
-def host_ms(step, iters):
-    ts = []
-    for _ in range(iters):
-        torch.cuda.synchronize()
-        t0 = time.perf_counter()
-        step()
-        torch.cuda.synchronize()
-        ts.append((time.perf_counter() - t0) * 1e3)
-    return statistics.median(ts)
-
-
-def make_graph(step):
-    side = torch.cuda.Stream()
-    side.wait_stream(torch.cuda.current_stream())
-    with torch.cuda.stream(side):
-        for _ in range(2):
-            step()
-    torch.cuda.current_stream().wait_stream(side)
-    graph = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(graph):
-        step()
-    graph.replay()
-    torch.cuda.synchronize()
-    return graph
-
-
-def graph_ms(graph, iters):
-    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    a.record()
-    for _ in range(iters):
-        graph.replay()
-    b.record()
-    torch.cuda.synchronize()
-    return a.elapsed_time(b) / iters
-
-
-def launches(step):
-    step()
-    torch.cuda.synchronize()
-    with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
-        step()
-        torch.cuda.synchronize()
-    kern = [e for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA and 'Memcpy' not in e.name
-            and 'Memset' not in e.name]
-    return len(kern)
-
-
-def summary(xs):
-    return {'median': statistics.median(xs), 'min': min(xs), 'max': max(xs), 'all': xs}
-
-
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument('--rounds', type=int, default=5)
@@ -121,16 +64,18 @@ def main():
     for dt in (torch.float16, torch.bfloat16):
         name = str(dt).replace('torch.', '')
         arms = {arm: make_step(arm, dt) for arm in ('new', 'eager', 'fp32')}
-        graphs = {arm: make_graph(s) for arm, s in arms.items()}
+        graphs = {arm: capture(s) for arm, s in arms.items()}
         for s in arms.values():
-            host_ms(s, 3)
+            for _ in range(3):
+                s()
         host = {a: [] for a in arms}
         gpu = {a: [] for a in arms}
         for _ in range(args.rounds):                      # alternate the arms within the call
             for arm, s in arms.items():
-                host[arm].append(host_ms(s, args.iters))
-                gpu[arm].append(graph_ms(graphs[arm], args.iters))
-        r = {arm: {'eager_step_ms': summary(host[arm]), 'graph_step_ms': summary(gpu[arm]), 'launches': launches(s)}
+                host[arm].append(statistics.median(host_ms(s)[0] for _ in range(args.iters)))
+                gpu[arm].append(replay_ms(graphs[arm], args.iters))
+        r = {arm: {'eager_step_ms': summary(host[arm]), 'graph_step_ms': summary(gpu[arm]),
+                   'launches': kernel_launches(s)}
              for arm, s in arms.items()}
         res[name] = r
         for arm in arms:

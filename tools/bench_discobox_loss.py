@@ -19,7 +19,6 @@ against one call per (level, image); and the card's name and power limit read in
 import argparse
 import json
 import os
-import statistics
 import sys
 
 import numpy as np
@@ -27,8 +26,7 @@ import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, 'tools'))
-from bench_condinst_box_loss import card, launches, syncs, timed  # noqa: E402
+from benchkit import card, launches, ms_summary, peak_alloc, syncs, time_call  # noqa: E402
 from oracle import discobox_loss as odl  # noqa: E402
 
 DEV = 'cuda:0'
@@ -77,15 +75,6 @@ def arms(head, w):
     return {'ref': ref, 'new': new}
 
 
-def peak_bytes(fn):
-    torch.cuda.synchronize()
-    base = torch.cuda.memory_allocated()
-    torch.cuda.reset_peak_memory_stats()
-    fn()
-    torch.cuda.synchronize()
-    return torch.cuda.max_memory_allocated() - base
-
-
 def conv_alone(head, w, reps=20):
     """GPU time (ms) of the student convolution of every level and image, forward + backward under float16 autocast."""
     from boxinstseg_b200.ops.dynconv import disco_cells_conv
@@ -112,11 +101,10 @@ def conv_alone(head, w, reps=20):
     times = {k: [] for k in fns}
     for r in range(reps):
         for name in (list(fns) if r % 2 == 0 else list(fns)[::-1]):
-            times[name].append(timed(fns[name]))
+            times[name].append(time_call(fns[name])[0])
     rows = sum(int(o.numel()) for lvl in orders for o in lvl)
     return dict(rows=rows, I_pad=max(sum(int(orders[lv][b].numel()) for lv in range(len(GRIDS))) for b in range(B)),
-                **{k: dict(median_ms=statistics.median(v), min_ms=min(v), max_ms=max(v), launches=launches(fns[k]))
-                   for k, v in times.items()})
+                **{k: dict(**ms_summary(v), launches=launches(fns[k])) for k, v in times.items()})
 
 
 def main():
@@ -138,14 +126,14 @@ def main():
     times = {k: [] for k in fns}
     for r in range(args.rounds):                                   # alternate the arms, starting side swapped each round
         for name in (list(fns) if r % 2 == 0 else list(fns)[::-1]):
-            times[name].append(timed(fns[name]))
+            times[name].append(time_call(fns[name])[0])
     res = dict(card=card(), workload='DiscoBoxSOLOv2Head.loss at config C: 2 x 800x1024, mask features [2,256,200,256], '
                                      'grids 40/36/24/16/12, 8 GT per image, 80 classes, float16 autocast, independent '
                                      'teacher, use_loss_ts; forward + backward to cate_preds, s_kernel_preds_raw, s_ins_pred',
                rounds=args.rounds)
     for name, fn in fns.items():
-        res[name] = dict(median_ms=statistics.median(times[name]), min_ms=min(times[name]), max_ms=max(times[name]),
-                         launches=launches(fn), host_syncs=syncs(fn), peak_alloc_bytes=peak_bytes(fn))
+        res[name] = dict(**ms_summary(times[name]), launches=launches(fn), host_syncs=syncs(fn),
+                         peak_alloc_bytes=peak_alloc(fn)[0])
     res['speedup_median_eager'] = res['ref']['median_ms'] / res['new']['median_ms']
     res['student_conv_alone'] = conv_alone(head, w)
     text = json.dumps(res, indent=1)

@@ -8,13 +8,12 @@ Prints one line per case, with the card's name and power limit; `--out PATH` als
 import argparse
 import json
 import os
-import subprocess
 import sys
-import time
 
 import torch
 
 sys.path.insert(0, '.')
+from benchkit import capture, card, host_ms, replay_ms, time_queued  # noqa: E402
 from boxinstseg_b200 import _lib as L  # noqa: E402
 
 DEV = 'cuda:0'
@@ -22,27 +21,16 @@ PEAK = json.load(open('MEASURED_PEAKS.json')).get('hbm_gbs', 3350.0) if os.path.
 HALF = {torch.float16: 0, torch.bfloat16: 1}
 
 
-def timeit(fn, iters=50):
+def l2_cold_us(fn, iters=50):
+    """Median GPU time (µs) of one call queued behind an L2 flush, which also hides the call's launch."""
     for _ in range(5):
         fn()
     flush = torch.empty(256 << 20, dtype=torch.uint8, device=DEV)
     ts = []
     for _ in range(iters):
         flush.zero_()
-        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        a.record()
-        fn()
-        b.record()
-        torch.cuda.synchronize()
-        ts.append(a.elapsed_time(b) * 1e3)
-    ts.sort()
-    return ts[len(ts) // 2]
-
-
-def card():
-    q = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit,clocks.max.sm', '--format=csv,noheader'],
-                       capture_output=True, text=True)
-    return {'torch_name': torch.cuda.get_device_name(0), 'nvidia_smi': q.stdout.strip().splitlines()[:1]}
+        ts.append(time_queued(fn)[0] * 1e3)
+    return sorted(ts)[len(ts) // 2]
 
 
 def case(name, B, C, h, w, I, dt=torch.float32):
@@ -65,17 +53,17 @@ def case(name, B, C, h, w, I, dt=torch.float32):
         fwd = lambda: lib.bxs_dynconv1x1_half_forward(L.ptr(f), L.ptr(k), L.ptr(out), B, C, P, I, d, st)   # noqa: E731
         bwd = lambda a, b: lib.bxs_dynconv1x1_half_backward(L.ptr(f), L.ptr(k), L.ptr(g), a, b, L.ptr(ws), B, C, P, I, d, st)  # noqa: E731
     assert fwd() == 0 and bwd(L.ptr(gf) if I <= 256 else None, L.ptr(gk)) == 0
-    res['fwd_us'] = timeit(fwd)
+    res['fwd_us'] = l2_cold_us(fwd)
     if I <= 256:
-        res['bwd_feat_us'] = timeit(lambda: bwd(L.ptr(gf), None))
-    res['bwd_kernel_us'] = timeit(lambda: bwd(None, L.ptr(gk)))
+        res['bwd_feat_us'] = l2_cold_us(lambda: bwd(L.ptr(gf), None))
+    res['bwd_kernel_us'] = l2_cold_us(lambda: bwd(None, L.ptr(gk)))
     f2, g2 = f.flatten(2), g.flatten(2)
     for tf32 in ((False, True) if dt == torch.float32 else (False,)):
         torch.backends.cuda.matmul.allow_tf32 = tf32
         tag = 'cublas_' + ('tf32' if tf32 else res['dtype'])
-        res[tag + '_fwd_us'] = timeit(lambda: torch.bmm(k, f2))
-        res[tag + '_bwd_feat_us'] = timeit(lambda: torch.bmm(k.transpose(1, 2), g2))
-        res[tag + '_bwd_kernel_us'] = timeit(lambda: torch.bmm(g2, f2.transpose(1, 2)))
+        res[tag + '_fwd_us'] = l2_cold_us(lambda: torch.bmm(k, f2))
+        res[tag + '_bwd_feat_us'] = l2_cold_us(lambda: torch.bmm(k.transpose(1, 2), g2))
+        res[tag + '_bwd_kernel_us'] = l2_cold_us(lambda: torch.bmm(g2, f2.transpose(1, 2)))
     torch.backends.cuda.matmul.allow_tf32 = False
     byts = f.element_size() * (B * C * P + B * I * P + B * I * C)
     for key in ('fwd_us', 'bwd_feat_us', 'bwd_kernel_us'):
@@ -113,43 +101,19 @@ def config_c_step(iters=20):
                 out = dynconv1x1(x.float() if cast_fp32 else x, k[b].t()[None].contiguous())
             torch.autograd.grad(out, [f, k], g[None].to(out.dtype))
 
-    def graph_us(fn, reps=50):
-        """GPU time of one call, replayed from a CUDA graph (the eager legs are bound by the host's launch rate)."""
-        side = torch.cuda.Stream()
-        side.wait_stream(torch.cuda.current_stream())
-        with torch.cuda.stream(side):
-            fn()
-        torch.cuda.current_stream().wait_stream(side)
-        graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(graph):
-            fn()
-        graph.replay()
-        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        a.record()
-        for _ in range(reps):
-            graph.replay()
-        b.record()
-        torch.cuda.synchronize()
-        return a.elapsed_time(b) * 1e3 / reps
-
-    def timed(fn):
+    def median_step_ms(fn):
         for _ in range(3):
             fn()
-        ts = []
-        for _ in range(iters):
-            torch.cuda.synchronize()
-            t0 = time.perf_counter()
-            fn()
-            torch.cuda.synchronize()
-            ts.append((time.perf_counter() - t0) * 1e3)
-        return sorted(ts)[len(ts) // 2]
+        return sorted(host_ms(fn)[0] for _ in range(iters))[iters // 2]
 
     res = {}
     for _ in range(2):                                           # alternate, to see the spread
-        res.setdefault('step_fp32_ms', []).append(timed(lambda: step(d['feat'], False)))
-        res.setdefault('step_autocast_fp16_ms', []).append(timed(lambda: step(feat16, True)))
-        res.setdefault('conv_legs_fp16_native_graph_us', []).append(graph_us(lambda: conv_legs(False)))
-        res.setdefault('conv_legs_fp16_cast_tf32_graph_us', []).append(graph_us(lambda: conv_legs(True)))
+        res.setdefault('step_fp32_ms', []).append(median_step_ms(lambda: step(d['feat'], False)))
+        res.setdefault('step_autocast_fp16_ms', []).append(median_step_ms(lambda: step(feat16, True)))
+        # the eager legs are bound by the host's launch rate: their GPU time comes from a graph replay
+        for tag, cast in (('native', False), ('cast_tf32', True)):
+            graph = capture(lambda: conv_legs(cast))
+            res.setdefault(f'conv_legs_fp16_{tag}_graph_us', []).append(replay_ms(graph, 50) * 1e3)
     print('config_C_step', json.dumps(res), flush=True)
     return res
 

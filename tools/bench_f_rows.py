@@ -10,50 +10,18 @@ import time
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch  # noqa: E402
+from benchkit import graph_us, host_ms, time_call  # noqa: E402
 
 dev = torch.device('cuda:0')
 
 
-def timeit(fn, reps=20, warm=3):
-    for _ in range(warm):
-        fn()
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(reps):
-        fn()
-    e1.record()
-    torch.cuda.synchronize()
-    return e0.elapsed_time(e1) / reps * 1e3      # us
-
-
-def graph_time(fn, reps=20, per_graph=4):
-    try:
-        fn()
-        torch.cuda.synchronize()
-        side = torch.cuda.Stream()
-        side.wait_stream(torch.cuda.current_stream())
-        with torch.cuda.stream(side):
-            fn()
-        torch.cuda.current_stream().wait_stream(side)
-        g = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(g):
-            for _ in range(per_graph):
-                fn()
-        return timeit(g.replay, reps=reps, warm=2) / per_graph
-    except Exception as exc:                     # noqa: BLE001
-        torch.cuda.synchronize()
-        return 'not capturable: ' + str(exc).split('\n')[0][:80]
-
-
-def wall(fn, reps=5):
-    fn()
-    torch.cuda.synchronize()
-    t = time.perf_counter()
-    for _ in range(reps):
-        fn()
-    torch.cuda.synchronize()
-    return (time.perf_counter() - t) / reps * 1e6
+def row(ours, ref, ref_graph=True, **extra):
+    """Eager and graph-replay µs of this package's call and of the reference's composition, then `extra`."""
+    r = dict(us=time_call(ours, reps=20, warmup=3)[0] * 1e3, graph_us=graph_us(ours, 20, per_graph=4),
+             reference_eager_us=time_call(ref, reps=5, warmup=3)[0] * 1e3)
+    if ref_graph:
+        r['reference_graph_us'] = graph_us(ref, 5)
+    return dict(r, **extra)
 
 
 res = {}
@@ -69,8 +37,7 @@ head = build_head(dict(type='CondInstBoxHead', num_classes=80, in_channels=256, 
                        strides=CFG['strides']))
 ours = lambda: head.get_targets(pts, bx, lb)
 ref = lambda: oft.get_targets(pts, [b.clone() for b in bx], [l.clone() for l in lb], CFG['regress_ranges'], CFG['strides'], 80)
-res['fcos_targets_A'] = dict(us=timeit(ours), graph_us=graph_time(ours), reference_eager_us=timeit(ref, reps=5),
-                             locations=2 * 17064, out_mb=2 * 17064 * 32 / 1e6)
+res['fcos_targets_A'] = row(ours, ref, ref_graph=False, locations=2 * 17064, out_mb=2 * 17064 * 32 / 1e6)
 
 # ---- f2: DiscoBox SOLO targets (the reference: host loops + cv2 per ground truth) ---------------------------------------
 from boxinstseg_b200.models.dense_heads.disco_targets import disco_target_single  # noqa: E402
@@ -87,7 +54,9 @@ for best in (False, True):
     for _ in range(2):
         ost.disco_target_single(dbox, dlab, dmask, fsize, best=best, **big)
     host = (time.perf_counter() - t0) / 2 * 1e6
-    res['disco_targets_best' if best else 'disco_targets'] = dict(wall_us=wall(ours), reference_host_loop_us=host, gts=12,
+    ours()
+    wall_us = host_ms(lambda: [ours() for _ in range(5)])[0] * 1e3 / 5
+    res['disco_targets_best' if best else 'disco_targets'] = dict(wall_us=wall_us, reference_host_loop_us=host, gts=12,
                                                                   mask='800x1024')
 
 # ---- f4: SemanticCorrSolver.solve + transfer -------------------------------------------------------------------------------
@@ -104,16 +73,12 @@ oc.window_mask = lambda h, w, dk: win                      # the reference build
 ours = lambda: s.votes(Cu, FEAT, FEAT)
 ref = lambda: oc.solve_votes(Cu, FEAT, FEAT, SOLVER['dist_kernel'], SOLVER['num_iter'], SOLVER['num_smooth_iter'])
 T = ours()
-res['corr_solve_K5_7x7_10it'] = dict(us=timeit(ours), graph_us=graph_time(ours), reference_eager_us=timeit(ref, reps=5),
-                                     reference_graph_us=graph_time(ref, reps=5, per_graph=1),
-                                     max_abs_diff=float((T - ref()).abs().max()))
+res['corr_solve_K5_7x7_10it'] = row(ours, ref, max_abs_diff=float((T - ref()).abs().max()))
 ours = lambda: s.transfer(T, Cu, m0, m1, FEAT, FEAT)
 ref = lambda: oc.transfer(T, Cu, m0, m1, FEAT, FEAT)
 fg, bg = ours()
 _, rfg, rbg = ref()
-res['corr_transfer_K5_28x28'] = dict(us=timeit(ours), graph_us=graph_time(ours), reference_eager_us=timeit(ref, reps=5),
-                                     reference_graph_us=graph_time(ref, reps=5, per_graph=1),
-                                     reference_intermediates_mb=6 * 5 * 784 * 784 * 4 / 1e6,
+res['corr_transfer_K5_28x28'] = row(ours, ref, reference_intermediates_mb=6 * 5 * 784 * 784 * 4 / 1e6,
                                      max_abs_diff=float(max((fg - rfg).abs().max(), (bg - rbg).abs().max())))
 oc.window_mask = oc_window
 print(json.dumps({k: {kk: (round(vv, 2) if isinstance(vv, float) else vv) for kk, vv in v.items()} for k, v in res.items()}, indent=1))

@@ -13,25 +13,18 @@ Prints one line per G, with the card's name and power limit; `--out PATH` also w
 import argparse
 import json
 import os
-import subprocess
 import sys
-import time
 
 import torch
 from scipy.optimize import linear_sum_assignment as scipy_lsa
 
 sys.path.insert(0, '.')
+from benchkit import card, host_ms, time_call  # noqa: E402
 from boxinstseg_b200.core import MaskHungarianAssigner  # noqa: E402
 from boxinstseg_b200.ops.lsap import solve_batched  # noqa: E402
 
 DEV = 'cuda:0'
 LAYERS, B, Q = 10, 2, 100
-
-
-def card():
-    q = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit,clocks.max.sm', '--format=csv,noheader'],
-                       capture_output=True, text=True)
-    return {'torch_name': torch.cuda.get_device_name(0), 'nvidia_smi': q.stdout.strip().splitlines()[:1]}
 
 
 def costs_for(G, seed):
@@ -70,32 +63,11 @@ def kernel_step(costs):
     return [solve_batched(layer) for layer in costs]
 
 
-def host_ms(fn, costs, reps):
+def spread(timer, fn, reps):
+    """(median, min, max) ms of `reps` calls of fn on `timer` (host_ms or time_call), after three untimed calls."""
     for _ in range(3):
-        fn(costs)
-    torch.cuda.synchronize()
-    ts = []
-    for _ in range(reps):
-        t0 = time.perf_counter()
-        fn(costs)
-        torch.cuda.synchronize()
-        ts.append((time.perf_counter() - t0) * 1e3)
-    ts.sort()
-    return ts[len(ts) // 2], ts[0], ts[-1]
-
-
-def event_ms(costs, reps):
-    for _ in range(3):
-        kernel_step(costs)
-    ts = []
-    for _ in range(reps):
-        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        a.record()
-        kernel_step(costs)
-        b.record()
-        torch.cuda.synchronize()
-        ts.append(a.elapsed_time(b))
-    ts.sort()
+        fn()
+    ts = sorted(timer(fn)[0] for _ in range(reps))
     return ts[len(ts) // 2], ts[0], ts[-1]
 
 
@@ -106,9 +78,9 @@ def case(G, reps):
     for (r, k), m in zip(want, got):
         rows = torch.nonzero(m >= 0).squeeze(1)
         assert torch.equal(rows, r) and torch.equal(m[rows].long(), k), 'kernel and scipy disagree'
-    s = host_ms(scipy_step, costs, reps)
-    k = host_ms(kernel_step, costs, reps)
-    e = event_ms(costs, reps)
+    s = spread(host_ms, lambda: scipy_step(costs), reps)
+    k = spread(host_ms, lambda: kernel_step(costs), reps)
+    e = spread(time_call, lambda: kernel_step(costs), reps)
     row = {'G': G, 'problems': LAYERS * B, 'scipy_host_ms': s, 'kernel_host_ms': k, 'kernel_event_ms': e}
     print(f'G={G:3d}  {LAYERS}x{B} matchings of {Q}x{G}: scipy path {s[0]:.3f} ms (min {s[1]:.3f}, max {s[2]:.3f}) | '
           f'kernel host clock {k[0]:.3f} ms (min {k[1]:.3f}, max {k[2]:.3f}) | kernel events {e[0]:.3f} ms '

@@ -9,48 +9,20 @@ import sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch  # noqa: E402
 import torch.nn.functional as F  # noqa: E402
+from benchkit import graph_us, time_call  # noqa: E402
 
 dev = torch.device('cuda:0')
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 PEAK = json.load(open(os.path.join(ROOT, 'MEASURED_PEAKS.json')))['hbm_gbs'] if os.path.exists(os.path.join(ROOT, 'MEASURED_PEAKS.json')) else 3350.0   # H100 SXM data sheet
 
 
-def timeit(fn, reps=20, warm=3):
-    for _ in range(warm):
-        fn()
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(reps):
-        fn()
-    e1.record()
-    torch.cuda.synchronize()
-    return e0.elapsed_time(e1) / reps * 1e3      # us
-
-
-def graph_time(fn, reps=20, per_graph=4):
-    """fn captured `per_graph` times into one CUDA graph, replayed; None when the op cannot be captured."""
-    try:
-        fn()
-        torch.cuda.synchronize()
-        side = torch.cuda.Stream()
-        side.wait_stream(torch.cuda.current_stream())
-        with torch.cuda.stream(side):
-            fn()
-        torch.cuda.current_stream().wait_stream(side)
-        g = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(g):
-            for _ in range(per_graph):
-                fn()
-        return timeit(g.replay, reps=reps, warm=2) / per_graph
-    except Exception as exc:                     # noqa: BLE001
-        torch.cuda.synchronize()
-        return 'not capturable: ' + str(exc).split('\n')[0][:80]
+def eager_us(fn, reps=20, warm=3):
+    return time_call(fn, reps=reps, warmup=warm)[0] * 1e3
 
 
 def both(res, key, fn, reps=20, warm=3):
-    res[key + '_us'] = timeit(fn, reps=reps, warm=warm)
-    res[key + '_graph_us'] = graph_time(fn, reps=max(reps // 2, 3))
+    res[key + '_us'] = eager_us(fn, reps=reps, warm=warm)
+    res[key + '_graph_us'] = graph_us(fn, max(reps // 2, 3), per_graph=4)
 
 
 res = {}
@@ -65,13 +37,13 @@ for name, (B, C, h, w, I) in dict(box2mask_E=(1, 256, 256, 256, 100), discobox_C
     def run():
         it[0] += 1
         return dynconv1x1(feats[it[0] % 4], kern)
-    us = timeit(run)
+    us = eager_us(run)
     byts = B * (C * h * w * 4 + I * h * w * 4 + I * C * 4)
     flops = 2.0 * B * I * C * h * w
     entry = dict(us=us, algo_mb=byts / 1e6, gbs=byts / us / 1e3, frac_hbm=byts / us / 1e3 / PEAK, tflops=flops / us / 1e6)
     for tf32 in (False, True):
         torch.backends.cuda.matmul.allow_tf32 = tf32
-        entry['cublas_tf32_us' if tf32 else 'cublas_fp32_us'] = timeit(
+        entry['cublas_tf32_us' if tf32 else 'cublas_fp32_us'] = eager_us(
             lambda: torch.bmm(kern, feats[it[0] % 4].flatten(2)))
     torch.backends.cuda.matmul.allow_tf32 = False
     res['dynconv_' + name] = entry
@@ -96,12 +68,13 @@ for name, (n, h, w) in dict(levelset_D_200x256=(16, 200, 256), box2mask_E_96x96=
     guide = F.interpolate(torch.randn(n, 3, h // 8, w // 8, device=dev, generator=g), size=(h, w), mode='bilinear') + \
         0.05 * torch.randn(n, 3, h, w, device=dev, generator=g)
     feat1 = torch.rand(n, 1, h, w, device=dev, generator=g).requires_grad_(True)
-    res[f'mst_{name}_us'] = timeit(lambda: mst(guide), reps=5, warm=1)
+    res[f'mst_{name}_us'] = eager_us(lambda: mst(guide), reps=5, warm=1)
     tree = mst(guide)
-    res[f'bfs_{name}_us'] = timeit(lambda: bfs(tree, 4), reps=5, warm=1)
-    res[f'treefilter_fwd_{name}_us'] = timeit(lambda: tf(feat1, guide, tree), reps=5, warm=1)
+    res[f'bfs_{name}_us'] = eager_us(lambda: bfs(tree, 4), reps=5, warm=1)
+    res[f'treefilter_fwd_{name}_us'] = eager_us(lambda: tf(feat1, guide, tree), reps=5, warm=1)
     o = tf(feat1, guide, tree, low_tree=False)
-    res[f'treefilter_bwd_{name}_us'] = timeit(lambda: torch.autograd.grad(o.sum(), feat1, retain_graph=True), reps=5, warm=1)
+    res[f'treefilter_bwd_{name}_us'] = eager_us(lambda: torch.autograd.grad(o.sum(), feat1, retain_graph=True),
+                                                reps=5, warm=1)
     res[f'tree_levels_{name}'] = int(bfs_order(tree, 4).num_levels.max())
 
 from boxinstseg_b200.models.losses import LCM, LevelsetLoss, projection_losses  # noqa: E402

@@ -17,16 +17,14 @@ limit read in the same run.  Prints one JSON document; `--out PATH` also writes 
 import argparse
 import json
 import os
-import statistics
-import subprocess
 import sys
-import warnings
 
 import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 from bench_configs import HP, WP, _image_and_boxes  # noqa: E402
+from benchkit import card, launches, ms_summary, peak_alloc, syncs, time_call  # noqa: E402
 from oracle import solo_head as osh  # noqa: E402
 
 DEV = 'cuda:0'
@@ -34,11 +32,6 @@ HEAD = dict(type='BoxSOLOv2Head', num_classes=80, in_channels=256, seg_feat_chan
             strides=[8, 8, 16, 32, 32], scale_ranges=((1, 96), (48, 192), (96, 384), (192, 768), (384, 2048)), sigma=0.2,
             num_grids=[40, 36, 24, 16, 12], cate_down_pos=0,
             loss_cate=dict(type='FocalLoss', use_sigmoid=True, gamma=2.0, alpha=0.25, loss_weight=1.0))
-
-
-def card():
-    q = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit', '--format=csv,noheader'], capture_output=True, text=True)
-    return {'torch_name': torch.cuda.get_device_name(0), 'nvidia_smi': q.stdout.strip().splitlines()[:1]}
 
 
 def workload(seed=0):
@@ -74,39 +67,6 @@ def arms(head, feats, img, boxes, labels, masks):
     return {'ref': ref, 'new': new}
 
 
-def timed(fn):
-    torch.cuda.synchronize()
-    torch.cuda.reset_peak_memory_stats()
-    base = torch.cuda.memory_allocated()
-    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    a.record()
-    fn()
-    b.record()
-    torch.cuda.synchronize()
-    return a.elapsed_time(b), torch.cuda.max_memory_allocated() - base
-
-
-def syncs(fn):
-    torch.cuda.synchronize()
-    with warnings.catch_warnings(record=True) as seen:
-        warnings.simplefilter('always')
-        torch.cuda.set_sync_debug_mode('warn')
-        try:
-            fn()
-        finally:
-            torch.cuda.set_sync_debug_mode(0)
-    return sum('synchroniz' in str(w.message) for w in seen)
-
-
-def launches(fn):
-    from torch.profiler import ProfilerActivity, profile
-    torch.cuda.synchronize()
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        fn()
-        torch.cuda.synchronize()
-    return sum(1 for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA)
-
-
 def focal_alone(head, feats, reps=50):
     from boxinstseg_b200.ops.focal import sigmoid_focal_loss_levels
     with torch.no_grad():
@@ -128,8 +88,8 @@ def focal_alone(head, feats, reps=50):
     for name, fn in (('kernel', kernel), ('torch_lines', torch_lines)):
         for _ in range(5):
             fn()
-        ts = [timed(fn)[0] for _ in range(reps)]
-        out[name] = dict(median_ms=statistics.median(ts), min_ms=min(ts), max_ms=max(ts), launches=launches(fn))
+        ts = [time_call(fn)[0] for _ in range(reps)]
+        out[name] = dict(**ms_summary(ts), launches=launches(fn))
     out['bytes'] = dict(logits=sum(c.numel() * 4 for c in cate), grad=sum(c.numel() * 4 for c in cate))
     return out
 
@@ -150,14 +110,14 @@ def main():
     times, peaks = {k: [] for k in fns}, {k: 0 for k in fns}
     for r in range(args.rounds):                                   # alternate the arms, starting side swapped each round
         for name in (list(fns) if r % 2 == 0 else list(fns)[::-1]):
-            t, p = timed(fns[name])
+            p, t = peak_alloc(lambda: time_call(fns[name])[0])
             times[name].append(t)
             peaks[name] = max(peaks[name], p)
     res = dict(card=card(), workload='BoxSOLOv2 head step at config D: 2 x 800x1024, 8 GT / image, 256-channel stand-in towers, '
                                      'forward + backward to every parameter and the FPN inputs', rounds=args.rounds)
     for name, fn in fns.items():
-        res[name] = dict(median_ms=statistics.median(times[name]), min_ms=min(times[name]), max_ms=max(times[name]),
-                         peak_alloc_bytes=peaks[name], launches=launches(fn), host_syncs=syncs(fn))
+        res[name] = dict(**ms_summary(times[name]), peak_alloc_bytes=peaks[name], launches=launches(fn),
+                         host_syncs=syncs(fn))
     res['speedup_median'] = res['ref']['median_ms'] / res['new']['median_ms']
     res['focal'] = focal_alone(case[0], case[1])
     text = json.dumps(res, indent=1)

@@ -17,16 +17,14 @@ below; the card's name and power limit are read in the same run.  Prints one JSO
 import argparse
 import json
 import os
-import statistics
-import subprocess
 import sys
 import types
-import warnings
 
 import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
+from benchkit import card, ms_summary, peak_alloc, profile, syncs, time_call  # noqa: E402
 from oracle import solo_seg as oss  # noqa: E402
 
 DEV = 'cuda:0'
@@ -34,11 +32,6 @@ GRIDS, STRIDES = [40, 36, 24, 16, 12], [8, 8, 16, 32, 32]
 H, W, C, E = 200, 336, 80, 256
 META = dict(img_shape=(800, 1067, 3), ori_shape=(480, 640, 3), pad_shape=(800, 1344, 3))
 HBM = 3.35e12
-
-
-def card():
-    q = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit', '--format=csv,noheader'], capture_output=True, text=True)
-    return {'torch_name': torch.cuda.get_device_name(0), 'nvidia_smi': q.stdout.strip().splitlines()[:1]}
 
 
 def _cate(gen, B, K):
@@ -116,39 +109,6 @@ def oss_cfg(c):
     return types.SimpleNamespace(**c)
 
 
-def time_call(fn):
-    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    a.record()
-    out = fn()
-    b.record()
-    torch.cuda.synchronize()
-    return a.elapsed_time(b), out
-
-
-def count_syncs(fn):
-    torch.cuda.synchronize()
-    with warnings.catch_warnings(record=True) as rec:
-        warnings.simplefilter('always')
-        torch.cuda.set_sync_debug_mode('warn')
-        try:
-            fn()
-        finally:
-            torch.cuda.set_sync_debug_mode('default')
-    return sum('synchroniz' in str(r.message) for r in rec)
-
-
-def profile(fn):
-    from torch.profiler import ProfilerActivity, profile as prof
-    with prof(activities=[ProfilerActivity.CUDA]) as p:
-        fn()
-        torch.cuda.synchronize()
-    kernels = {}
-    for e in p.key_averages():
-        if e.device_type.name == 'CUDA' and e.count:
-            kernels[e.key] = (e.count, e.device_time_total / 1e3)
-    return kernels
-
-
 def hbm_bytes(cate, thr, out, disco):
     """Algorithmic HBM bytes of the new arm's kernels: the stats kernel reads every distinct candidate row once (float32
     probabilities, or float16 logits for DiscoBox) and writes its packed bits; the paste writes n x H_ori x W_ori bytes (its
@@ -178,13 +138,10 @@ def main():
                     t[k].append(time_call(f)[0])
             rec = {}
             for k, f in fns.items():
-                torch.cuda.reset_peak_memory_stats()
-                base = torch.cuda.memory_allocated()
-                _, out = time_call(f)
-                peak = torch.cuda.max_memory_allocated() - base
+                peak, out = peak_alloc(f)
                 kern = profile(f)
-                rec[k] = {'median_ms': statistics.median(t[k]), 'min_ms': min(t[k]), 'max_ms': max(t[k]),
-                          'launches': sum(c for c, _ in kern.values()), 'syncs': count_syncs(f), 'peak_bytes': peak,
+                rec[k] = {**ms_summary(t[k]), 'launches': sum(c for c, _ in kern.values()), 'syncs': syncs(f),
+                          'peak_bytes': peak,
                           'instances': [len(r.scores) for r in out]}
                 if k == 'new':
                     hbm = hbm_bytes(cate, cfg(disco)['score_thr'], out, disco)

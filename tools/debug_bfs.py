@@ -3,19 +3,14 @@ import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
 import torch.nn.functional as F
+from benchkit import time_call
 from boxinstseg_b200 import _lib as L
 from boxinstseg_b200.ops.tree_filter import MinimumSpanningTree, TreeFilter2D, bfs
 from boxinstseg_b200.ops.tree_filter import tree_filter_cuda as C
 dev = torch.device('cuda:0')
 lib = L.lib()
 g = torch.Generator(device=dev).manual_seed(0)
-def timeit(fn, reps=5):
-    fn(); torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(reps): fn()
-    e1.record(); torch.cuda.synchronize()
-    return e0.elapsed_time(e1) / reps * 1e3
+us = lambda fn: time_call(fn, reps=5, warmup=1)[0] * 1e3  # noqa: E731
 for (n, h, w) in [(2, 200, 256), (16, 200, 256), (2, 96, 96), (2, 50, 64)]:
     guide = F.interpolate(torch.randn(n, 3, h // 8, w // 8, device=dev, generator=g), size=(h, w), mode='bilinear') + 0.05 * torch.randn(n, 3, h, w, device=dev, generator=g)
     mst = MinimumSpanningTree(TreeFilter2D.norm2_distance)
@@ -34,7 +29,7 @@ for (n, h, w) in [(2, 200, 256), (16, 200, 256), (2, 96, 96), (2, 50, 64)]:
     flags = ws[off:off + 4 * B].view(torch.int32)
     print(f'{n}x{h}x{w}: rc={rc} flags={flags.tolist()} levels={nlv.tolist()[:4]}', flush=True)
     print('  ',
-          f'bfs {timeit(lambda: bfs(tree, 4)):.0f} us  mst {timeit(lambda: mst(guide)):.0f} us')
+          f'bfs {us(lambda: bfs(tree, 4)):.0f} us  mst {us(lambda: mst(guide)):.0f} us')
     tf = TreeFilter2D()
     feat = torch.rand(n, 1, h, w, device=dev, generator=g).requires_grad_(True)
     emb = guide.clone().requires_grad_(True)
@@ -45,4 +40,4 @@ for (n, h, w) in [(2, 200, 256), (16, 200, 256), (2, 96, 96), (2, 50, 64)]:
     def fb():
         ew = tf.build_edge_weight(emb, idx, par, False, chd)
         return torch.autograd.grad(refine(f3, ew, idx, par, chd, False).sum(), [feat, emb])
-    print('   refine fwd', f'{timeit(lambda: refine(f3.detach(), ew0, idx, par, chd, False)):.0f} us', 'fwd+bwd', f'{timeit(fb):.0f} us', flush=True)
+    print('   refine fwd', f'{us(lambda: refine(f3.detach(), ew0, idx, par, chd, False)):.0f} us', 'fwd+bwd', f'{us(fb):.0f} us', flush=True)

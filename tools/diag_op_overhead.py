@@ -3,6 +3,7 @@ import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
 from bench import synthetic_case, N_INST, H, W
+from benchkit import capture, replay_ms
 from boxinstseg_b200 import _lib as L
 from boxinstseg_b200.ops import boxinst as OB
 from boxinstseg_b200.ops.boxinst import boxinst_mask_loss, boxinst_targets
@@ -61,20 +62,8 @@ def v_raw_fresh(x):           # raw calls but with per-step torch.empty buffers 
 
 def measure(fn, name):
     keep.clear()
-    side = torch.cuda.Stream(); side.wait_stream(torch.cuda.current_stream())
-    with torch.cuda.stream(side):
-        for x in xs: fn(x)
-    torch.cuda.current_stream().wait_stream(side); torch.cuda.synchronize()
-    keep.clear()
-    g = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(g):
-        for x in xs: fn(x)
-    g.replay(); torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(50): g.replay()
-    e1.record(); torch.cuda.synchronize()
-    print(f'{name:28s} {e0.elapsed_time(e1) / 50 / R * 1e3:7.2f} us/step', flush=True)
+    g = capture(lambda: [fn(x) for x in xs])
+    print(f'{name:28s} {replay_ms(g, 50) / R * 1e3:7.2f} us/step', flush=True)
 
 for fn, name in [(v_raw, 'raw C ABI'), (v_raw_fresh, 'raw, fresh buffers per step'), (v_fwd_only, 'op forward only'),
                  (v_full, 'op + autograd.backward'), (v_grad, 'op + autograd.grad'), (v_sum_backward, 'op + (prj+pair).backward()')]:

@@ -3,28 +3,11 @@ import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
 import bench_configs as bc
+from benchkit import capture, replay_ms
 dev = torch.device('cuda:0')
 for levels in ([(200, 256)], [(200, 256), (200, 256)], [(100, 128)], [(50, 64)], bc.LEVELS_D):
     bc.LEVELS_D = list(levels)
     step, info = bc.build_D(dev, 1234)
     for _ in range(2):
         step()
-    torch.cuda.synchronize()
-    side = torch.cuda.Stream()
-    side.wait_stream(torch.cuda.current_stream())
-    with torch.cuda.stream(side):
-        step()
-    torch.cuda.current_stream().wait_stream(side)
-    g = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(g):
-        step()
-    for _ in range(3):
-        g.replay()
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(10):
-        g.replay()
-    e1.record()
-    torch.cuda.synchronize()
-    print(levels, f'{e0.elapsed_time(e1) / 10:.3f} ms per step', flush=True)
+    print(levels, f'{replay_ms(capture(step), 10):.3f} ms per step', flush=True)

@@ -3,6 +3,7 @@
       python tools/quick_corr_check.py"""
 import numpy as np, torch, sys
 sys.path.insert(0, '.')
+from benchkit import graph_us
 from boxinstseg_b200.models.dense_heads.disco_corr import SemanticCorrSolver
 from oracle.make_golden_corr import SOLVER, FEAT
 g = np.load('tests/golden/corr.npz')
@@ -15,14 +16,4 @@ for seed in (0, 1, 2):
     ref = g[f's{seed}_T']
     worst = max(worst, float(np.abs(T.cpu().numpy() - ref).max() / np.abs(ref).max()))
 print('solve vs reference golden, max scaled diff:', worst)
-fn = lambda: s.votes(Cu, FEAT, FEAT)
-fn(); torch.cuda.synchronize()
-gr = torch.cuda.CUDAGraph()
-with torch.cuda.graph(gr):
-    for _ in range(4): fn()
-e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-gr.replay(); torch.cuda.synchronize()
-e0.record()
-for _ in range(20): gr.replay()
-e1.record(); torch.cuda.synchronize()
-print('corr_solve graph us:', e0.elapsed_time(e1) / 80 * 1e3)
+print('corr_solve graph us:', graph_us(lambda: s.votes(Cu, FEAT, FEAT), 20, per_graph=4))
