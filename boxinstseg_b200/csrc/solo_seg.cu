@@ -15,6 +15,8 @@
 //           threshold.  The [n, 4h, 4w] intermediate of the reference never exists.
 //   maskformer paste: the same per-pixel function (paste_value) on Box2Mask's logit rows, with a first stage of any size
 //           and stages that may be skipped, plus each mask's area, masked sum and box folded in the pass that writes it.
+//   extents: each mask's set-pixel count and box from bool / uint8 masks (16-byte row loads where W and the base allow),
+//           per-CTA partials reduced as the maskformer paste reduces its own.
 #include <cuda_fp16.h>
 
 #include <type_traits>
@@ -228,17 +230,35 @@ __global__ void __launch_bounds__(SS_NT) solo_paste_kernel(RowSources src, const
   }
 }
 
+// A CTA's MaskStats -> *out, written by thread 0: lanes by the butterfly, warps in index order, so that the float64 sum is
+// the same from run to run.  Every thread of the CTA calls it.
+__device__ __forceinline__ void mask_stats_cta_partial(MaskStats st, MaskStats* s_part, MaskStats* out) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  st.sum = warp_sum(st.sum);
+  st.area = __reduce_add_sync(kFull, st.area);
+  st.x0 = __reduce_min_sync(kFull, st.x0);
+  st.y0 = __reduce_min_sync(kFull, st.y0);
+  st.x1 = __reduce_max_sync(kFull, st.x1);
+  st.y1 = __reduce_max_sync(kFull, st.y1);
+  if (lane == 0) s_part[warp] = st;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    MaskStats s = s_part[0];
+    for (int i = 1; i < SS_NT / kWarp; ++i) mask_stats_merge(s, s_part[i]);
+    *out = s;
+  }
+  __syncthreads();
+}
+
 // MaskFormer's instance masks (maskformer_fusion_head.py:112-241 after box2mask_head.py:445-459): the same per-pixel paste
 // of logit rows, thresholded at 0, a float16 row rounded after each stage; each CTA also folds its set pixels into a
-// MaskStats (sigmoid as torch computes it for T) and writes it to part[k * gridDim.x + blockIdx.x], reduced in a fixed order
-// (lanes by the butterfly, warps in index order) so that the float64 sum is the same from run to run.
+// MaskStats (sigmoid as torch computes it for T) and writes it to part[k * gridDim.x + blockIdx.x].
 template <typename T>
 __global__ void __launch_bounds__(SS_NT) maskformer_paste_kernel(RowSources src, const int64_t* __restrict__ rows, int64_t n,
                                                                  PasteGeom g, uint8_t* __restrict__ out,
                                                                  MaskStats* __restrict__ part) {
   constexpr bool kRound = std::is_same<T, __half>::value;
   __shared__ MaskStats s_part[SS_NT / kWarp];
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int64_t npix = (int64_t)g.H_out * g.W_out;
   for (int64_t k = blockIdx.y; k < n; k += gridDim.y) {
     const T* p = row_ptr<T>(src, rows[k], (int64_t)g.h * g.w);
@@ -254,37 +274,77 @@ __global__ void __launch_bounds__(SS_NT) maskformer_paste_kernel(RowSources src,
       o[pix] = on;
       if (on) mask_stats_add(st, y, x, kRound ? prob(__float2half_rn(v), true) : prob(v, true));
     }
-    st.sum = warp_sum(st.sum);
-    st.area = __reduce_add_sync(kFull, st.area);
-    st.x0 = __reduce_min_sync(kFull, st.x0);
-    st.y0 = __reduce_min_sync(kFull, st.y0);
-    st.x1 = __reduce_max_sync(kFull, st.x1);
-    st.y1 = __reduce_max_sync(kFull, st.y1);
-    if (lane == 0) s_part[warp] = st;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      MaskStats s = s_part[0];
-      for (int i = 1; i < SS_NT / kWarp; ++i) mask_stats_merge(s, s_part[i]);
-      part[k * gridDim.x + blockIdx.x] = s;
-    }
-    __syncthreads();
+    mask_stats_cta_partial(st, s_part, part + k * gridDim.x + blockIdx.x);
   }
 }
 
-// the n_part partials of every row, in index order -> area, masked_sum (one float32 rounding), box
-__global__ void __launch_bounds__(SS_NT) maskformer_stats_kernel(const MaskStats* __restrict__ part, int64_t n, int n_part,
-                                                                 int32_t* __restrict__ area, float* __restrict__ masked_sum,
-                                                                 float* __restrict__ box) {
+// the n_part partials of every row, in index order -> area, masked_sum (one float32 rounding; kSum = false: not written),
+// box.  The maskformer paste and the mask extents reduce their partials here.
+template <bool kSum>
+__global__ void __launch_bounds__(SS_NT) mask_stats_reduce_kernel(const MaskStats* __restrict__ part, int64_t n, int n_part,
+                                                                  int32_t* __restrict__ area, float* __restrict__ masked_sum,
+                                                                  float* __restrict__ box) {
   const int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (k >= n) return;
   MaskStats s = part[k * n_part];
   for (int i = 1; i < n_part; ++i) mask_stats_merge(s, part[k * n_part + i]);
   area[k] = s.area;
-  masked_sum[k] = (float)s.sum;
+  if constexpr (kSum) masked_sum[k] = (float)s.sum;
   mask_stats_box(s, box + 4 * k);
 }
 
 constexpr int MF_MAX_PARTS = 64;       // CTAs per row of the maskformer paste: 256-thread CTAs, one partial each
+
+// The set (non-zero) bytes of the 16 bytes q, the first at column x of row y, folded into s.  W % 16 == 0 keeps the 16
+// bytes in one row.  __vcmpne4 gives 0xff per non-zero byte; its low bits, gathered, are a 16-bit mask of the set bytes.
+__device__ __forceinline__ void mask_extents_add16(MaskStats& s, const uint4& q, int y, int x) {
+  const unsigned w[4] = {q.x, q.y, q.z, q.w};
+  unsigned m = 0;
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    const unsigned b = __vcmpne4(w[j], 0u) & 0x01010101u;
+    m |= ((b | (b >> 7) | (b >> 14) | (b >> 21)) & 0xfu) << (4 * j);
+  }
+  if (!m) return;
+  s.area += __popc(m);
+  s.x0 = min(s.x0, x + __ffs(m) - 1);
+  s.x1 = max(s.x1, x + 31 - __clz(m));
+  s.y0 = min(s.y0, y);
+  s.y1 = max(s.y1, y);
+}
+
+// Each CTA folds the set bytes of its share of mask k (its own run of the mask's 16-byte vectors, kVec, or bytes) into
+// a MaskStats and writes it to part[k * gridDim.x + blockIdx.x], as the maskformer paste writes its partials; the sum
+// stays 0.  Integer counts and extents only: the result does not depend on the order of the reduction.
+template <bool kVec>
+__global__ void __launch_bounds__(SS_NT) mask_extents_kernel(const uint8_t* __restrict__ masks, int64_t n, int H, int W,
+                                                             MaskStats* __restrict__ part) {
+  __shared__ MaskStats s_part[SS_NT / kWarp];
+  const int hw = H * W;
+  const int items = kVec ? hw / 16 : hw;
+  const int stride = gridDim.x * SS_NT;
+  for (int64_t k = blockIdx.y; k < n; k += gridDim.y) {
+    const uint8_t* m = masks + k * hw;
+    MaskStats st = mask_stats_empty();
+#pragma unroll 4
+    for (int i = blockIdx.x * SS_NT + threadIdx.x; i < items; i += stride) {
+      if constexpr (kVec) {
+        const int o = 16 * i, y = o / W;
+        mask_extents_add16(st, __ldg(reinterpret_cast<const uint4*>(m) + i), y, o - y * W);
+      } else if (__ldg(m + i)) {
+        const int y = i / W;
+        mask_stats_add(st, y, i - y * W, 0.f);
+      }
+    }
+    mask_stats_cta_partial(st, s_part, part + k * gridDim.x + blockIdx.x);
+  }
+}
+
+// CTAs per mask of mask_extents_kernel: about four vectors (or bytes) per thread, at most MF_MAX_PARTS
+int64_t extents_parts(int64_t H, int64_t W, bool vec) {
+  const int64_t items = vec ? H * W / 16 : H * W;
+  return std::max<int64_t>(1, std::min<int64_t>(ceil_div(items, 4 * SS_NT), MF_MAX_PARTS));
+}
 
 }  // namespace
 }  // namespace bxs
@@ -387,6 +447,29 @@ extern "C" int bxs_maskformer_paste_masks(const void* const* src_host, const int
   auto kern = dtype == 0 ? maskformer_paste_kernel<float> : maskformer_paste_kernel<__half>;
   kern<<<dim3(gx, gy), SS_NT, 0, s>>>(src, rows, n, g, out, part);
   if (int rc = check_launch()) return rc;
-  maskformer_stats_kernel<<<(unsigned)ceil_div(n, SS_NT), SS_NT, 0, s>>>(part, n, (int)gx, area, masked_sum, box);
+  mask_stats_reduce_kernel<true><<<(unsigned)ceil_div(n, SS_NT), SS_NT, 0, s>>>(part, n, (int)gx, area, masked_sum, box);
+  return check_launch();
+}
+
+extern "C" int64_t bxs_mask_extents_workspace_bytes(int64_t n, int64_t H, int64_t W) {
+  if (n <= 0 || H < 0 || W < 0) return 0;
+  return n * extents_parts(H, W, false) * (int64_t)sizeof(MaskStats);      // the byte path's count bounds the vector path's
+}
+
+extern "C" int bxs_mask_extents(const uint8_t* masks, int64_t n, int64_t H, int64_t W, void* workspace, int32_t* area,
+                                float* box, bxs_stream_t stream) {
+  if (n < 0 || H < 0 || W < 0) return BXS_ERR_INVALID_ARG;
+  if (H * W > INT32_MAX) return BXS_ERR_UNSUPPORTED;
+  if (n == 0) return BXS_OK;
+  if ((!masks && H * W > 0) || !workspace || !area || !box) return BXS_ERR_INVALID_ARG;
+  const bool vec = W % 16 == 0 && reinterpret_cast<uintptr_t>(masks) % 16 == 0;
+  const int64_t gx = extents_parts(H, W, vec);
+  const unsigned gy = (unsigned)std::min<int64_t>(n, 65535);
+  MaskStats* part = static_cast<MaskStats*>(workspace);
+  cudaStream_t s = as_stream(stream);
+  auto kern = vec ? mask_extents_kernel<true> : mask_extents_kernel<false>;
+  kern<<<dim3((unsigned)gx, gy), SS_NT, 0, s>>>(masks, n, (int)H, (int)W, part);
+  if (int rc = check_launch()) return rc;
+  mask_stats_reduce_kernel<false><<<(unsigned)ceil_div(n, SS_NT), SS_NT, 0, s>>>(part, n, (int)gx, area, nullptr, box);
   return check_launch();
 }

@@ -1,6 +1,7 @@
 """SOLOv2 inference on the kernels of csrc/solo_seg.cu: per-row mask statistics, Matrix NMS (mmdet/core/post_processing/
 matrix_nms.py) and the fused mask paste of get_seg_single (box_solov2_head.py:576-585, discobox_head.py:1645-1653); and
-Box2Mask's instance masks on the same paste (maskformer_fusion_head.py:112-241), with their statistics.
+Box2Mask's instance masks on the same paste (maskformer_fusion_head.py:112-241), with their statistics; and the area and
+box of finished masks, for the detectors' ``format_results``.
 
 Row sources: the mask rows the kernels read are given as a list of tensors [rows_s, h, w] (float32 or float16, any layout:
 made dense here) and addressed by a row id into their concatenation, so that BoxSOLOv2's per-level [B,S^2,h,w] predictions are
@@ -111,6 +112,26 @@ def maskformer_paste_rows(src, rows, pad_hw, img_hw, ori_hw=None):
                                                    H_out, W_out, L.ptr(ws), L.ptr(out), L.ptr(area), L.ptr(msum),
                                                    L.ptr(box), L.stream()), 'maskformer_paste_masks')
     return out, area, msum, box
+
+
+def mask_extents(masks):
+    """(area int32 [n], box float32 [n, 4]) of bool or uint8 masks [n, H, W]: each mask's count of set (non-zero) pixels and
+    [x_min, y_min, x_max + 1, y_max + 1] of them, zeros for an empty mask.  Two launches, no host read."""
+    if masks.dtype not in (torch.bool, torch.uint8):
+        raise TypeError(f'masks must be bool or uint8, got {masks.dtype}')
+    if masks.dim() != 3:
+        raise ValueError(f'masks must be [n, H, W], got {tuple(masks.shape)}')
+    masks = masks.contiguous()
+    L.require_cuda(masks)
+    n, H, W = masks.shape
+    dev = masks.device
+    area = torch.empty(n, dtype=torch.int32, device=dev)
+    box = torch.empty((n, 4), dtype=torch.float32, device=dev)
+    with torch.cuda.device(dev):
+        ws = torch.empty(L.lib().bxs_mask_extents_workspace_bytes(n, H, W), dtype=torch.uint8, device=dev)
+        L.check(L.lib().bxs_mask_extents(L.ptr(masks), n, H, W, L.ptr(ws), L.ptr(area), L.ptr(box), L.stream()),
+                'mask_extents')
+    return area, box
 
 
 def paste_masks(rows, featmap_size, img_shape, ori_shape, mask_thr):

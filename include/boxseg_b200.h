@@ -726,6 +726,13 @@ int bxs_fcos_loss_backward(float* g_pred, int64_t n_pred, const float* g_loss_bb
  *   sigmoid(v) over them (torch's sigmoid for the dtype, accumulated in float64 in a fixed order, rounded once), box f32
  *   [n,4] = [x_min, y_min, x_max + 1, y_max + 1] of them (mask2bbox), zeros for an empty mask.  h <= H_pad, w <= W_pad,
  *   H_img <= H_pad, W_img <= W_pad.  workspace: bxs_maskformer_paste_workspace_bytes(n) bytes, 8-byte aligned.  Two launches.
+ * bxs_mask_extents (format_results of SingleStageBoxInsDetector / SingleStageWSInsDetector: seg_mask.sum() and the min / max
+ *   of torch.where(seg_mask)): for n masks u8 [n, H, W] (bool or uint8 bytes, dense; any non-zero byte is set) -> area i32
+ *   [n] = the set pixels, box f32 [n,4] = [x_min, y_min, x_max + 1, y_max + 1] of them, zeros for an empty mask.  Rows are
+ *   read 16 bytes at a time when W % 16 == 0 and masks is 16-byte aligned, else byte by byte.  workspace:
+ *   bxs_mask_extents_workspace_bytes(n, H, W) bytes, 8-byte aligned.  Two launches; n == 0 is a no-op.  masks may be NULL
+ *   when H * W == 0.  BXS_ERR_INVALID_ARG: a negative size, a NULL pointer with n > 0; BXS_ERR_UNSUPPORTED: H * W above
+ *   INT32_MAX.
  * No host synchronisation, deterministic.  BXS_ERR_INVALID_ARG: a NULL pointer the call needs, a negative count, a
  * non-positive size, an unknown dtype or kernel.  BXS_ERR_UNSUPPORTED: n_src > 8, more than INT32_MAX rows or pixels per
  * plane, more than 65535 images or 65535 * 32 slots.  All checks run before any device call.
@@ -745,6 +752,9 @@ int bxs_maskformer_paste_masks(const void* const* src_host, const int64_t* src_r
                                int dtype, const int64_t* rows, int64_t n, int64_t H_pad, int64_t W_pad, int64_t H_img,
                                int64_t W_img, int rescale, int64_t H_out, int64_t W_out, void* workspace, uint8_t* out,
                                int32_t* area, float* masked_sum, float* box, bxs_stream_t stream);
+int64_t bxs_mask_extents_workspace_bytes(int64_t n, int64_t H, int64_t W);
+int bxs_mask_extents(const uint8_t* masks, int64_t n, int64_t H, int64_t W, void* workspace, int32_t* area, float* box,
+                     bxs_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------
  * CondInst inference   replaces the level loop of CondInstBoxHead._get_bboxes (condinst_head.py:762-813), the NMS of

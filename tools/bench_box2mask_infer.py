@@ -30,7 +30,7 @@ from oracle import box2mask_infer as obi  # noqa: E402
 
 HBM = 3.35e12
 Q, K, HW, PAD, IMG, ORI = 100, 80, (200, 272), (800, 1088), (800, 1067), ((480, 640), (427, 640))
-KERNELS = ('maskformer_paste_kernel', 'maskformer_stats_kernel')
+KERNELS = ('maskformer_paste_kernel', 'mask_stats_reduce_kernel')
 
 
 def workload(B, seed=0):
@@ -68,7 +68,7 @@ def kernel_bytes(B):
     and writes 24 bytes per mask."""
     n, out_px = 100 * B, 100 * sum(ORI[b][0] * ORI[b][1] for b in range(B))
     return {'maskformer_paste_kernel': n * HW[0] * HW[1] * 4 + out_px + n * 64 * 32,
-            'maskformer_stats_kernel': n * 64 * 32 + n * 24}
+            'mask_stats_reduce_kernel': n * 64 * 32 + n * 24}
 
 
 def main():
