@@ -806,6 +806,35 @@ int bxs_box_nms(const float* boxes, const int64_t* seg_start, const int64_t* mas
 int bxs_condinst_paste_masks(const float* logits, int64_t n, int64_t h, int64_t w, int64_t factor, int64_t H_img, int64_t W_img,
                              int64_t H_out, int64_t W_out, int rescale, uint8_t* out, bxs_stream_t stream);
 
+/* ---------------------------------------------------------------------------------------
+ * COCO RLE of instance masks   replaces pycocotools' mask.encode in mmdet's encode_mask_results (mmdet/core/mask/utils.py:
+ *     38-65): rleEncode + rleToString of maskApi.c, byte for byte.
+ * masks: n masks u8 [n, H, W] (the bytes of a bool or uint8 tensor, dense, row-major).  Walked in column-major order
+ *   j = x * H + y with the previous byte starting at 0, a run closes wherever a byte differs from the one before it
+ *   (byte values, not set / not set: in a uint8 mask 1 -> 2 closes a run, as in pycocotools).
+ * bxs_mask_rle_runs -> offsets i64 [n + 1]: the first count of each mask, offsets[n] = R, the total count (each mask has
+ *   its boundaries + 1 counts).  It leaves the boundaries of every segment in the workspace for bxs_mask_rle_counts.
+ * bxs_mask_rle_counts: the same masks, the workspace and offsets as bxs_mask_rle_runs left them -> counts u32 [R]: mask k's
+ *   uncompressed RLE at offsets[k] .. offsets[k + 1] - 1 (the first is 0 when the first byte is non-zero; an all-zero
+ *   mask gives [H * W]).  workspace: bxs_mask_rle_counts_workspace_bytes(n, H, W) bytes, 8-byte aligned, for both calls.
+ * bxs_mask_rle_strings: counts u32 [R] and offsets i64 [n + 1] as above -> chars u8 [<= 6 R]: the strings of rleToString
+ *   (no terminator), mask k's at char_offsets[k] .. char_offsets[k + 1] - 1 of i64 [n + 1].  workspace:
+ *   bxs_mask_rle_strings_workspace_bytes(n, R) bytes, 8-byte aligned.
+ * The caller reads R between bxs_mask_rle_runs and bxs_mask_rle_counts to size counts and chars.  Three launches per call
+ *   (one memset for the counts when H * W == 0).  No host synchronisation, no atomics: deterministic.  n == 0 is a no-op;
+ *   masks may be NULL when H * W == 0.  BXS_ERR_INVALID_ARG: a negative size, a NULL pointer with n > 0, R < n.
+ *   BXS_ERR_UNSUPPORTED: H * W >= 2^29 (every delta then fits 6 characters, pycocotools' own buffer).  All checks run
+ *   before any device call.
+ * --------------------------------------------------------------------------------------- */
+int64_t bxs_mask_rle_counts_workspace_bytes(int64_t n, int64_t H, int64_t W);
+int bxs_mask_rle_runs(const uint8_t* masks, int64_t n, int64_t H, int64_t W, void* workspace, int64_t* offsets,
+                      bxs_stream_t stream);
+int bxs_mask_rle_counts(const uint8_t* masks, int64_t n, int64_t H, int64_t W, const void* workspace, const int64_t* offsets,
+                        uint32_t* counts, bxs_stream_t stream);
+int64_t bxs_mask_rle_strings_workspace_bytes(int64_t n, int64_t R);
+int bxs_mask_rle_strings(const uint32_t* counts, const int64_t* offsets, int64_t n, int64_t R, void* workspace,
+                         uint8_t* chars, int64_t* char_offsets, bxs_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
