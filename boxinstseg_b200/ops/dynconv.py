@@ -214,6 +214,14 @@ def _cells_operand_grad_mm(ops, kerns, cells, g, level_op, counts):
     return g_ops
 
 
+CELLS_MAX_IMAGES = 16      # images of one bxs_dynconv1x1_cells_* or bxs_disco_cells_* call (their problem tables)
+
+
+def _image_groups(B):
+    """[b0, b1) ranges of at most CELLS_MAX_IMAGES images covering the batch in order."""
+    return [(b0, min(b0 + CELLS_MAX_IMAGES, B)) for b0 in range(0, max(B, 1), CELLS_MAX_IMAGES)]
+
+
 def solo_cells_conv(feature_pred, kernel_preds, cells, out_sizes):
     """The positive rows of BoxSOLOv2's per-level dynamic convolution (box_solov2_head.py:204-216, indexed as :317-320).
 
@@ -223,7 +231,8 @@ def solo_cells_conv(feature_pred, kernel_preds, cells, out_sizes):
     in order: the reference's rows.  The resize is applied to the operand instead of the result (both are linear and
     per channel): levels of feature_pred's own size convolve it directly, every other size convolves one
     ``bilinear_resize`` of it, shared by the consecutive levels of that size.  All levels and images run in one launch
-    (TF32 operands, FP32 accumulation); other dtypes are promoted to float32.  Differentiable with respect to
+    (TF32 operands, FP32 accumulation); a batch of more than 16 images runs one launch per group of 16 and concatenates
+    each level's rows in image order.  Other dtypes are promoted to float32.  Differentiable with respect to
     feature_pred and kernel_preds; gradients are deterministic.  C % 32 == 0, C <= 256, h_l*w_l % 4 == 0."""
     f = L.dense_aligned(feature_pred.float())
     L.require_cuda(f)
@@ -235,10 +244,16 @@ def solo_cells_conv(feature_pred, kernel_preds, cells, out_sizes):
         level_op.append(len(op_sizes) - 1)
     ops = [f if s == tuple(f.shape[-2:]) else bilinear_resize(f, s) for s in op_sizes]
     kerns = [k.contiguous().float() for k in kernel_preds]
-    counts = [[int(c.numel()) for c in lvl] for lvl in cells]
-    flat = [c.reshape(-1) for lvl in cells for c in lvl]
-    flat = torch.cat(flat).to(device=f.device, dtype=torch.int32) if flat else f.new_zeros(0, dtype=torch.int32)
-    return list(_SoloCells.apply((level_op, counts), flat, *ops, *kerns))
+    groups = []
+    for b0, b1 in _image_groups(f.shape[0]):
+        counts = [[int(c.numel()) for c in lvl[b0:b1]] for lvl in cells]
+        flat = [c.reshape(-1) for lvl in cells for c in lvl[b0:b1]]
+        flat = torch.cat(flat).to(device=f.device, dtype=torch.int32) if flat else f.new_zeros(0, dtype=torch.int32)
+        whole = b1 - b0 == f.shape[0]
+        groups.append(_SoloCells.apply((level_op, counts), flat, *[t if whole else t[b0:b1] for t in ops + kerns]))
+    if len(groups) == 1:
+        return list(groups[0])
+    return [torch.cat(rows, 0) for rows in zip(*groups)]        # the level rows are image-major: groups in image order
 
 
 _PACK_DTYPE = {torch.float32: 0, torch.float16: 1, torch.bfloat16: 2}
@@ -279,11 +294,12 @@ def disco_cells_conv(ins_pred, kernel_preds_raw, grid_orders):
     ins_pred [B,C,h,w]; kernel_preds_raw: per level the raw grid [B,C,S,S]; grid_orders: per level a list of B int tensors,
     the covered cells (gy*S + gx) of each image in the target builder's order, repeats included.  Every level convolves the
     same ``ins_pred[b]``, so the kernels of all levels of image b are packed, in the grids' dtype, into one [B,I_pad,C]
-    operand (``bxs_disco_cells_pack``; I_pad the largest per-image total, zero rows past an image's own) and convolved by
-    ``dynconv1x1`` under its dtype and autocast rules.  Returns (per level [n_l,h,w] or None for a level without cells, per
-    level the int64 image of each row or None): the rows the reference concatenates.  Differentiable with respect to
-    ins_pred and kernel_preds_raw; d/d kernel_preds_raw sums repeated cells in row order (``bxs_disco_cells_unpack_grad``),
-    bit-identical from run to run.  The per-(level, image) counts are the cell tensors' shapes: nothing is read back."""
+    operand (``bxs_disco_cells_pack``, one call per group of at most 16 images; I_pad the largest per-image total of the
+    whole batch, zero rows past an image's own) and convolved by ``dynconv1x1`` under its dtype and autocast rules.
+    Returns (per level [n_l,h,w] or None for a level without cells, per level the int64 image of each row or None): the
+    rows the reference concatenates.  Differentiable with respect to ins_pred and kernel_preds_raw; d/d kernel_preds_raw
+    sums repeated cells in row order (``bxs_disco_cells_unpack_grad``), bit-identical from run to run.  The
+    per-(level, image) counts are the cell tensors' shapes: nothing is read back."""
     B = ins_pred.shape[0]
     n_lv = len(kernel_preds_raw)
     counts = [int(grid_orders[l][b].numel()) for l in range(n_lv) for b in range(B)]
@@ -295,9 +311,14 @@ def disco_cells_conv(ins_pred, kernel_preds_raw, grid_orders):
     dt = kernel_preds_raw[0].dtype if kernel_preds_raw[0].dtype in _PACK_DTYPE else torch.float32
     grids = [L.dense_aligned(k.to(dt)) for k in kernel_preds_raw]
     L.require_cuda(*grids)
-    cells = torch.cat([grid_orders[l][b].reshape(-1) for l in range(n_lv) for b in range(B)]).to(dev, torch.int32)
-    packed = _DiscoPack.apply(counts, I_pad, cells, *grids)
-    rows = dynconv1x1(ins_pred, packed)                                                 # [B,I_pad,h,w]
+    packs = []
+    for b0, b1 in _image_groups(B):
+        cells = torch.cat([grid_orders[l][b].reshape(-1) for l in range(n_lv) for b in range(b0, b1)]).to(dev, torch.int32)
+        g_counts = [counts[l * B + b] for l in range(n_lv) for b in range(b0, b1)]
+        whole = b1 - b0 == B
+        packs.append(_DiscoPack.apply(g_counts, I_pad, cells, *[g if whole else g[b0:b1] for g in grids]))
+    packed = packs[0] if len(packs) == 1 else torch.cat(packs, 0)                      # [B,I_pad,C]
+    rows = dynconv1x1(ins_pred, packed)                                              # [B,I_pad,h,w]
     preds, img_inds = [], []
     row0 = [0] * B
     for l in range(n_lv):

@@ -56,6 +56,16 @@ def rel_err(a, b):
     return ((a - b).norm() / b.norm().clamp(min=1e-30)).item()
 
 
+def scaled_err(got, ref):
+    """Element-wise: max |got - ref| / (|ref| + 1e-2 max |ref|).  Unlike ``rel_err`` a single wrong element of a large
+    tensor shows: one element off by 1 % of the tensor's largest value already scores 0.5."""
+    got, ref = got.detach().double().cpu(), ref.detach().double().cpu()
+    if ref.numel() == 0:
+        return 0.0
+    floor = 1e-2 * ref.abs().max().item() + 1e-300
+    return ((got - ref).abs() / (ref.abs() + floor)).max().item()
+
+
 def host_twin(name):
     """Compiles tests/host_harness/<name>.cpp -- the HOST build of the very header a kernel is made of -- with g++ and
     returns the ctypes handle (test infrastructure: lets the CPU suite check a kernel's arithmetic and indexing bit for bit

@@ -138,6 +138,28 @@ def test_batched_conv_equals_per_level_image(dt, teacher):
     assert any(p is not None and p.dtype == dt for p in new[0])
 
 
+@pytest.mark.parametrize('dt', DTYPES)
+def test_batched_conv_equals_per_level_image_beyond_16_images(dt):
+    """17 images: the kernels are packed in two groups (16 + 1 images, one bxs_disco_cells_pack call each, the batch's
+    I_pad) and convolved in one dynconv1x1 call; every network's rows and image indices equal one convolution per (level,
+    image), bit for bit."""
+    head = _head()
+    G = (3, 4, 3, 5, 3, 3, 4, 3, 3, 4, 3, 5, 3, 3, 4, 3, 3)
+    cate, s_k, t_k, s_in, t_in, boxes, labels, masks, img = _gpu_case(2, G=G, empty_image=2)   # image 2: no covered cell
+    assert s_in.shape[0] == 17
+    ctx = torch.autocast('cuda', dtype=dt) if dt != torch.float32 else torch.autocast('cuda', enabled=False)
+    with ctx:
+        new = head.corr_inputs(s_k, t_k, s_in, t_in, boxes, labels, masks, use_ind_teacher=True, best=False)
+        old = head.corr_inputs(s_k, t_k, s_in, t_in, boxes, labels, masks, use_ind_teacher=True, best=False,
+                               conv=head.dynamic_conv)
+    assert {int(i) for i in torch.cat([i for i in new[2] if i is not None])} == set(range(17)) - {2}
+    for a_list, b_list in zip(new, old):
+        for a, b in zip(a_list, b_list):
+            assert (a is None) == (b is None)
+            if a is not None:
+                assert a.dtype == b.dtype and torch.equal(a, b)
+
+
 # ---------------------------------------------------------------------------------------------------------- the loss
 def _run_loss(head, inputs, ts, ind, use_corr=False, s_feat=None, t_feat=None):
     cate, s_k, t_k, s_in, t_in, boxes, labels, masks, img = inputs

@@ -26,6 +26,7 @@ import torch.nn.functional as F
 
 from oracle import boxinst as ob
 from oracle import levelset as ol
+from tests.helpers import scaled_err
 
 pytestmark = pytest.mark.gpu
 DEV = 'cuda:0'
@@ -51,14 +52,6 @@ def sms():
     n = L.lib().bxs_device_sm_count()
     assert n > 0
     return n
-
-
-def scaled_err(got, ref):
-    got, ref = got.detach().double().cpu(), ref.detach().double().cpu()
-    if ref.numel() == 0:
-        return 0.0
-    floor = 1e-2 * ref.abs().max().item() + 1e-300
-    return ((got - ref).abs() / (ref.abs() + floor)).max().item()
 
 
 def check_close(name, got, ref, tol):

@@ -16,7 +16,11 @@ DEV = 'cuda:0'
 DTYPES = [pytest.param(torch.float16, 1e-3, 2 ** 11, id='fp16'), pytest.param(torch.bfloat16, 8e-3, 2 ** 8, id='bf16')]
 # the shapes of test_dynconv_forward / test_dynconv_backward_kernels with h*w a multiple of 8, and config C's per-image conv
 SHAPES = [(1, 256, 16, 32, 16), (2, 256, 50, 64, 100), (1, 256, 200, 256, 37), (2, 128, 26, 36, 130), (1, 256, 96, 96, 300),
-          (1, 32, 8, 4, 5), (3, 64, 10, 16, 256), (2, 256, 40, 52, 129), (1, 256, 200, 256, 16)]
+          (1, 32, 8, 4, 5), (3, 64, 10, 16, 256), (2, 256, 40, 52, 129), (1, 256, 200, 256, 16),
+          # channel counts 96..224 (a half-filled second 64-channel K-block), kernel counts at the chunk edges, P = 8 and
+          # P % 128 == 8 (136 pixels)
+          (2, 96, 2, 4, 33), (1, 160, 8, 17, 65), (2, 192, 12, 20, 127), (1, 224, 16, 24, 257), (1, 96, 24, 40, 1),
+          (2, 160, 10, 16, 128), (1, 224, 8, 17, 255)]
 
 
 def _grads(feat, kern, gout, need=(True, True)):

@@ -1,20 +1,41 @@
 """GPU parity of the positive-cell dynamic convolution (``ops.dynconv.solo_cells_conv``, bxs_dynconv1x1_cells_*) against
 the reference's lines in float64: ``F.interpolate(F.conv2d(feature_pred, kernel cells, groups=B), (h_l, w_l))`` indexed by
-the positive cells (box_solov2_head.py:204-216, 317-320).  The op resizes the operand instead of the result; the two
-orders agree up to rounding, so the TF32 bar of the dense dynconv tests holds (1e-3 of the output's scale)."""
+the positive cells (box_solov2_head.py:204-216, 317-320).  The op resizes the operand instead of the result.
+
+Every case runs twice:
+  * random data, judged element-wise (``scaled_err``, tests/helpers.py) against the float64 reference.  The op's
+    operands are TF32 (10-bit mantissa) and it resizes before it convolves, so its rounding differs from the reference's;
+    the bars below sit above the largest value observed on an H100 80GB HBM3 (SXM, 700 W power limit), given next to
+    each;
+  * an exactness probe: features and kernel grids drawn from {-2..2}, output gradients from {-1, 0, 1}, every level the
+    feature map's size or exactly 1/2 or 1/4 of each side.  A bilinear resize by exactly 1/2 or 1/4 (align_corners=False)
+    averages 2x2 pixels, so every resized operand, output row, d/d feature and d/d kernel is a multiple of 1/4 far below
+    2^20: exact as a TF32 operand, in every FP32 partial sum and whatever the order of the sums.  The op must then equal
+    the float64 reference bit for bit, so one misplaced, dropped or stale element fails the case.
+Row order, determinism (bit-identical reruns) and exact zeros at the non-positive cells of d/d kernel are checked too."""
 import pytest
 import torch
 import torch.nn.functional as F
 
-from tests.helpers import rel_err
+from tests.helpers import scaled_err
 
 pytestmark = pytest.mark.gpu
 DEV = 'cuda:0'
 GRIDS = (40, 36, 24, 16, 12)
+# element-wise bars (scaled_err) for random data; the largest value observed over all cases in the comments
+TOL_OUT = 5e-2             # level rows                                     2.9e-2
+TOL_GFEAT = 5e-2           # d / d feature_pred                             2.7e-2
+TOL_GKERN = 5e-2           # d / d kernel grids                             2.7e-2
 
 
 def _sizes(h, w):
     return [(h, w), (h, w), (h // 2, w // 2), (h // 4, w // 4), (h // 4, w // 4)]
+
+
+def _sizes8(h, w):
+    """8 levels over 4 operands: the cells table's limits (consecutive levels of one size share an operand)."""
+    f, half, quarter = (h, w), (h // 2, w // 2), (h // 4, w // 4)
+    return [f, f, half, half, quarter, quarter, f, f]
 
 
 def _cells(B, grids, gen, counts=None):
@@ -46,45 +67,93 @@ def _reference(feat, kerns, cells, sizes):
     return outs
 
 
-def _check(B, C, h, w, grids, sizes, cells, seed):
+def _run(feat, kerns, gouts, cells, sizes):
+    """The op's level rows and gradients (d/d feature, d/d every grid); a second run must give the same bits."""
     from boxinstseg_b200.ops.dynconv import solo_cells_conv
-    gen = torch.Generator().manual_seed(seed)
-    feat = torch.randn(B, C, h, w, generator=gen).to(DEV)
-    kerns = [(torch.randn(B, C, S, S, generator=gen) * 0.05).to(DEV) for S in grids]
-    f = feat.clone().requires_grad_(True)
-    ks = [k.clone().requires_grad_(True) for k in kerns]
-    outs = solo_cells_conv(f, ks, cells, sizes)
-    gouts = [torch.randn(o.shape, generator=gen).to(DEV) for o in outs]
-    gf, *gk = torch.autograd.grad(sum((o * g).sum() for o, g in zip(outs, gouts)), [f, *ks], allow_unused=True)
-    # run to run: bit-identical
-    outs2 = solo_cells_conv(f, ks, cells, sizes)
-    gf2, *gk2 = torch.autograd.grad(sum((o * g).sum() for o, g in zip(outs2, gouts)), [f, *ks], allow_unused=True)
+    runs = []
+    for _ in range(2):
+        f = feat.clone().requires_grad_(True)
+        ks = [k.clone().requires_grad_(True) for k in kerns]
+        outs = solo_cells_conv(f, ks, cells, sizes)
+        gf, *gk = torch.autograd.grad(sum((o * g).sum() for o, g in zip(outs, gouts)), [f, *ks], allow_unused=True)
+        runs.append((outs, gf, [torch.zeros_like(k) if g is None else g for k, g in zip(ks, gk)]))
+    (outs, gf, gk), (outs2, gf2, gk2) = runs
     assert all(torch.equal(a, b) for a, b in zip(outs, outs2))
     assert torch.equal(gf, gf2) and all(torch.equal(a, b) for a, b in zip(gk, gk2))
+    return outs, gf, gk
 
+
+def _reference_grads(feat, kerns, gouts, cells, sizes):
     f64 = feat.double().requires_grad_(True)
     k64 = [k.double().requires_grad_(True) for k in kerns]
     refs = _reference(f64, k64, cells, sizes)
     rgf, *rgk = torch.autograd.grad(sum((r * g.double()).sum() for r, g in zip(refs, gouts)), [f64, *k64],
                                     allow_unused=True)
-    for o, r in zip(outs, refs):
-        assert o.shape == r.shape and o.dtype == torch.float32
-        if r.numel():
-            assert rel_err(o, r) < 1e-3, rel_err(o, r)
-    assert rel_err(gf, rgf) < 1e-3, rel_err(gf, rgf)
-    for l, (g, r) in enumerate(zip(gk, rgk)):
-        if r is None:
-            r = torch.zeros_like(g, dtype=torch.float64)
-        assert g.shape == ks[l].shape
+    return [r.detach() for r in refs], rgf, [torch.zeros_like(k) if g is None else g for k, g in zip(k64, rgk)]
+
+
+def _check_zero_cells(gk, cells):
+    """d/d kernel is exactly zero at every cell that is not positive."""
+    for l, g in enumerate(gk):
+        B, C = g.shape[:2]
         S2 = g.shape[2] * g.shape[3]
         pos = torch.zeros(B, S2, dtype=torch.bool, device=DEV)
         for b in range(B):
             pos[b, cells[l][b]] = True
-        neg = ~pos[:, None, :].expand(B, C, S2)
-        assert torch.all(g.flatten(2)[neg] == 0)                    # non-positive cells: exactly zero
-        if pos.any():
-            assert rel_err(g, r) < 1e-3, (l, rel_err(g, r))
+        assert torch.all(g.flatten(2)[~pos[:, None, :].expand(B, C, S2)] == 0), l
+
+
+def _elementwise(name, got, ref, tol):
+    assert got.shape == ref.shape, (name, got.shape, ref.shape)
+    err = scaled_err(got, ref)
+    print(f'[elementwise] {name}: {err:.3e} (bar {tol:.0e})')
+    assert err <= tol, (name, err)
+
+
+def _check(B, C, h, w, grids, sizes, cells, seed):
+    """Random data against the element-wise bars, then the exactness probe; returns the random run's rows."""
+    gen = torch.Generator().manual_seed(seed)
+    feat = torch.randn(B, C, h, w, generator=gen).to(DEV)
+    kerns = [(torch.randn(B, C, S, S, generator=gen) * 0.05).to(DEV) for S in grids]
+    n = [sum(int(c.numel()) for c in lvl) for lvl in cells]
+    gouts = [torch.randn((m,) + tuple(s), generator=gen).to(DEV) for m, s in zip(n, sizes)]
+    outs, gf, gk = _run(feat, kerns, gouts, cells, sizes)
+    refs, rgf, rgk = _reference_grads(feat, kerns, gouts, cells, sizes)
+    for l, (o, r) in enumerate(zip(outs, refs)):
+        assert o.shape == r.shape and o.dtype == torch.float32
+        _elementwise(f'rows {l}', o, r, TOL_OUT)
+    _elementwise('d/d feature', gf, rgf, TOL_GFEAT)
+    for l, (g, r) in enumerate(zip(gk, rgk)):
+        assert g.shape == kerns[l].shape
+        _elementwise(f'd/d kernel {l}', g, r, TOL_GKERN)
+    _check_zero_cells(gk, cells)
+    _probe(B, C, h, w, grids, sizes, cells, gen)
     return outs
+
+
+def _probe(B, C, h, w, grids, sizes, cells, gen):
+    for s in sizes:
+        assert s in ((h, w), (h // 2, w // 2), (h // 4, w // 4)) and (h // 4) * 4 == h and (w // 4) * 4 == w
+        assert s[0] * s[1] % 4 == 0
+    feat = torch.randint(-2, 3, (B, C, h, w), generator=gen).float().to(DEV)
+    kerns = [torch.randint(-2, 3, (B, C, S, S), generator=gen).float().to(DEV) for S in grids]
+    n = [sum(int(c.numel()) for c in lvl) for lvl in cells]
+    gouts = [(torch.randint(-1, 2, (m,) + tuple(s), generator=gen) * (torch.rand((m,) + tuple(s), generator=gen) < 0.5))
+             .float().to(DEV) for m, s in zip(n, sizes)]
+    refs, rgf, rgk = _reference_grads(feat, kerns, gouts, cells, sizes)
+    # the probe's precondition: every reference value a multiple of 1/4 below 2^20, and every partial sum of the op
+    # bounded by a sum of absolute values below 2^20 (|kernel * operand| <= 4 over C channels; |g * operand| <= 2 over the
+    # pixels of an operand or the kernels of an image)
+    for r in refs + [rgf] + rgk:
+        assert torch.equal(r * 4, (r * 4).round()) and bool((r.abs() < 2 ** 20).all())
+    assert 4 * C < 2 ** 20 and 2 * h * w < 2 ** 20 and 2 * sum(n) < 2 ** 20
+    outs, gf, gk = _run(feat, kerns, gouts, cells, sizes)
+    for l, (o, r) in enumerate(zip(outs, refs)):
+        assert o.shape == r.shape
+        assert torch.equal(o.double(), r), ('rows', l, (o.double() - r).abs().max().item())
+    assert torch.equal(gf.double(), rgf), ('d/d feature', (gf.double() - rgf).abs().max().item())
+    for l, (g, r) in enumerate(zip(gk, rgk)):
+        assert torch.equal(g.double(), r), ('d/d kernel', l, (g.double() - r).abs().max().item())
 
 
 @pytest.mark.parametrize('h,w', [(200, 256), (200, 336)])
@@ -97,12 +166,52 @@ def test_cells_config_d_shapes(h, w):
     _check(2, 256, h, w, GRIDS, _sizes(h, w), cells, seed=w)
 
 
-@pytest.mark.parametrize('B', [1, 8])
+@pytest.mark.parametrize('B', [1, 8, 16, 17, 33])
 def test_cells_batch_sizes(B):
+    """8 levels over 4 operands with random counts; 16 images fill one launch's table, 17 and 33 take two and three."""
     gen = torch.Generator().manual_seed(B)
     h, w = 64, 80
-    cells = _cells(B, GRIDS, gen)
-    _check(B, 256, h, w, GRIDS, _sizes(h, w), cells, seed=10 + B)
+    grids = (40, 36, 24, 16, 12, 12, 40, 36)
+    counts = [[int(torch.randint(0, S, (1,), generator=gen)) for _ in range(B)] for S in grids]
+    if B > 2:
+        for lvl in counts:
+            lvl[B // 2] = 0                         # an image without positives between images with some
+    _check(B, 256, h, w, grids, _sizes8(h, w), _cells(B, grids, gen, counts), seed=10 + B)
+
+
+# per level (8 levels, operands: levels 0-1 full size, 2-3 half, 4-5 quarter, 6-7 full again), per image (3: the middle one
+# without any positive); per (level, image) segment and per (operand, image) problem the kernel counts 0, 1, 31, 32, 33,
+# 127, 128 and 129 -- the edges of the 32-row K-blocks of d/d operand, the 128-row chunks of d/d kernel and the forward's
+# kernel chunks.  'native': the widest problem pads to exactly 256 kernels (operand 0, image 2: 128 + 128), the largest the
+# d/d operand kernel takes; 'fallback': operand 0, image 0 pads to 160 + 128 > 256, d/d operand through cuBLAS.
+EDGE_GRIDS = (12, 16, 12, 12, 12, 12, 16, 12)
+EDGE_COUNTS = {
+    'native': [[31, 0, 128], [1, 0, 128], [33, 0, 127], [0, 0, 0], [32, 0, 129], [0, 0, 1], [127, 0, 33], [0, 0, 31]],
+    'fallback': [[129, 0, 1], [128, 0, 0], [31, 0, 0], [0, 0, 0], [0, 0, 128], [0, 0, 1], [1, 0, 127], [127, 0, 1]],
+}
+# feature maps whose quarter-size operand has a pixel tail: 11x12 = 132 = 128 + 4, 14x18 = 252 = 128 + 124
+EDGE_MAPS = {'native': (44, 48), 'fallback': (56, 72)}
+
+
+@pytest.mark.parametrize('table', ['native', 'fallback'])
+@pytest.mark.parametrize('C', [32, 96, 160, 224, 256])
+def test_cells_envelope_edges(C, table):
+    from boxinstseg_b200.ops.dynconv import _cells_widest_problem
+    counts = EDGE_COUNTS[table]
+    level_op = [0, 0, 1, 1, 2, 2, 3, 3]
+    widest = _cells_widest_problem(level_op, counts)
+    assert widest == 256 if table == 'native' else widest > 256
+    gen = torch.Generator().manual_seed(C)
+    h, w = EDGE_MAPS[table]
+    _check(3, C, h, w, EDGE_GRIDS, _sizes8(h, w), _cells(3, EDGE_GRIDS, gen, counts), seed=C + len(table))
+
+
+def test_cells_four_pixel_operand():
+    """an 8x8 feature map: operands of 64, 16 and 4 pixels (one 128-pixel tile, almost all of it tail)."""
+    gen = torch.Generator().manual_seed(4)
+    grids, h, w = (12, 8, 6, 6), 8, 8
+    counts = [[33, 1, 0], [0, 64, 2], [36, 0, 35], [1, 1, 1]]
+    _check(3, 160, h, w, grids, [(8, 8), (4, 4), (2, 2), (2, 2)], _cells(3, grids, gen, counts), seed=4)
 
 
 def test_cells_every_cell_positive():
@@ -143,7 +252,7 @@ def test_cells_operand_grad_isolated_between_images():
     gf, = torch.autograd.grad(out, [f], g)
     ref = torch.einsum('cn,nhw->chw', k[0].detach().double().reshape(64, -1)[:, :5], g[:5].double())
     assert torch.isfinite(gf[0]).all()
-    assert rel_err(gf[0], ref) < 1e-3
+    _elementwise('d/d feature, image 0', gf[0], ref, TOL_GFEAT)
 
 
 def test_dynamic_conv_cells_matches_dense():
@@ -157,7 +266,7 @@ def test_dynamic_conv_cells_matches_dense():
     dense = head.dynamic_conv(feat, kp, out_size=(20, 24))
     rows = head.dynamic_conv(feat, kp, out_size=(20, 24), cells=cells)
     for b in range(2):
-        assert rel_err(rows[b], dense[b, cells[b]].double()) < 1e-3
+        _elementwise(f'rows of image {b} against the dense path', rows[b], dense[b, cells[b]], TOL_OUT)
 
 
 def test_cells_c_abi_limits():

@@ -292,6 +292,12 @@ def test_head_edge_cases_vs_reference_lines(name):
     _compare(_run_new(*case), _run_ref(*case), _run_ref_fp32(*case))
 
 
+def test_head_17_images_vs_reference_lines():
+    """17 images of 64x64, 64 channels: the positive-cell convolution runs in two groups (16 + 1 images)."""
+    case = _case(10, 17, 64, 64, 64, [2] * 17)
+    _compare(_run_new(*case), _run_ref(*case), _run_ref_fp32(*case))
+
+
 def test_batch_without_positives():
     """no positive anywhere (no ground truth at all): zero mask losses on the graph, finite gradients, and loss_cate over the
     all-background labels (the reference raises at box_solov2_head.py:366)."""
