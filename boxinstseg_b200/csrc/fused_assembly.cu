@@ -311,14 +311,14 @@ lsf_forward_kernel(const float* __restrict__ x, const float* __restrict__ y, con
 }
 
 // d/d (a, b) and d/d T of loss_n = w E / pix, chained to d/d logits (through a = s m, b = (1 - s) m) and d/d raw T
-// (through T m) when FUSED.  The clamp(sum S_k, min=eps) passes no gradient while it is active.
+// (through T m) when FUSED.  The clamp(sum S_k, min=eps) passes no gradient while it is active.  Instance n0 + blockIdx.y.
 template <bool FUSED>
 __global__ void __launch_bounds__(NT)
 lsf_backward_kernel(const float* __restrict__ x, const float* __restrict__ y, const float* __restrict__ T, int C, int64_t hw,
                     const LsfStats* __restrict__ stats, float loss_weight, const float* __restrict__ g_loss,
-                    float* __restrict__ g_x, float* __restrict__ g_T) {
+                    float* __restrict__ g_x, float* __restrict__ g_T, int64_t n0) {
   __shared__ LsfStats st;
-  const int n = blockIdx.y;
+  const int64_t n = n0 + blockIdx.y;            // instances go over launches of at most 65535 (gridDim.y)
   if (threadIdx.x == 0) st = stats[n];
   __syncthreads();
   const float scale = g_loss[n] * loss_weight / st.pix;
@@ -414,7 +414,7 @@ extern "C" int64_t bxs_levelset_fused_workspace_bytes(int64_t n) { return n <= 0
 extern "C" int bxs_levelset_fused_forward(const float* x, const float* y, const float* T, const float* pixel_num, float* loss,
                                           void* workspace, int64_t n, int64_t C, int64_t h, int64_t w, float loss_weight,
                                           int mode, bxs_stream_t stream) {
-  if (!x || !T || !loss || !workspace || n <= 0 || n >= 65536 / LS_CL || h <= 0 || w <= 0 || (mode == 0 && !pixel_num) ||
+  if (!x || !T || !loss || !workspace || n <= 0 || n > INT32_MAX / LS_CL || h <= 0 || w <= 0 || (mode == 0 && !pixel_num) ||
       (mode == 1 && !y) || (mode != 0 && mode != 1))
     return BXS_ERR_INVALID_ARG;
   if (C < 1 || C > LS_MAXC) return BXS_ERR_UNSUPPORTED;
@@ -432,18 +432,20 @@ extern "C" int bxs_levelset_fused_forward(const float* x, const float* y, const 
 extern "C" int bxs_levelset_fused_backward(const float* x, const float* y, const float* T, const void* workspace,
                                            const float* g_loss, float* g_x, float* g_T, int64_t n, int64_t C, int64_t h,
                                            int64_t w, float loss_weight, int mode, bxs_stream_t stream) {
-  if (!x || !T || !workspace || !g_loss || (!g_x && !g_T) || n <= 0 || n >= 65536 || h <= 0 || w <= 0 ||
+  if (!x || !T || !workspace || !g_loss || (!g_x && !g_T) || n <= 0 || h <= 0 || w <= 0 ||
       (mode == 1 && !y) || (mode != 0 && mode != 1))
     return BXS_ERR_INVALID_ARG;
   if (C < 1 || C > LS_MAXC) return BXS_ERR_UNSUPPORTED;
   const int64_t hw = h * w;
   const int chunks = (int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(hw, NT), ceil_div((int64_t)sm_count() * 8, n)));
   const LsfStats* stats = reinterpret_cast<const LsfStats*>(workspace);
-  if (mode == 1)
-    lsf_backward_kernel<true><<<dim3(chunks, (unsigned)n), NT, 0, as_stream(stream)>>>(x, y, T, (int)C, hw, stats, loss_weight,
-                                                                                       g_loss, g_x, g_T);
-  else
-    lsf_backward_kernel<false><<<dim3(chunks, (unsigned)n), NT, 0, as_stream(stream)>>>(x, y, T, (int)C, hw, stats, loss_weight,
-                                                                                        g_loss, g_x, g_T);
+  constexpr int64_t kMaxGridY = 65535;
+  for (int64_t n0 = 0; n0 < n; n0 += kMaxGridY) {
+    const dim3 grid(chunks, (unsigned)std::min(n - n0, kMaxGridY));
+    if (mode == 1)
+      lsf_backward_kernel<true><<<grid, NT, 0, as_stream(stream)>>>(x, y, T, (int)C, hw, stats, loss_weight, g_loss, g_x, g_T, n0);
+    else
+      lsf_backward_kernel<false><<<grid, NT, 0, as_stream(stream)>>>(x, y, T, (int)C, hw, stats, loss_weight, g_loss, g_x, g_T, n0);
+  }
   return check_launch();
 }

@@ -485,7 +485,8 @@ int bxs_tree_edge_weight_backward(const float* embed, const int32_t* sorted_inde
  * shared memory.  loss [n] = loss_weight * E / pixel_num.  workspace: bxs_levelset_fused_workspace_bytes(n),
  * carries the statistics to the backward.  backward: g_loss [n] -> g_x (mode 1: d/d logits [n,h,w]; mode 0:
  * d/d scores2 [n,2,h,w]) and/or g_T [n,C,h,w] (mode 1: d/d raw T, i.e. already multiplied by the box mask).
- * C <= 8.
+ * C <= 8.  n: any count up to INT32_MAX / 8 (the forward's grid is n clusters of 8 CTAs in x); the backward launches
+ * over groups of at most 65535 instances, so its grid limit is not visible to the caller.
  * --------------------------------------------------------------------------------------- */
 int64_t bxs_levelset_fused_workspace_bytes(int64_t n);
 int bxs_levelset_fused_forward(const float* x, const float* y, const float* T, const float* pixel_num, float* loss,
