@@ -66,6 +66,40 @@ def scaled_err(got, ref):
     return ((got - ref).abs() / (ref.abs() + floor)).max().item()
 
 
+# significand bits after the point, and log2 of the smallest subnormal spacing
+_HALF_BITS = {torch.float16: (10, -24), torch.bfloat16: (7, -133)}
+
+
+def ulp_half(ref, dt):
+    """Element-wise spacing of ``dt`` (float16 / bfloat16) at |ref|, floored at the type's smallest subnormal spacing:
+    the unit in which a result rounded once to ``dt`` is judged against its float64 reference ``ref``."""
+    bits, sub = _HALF_BITS[dt]
+    ref = ref.detach().double().cpu()
+    _, e = torch.frexp(ref)                                        # |ref| = m 2^e, m in [0.5, 1)
+    ulp = torch.ldexp(torch.ones_like(ref), e - 1 - bits)
+    return torch.where(ref == 0, torch.zeros_like(ref), ulp).clamp(min=2.0 ** sub)
+
+
+def tied_logits(n, h, w, dt, kind, gen):
+    """[n,h,w] 16-bit logits whose rounded sigmoids tie a lot: 'saturated' (every third row s == 1.0), 'quantised'
+    (multiples of 1/2), 'constant', or 'boundaries' (equal maxima on both sides of every 16-row and 256-column
+    boundary)."""
+    x = torch.randn(n, h, w, generator=gen) * 3
+    if kind == 'saturated':
+        x[:, ::3] = 9.5 + torch.rand(n, len(range(0, h, 3)), w, generator=gen) * 4     # fp16 / bf16 s == 1.0
+    elif kind == 'quantised':
+        x = torch.round(x * 2) / 2
+    elif kind == 'constant':
+        x = torch.full((n, h, w), 0.375)
+    elif kind == 'boundaries':
+        x = torch.randn(n, h, w, generator=gen) - 4
+        for y in range(15, h - 1, 16):
+            x[:, y:y + 2, ::7] = 2.0
+        for c in range(255, w - 1, 256):
+            x[:, ::5, c:c + 2] = 2.0
+    return x.to(dt)
+
+
 def host_twin(name):
     """Compiles tests/host_harness/<name>.cpp -- the HOST build of the very header a kernel is made of -- with g++ and
     returns the ctypes handle (test infrastructure: lets the CPU suite check a kernel's arithmetic and indexing bit for bit

@@ -8,6 +8,7 @@ import torch
 import torch.nn.functional as F
 
 from tests.discobox_half_oracle import disco_half_loss
+from tests.helpers import tied_logits
 
 pytestmark = pytest.mark.gpu
 DEV = 'cuda:0'
@@ -119,30 +120,12 @@ def test_empty_level(dt):
     assert float(ni) == float(nt) == float(cnt) == 0.0 and g.shape == x.shape and g.dtype == dt
 
 
-def _tied_logits(n, h, w, dt, kind, gen):
-    x = torch.randn(n, h, w, generator=gen) * 3
-    if kind == 'saturated':
-        x[:, ::3] = 9.5 + torch.rand(n, len(range(0, h, 3)), w, generator=gen) * 4     # fp16 / bf16 s == 1.0
-    elif kind == 'quantised':
-        x = torch.round(x * 2) / 2
-    elif kind == 'constant':
-        x = torch.full((n, h, w), 0.375)
-    elif kind == 'boundaries':
-        # equal maxima on both sides of every strip (16 rows) and tile (256 columns) boundary
-        x = torch.randn(n, h, w, generator=gen) - 4
-        for y in range(15, h - 1, 16):
-            x[:, y:y + 2, ::7] = 2.0
-        for c in range(255, w - 1, 256):
-            x[:, ::5, c:c + 2] = 2.0
-    return x.to(dt)
-
-
 @pytest.mark.parametrize('dt', DTYPES)
 @pytest.mark.parametrize('kind', ['saturated', 'quantised', 'constant', 'boundaries'])
 def test_ties_go_to_first_index(dt, kind):
     n, h, w = 4, 70, 530
     gen = torch.Generator().manual_seed(17)
-    x = _tied_logits(n, h, w, dt, kind, gen)
+    x = tied_logits(n, h, w, dt, kind, gen)
     tg = _targets(n, h, w, gen, zero=(3,))
     ii = torch.zeros(n, dtype=torch.int32)
     mf = _mean_field(1, h, w, 4)

@@ -5,11 +5,14 @@ Parity is measured against a float64 einsum of the SAME 16-bit operands, so only
 rounding of each result to the operand dtype remain: rel_err <= 1e-3 for FP16 (11-bit significand), <= 8e-3 for BF16
 (8-bit).  The exactness probes use small integer operands whose results are integers below 2^11 (FP16) or 2^8 (BF16):
 every product and partial sum is then exact in FP32 and so is the final rounding, so any error in the MN-major operand
-layout, the channel / pixel order of the epilogue or the split-K reduction shows up as a wrong integer."""
+layout, the channel / pixel order of the epilogue or the split-K reduction shows up as a wrong integer.
+
+Every element is also judged on its own, in units of the operand dtype T (see ``check_elementwise``):
+|got - ref| <= ulp_T(ref) + 2 n 2^-24 sum |a| |b|, n the length of the contraction."""
 import pytest
 import torch
 
-from tests.helpers import rel_err
+from tests.helpers import rel_err, ulp_half
 
 pytestmark = pytest.mark.gpu
 DEV = 'cuda:0'
@@ -39,6 +42,28 @@ def _refs(feat, kern, gout):
             torch.einsum('bihw,bchw->bic', g, f))
 
 
+# Element-wise bar, in units of T: |got - ref| <= ulp_T(ref) + c 2^-24 sum |a| |b|, with c = 2 n for a contraction of
+# length n (C for the forward, I for d/d feat, the pixel count h w for d/d kernel, however split-K cuts it).  A product of
+# two 16-bit operands is exact in FP32, and n - 1 FP32 additions in any order are off by at most (n - 1) 2^-24 sum |a| |b|
+# when each rounds to nearest (Higham, Accuracy and Stability of Numerical Algorithms, 2nd ed., eq. 3.5); the tensor
+# cores' FP32 accumulation is not specified to round to nearest, and an adder that truncates errs by up to twice that,
+# hence 2 n.  The single rounding to T then adds half an ulp of the FP32 value, at most one ulp_T(ref).  Largest share of
+# the FP32 allowance used over all cases on an H100 80GB HBM3 (SXM, 700 W power limit), in the comment.
+ACC_C = 2                       # c / n            0.003 of the allowance used (d/d feat of (1, 256, 200, 256, 37);
+                                #                  d/d kernel of the cancelling partials)
+
+
+def check_elementwise(name, got, ref, mag, n, dt):
+    """got [..] in dt against ref (float64) with mag = sum |a| |b| of each element, a contraction of length n."""
+    got = got.detach().cpu().double()
+    ulp = ulp_half(ref, dt)
+    allow = ACC_C * n * 2.0 ** -24 * mag
+    bad = (got - ref).abs() > ulp + allow
+    used = float((((got - ref).abs() - ulp).clamp(min=0) / allow.clamp(min=1e-300)).max())
+    print(f'[elementwise] {name} n={n}: share of the FP32 allowance used {used:.3f}')
+    assert not bad.any(), (name, int(bad.sum()), got[bad][:4].tolist(), ref[bad][:4].tolist())
+
+
 @pytest.mark.parametrize('dt,tol,limit', DTYPES)
 @pytest.mark.parametrize('B,C,h,w,I', SHAPES)
 def test_half_parity_exactness_determinism(B, C, h, w, I, dt, tol, limit):
@@ -49,8 +74,11 @@ def test_half_parity_exactness_determinism(B, C, h, w, I, dt, tol, limit):
     out, gf, gk = _grads(feat, kern, gout)
     assert out.dtype == gf.dtype == gk.dtype == dt
     assert out.shape == (B, I, h, w) and gf.shape == feat.shape and gk.shape == kern.shape
-    for got, ref in zip((out, gf, gk), _refs(feat, kern, gout)):
+    mags = _refs(feat.abs(), kern.abs(), gout.abs())
+    for name, got, ref, mag, n in zip(('forward', 'd/d feat', 'd/d kernel'), (out, gf, gk), _refs(feat, kern, gout), mags,
+                                      (C, I, h * w)):
         assert rel_err(got.cpu(), ref) <= tol, rel_err(got.cpu(), ref)
+        check_elementwise(f'{dt} {(B, C, h, w, I)} {name}', got, ref, mag, n, dt)
     # determinism: a second call, and each gradient on its own, give the same bits
     out2, gf2, gk2 = _grads(feat, kern, gout)
     _, gf1, _ = _grads(feat, kern, gout, (True, False))
@@ -68,6 +96,25 @@ def test_half_parity_exactness_determinism(B, C, h, w, I, dt, tol, limit):
     out, gf, gk = _grads(fi.to(dt).to(DEV), ki.to(dt).to(DEV), gi.to(dt).to(DEV))
     for name, got, ref in zip(('forward', 'd/d feat', 'd/d kernel'), (out, gf, gk), refs):
         assert torch.equal(got.cpu().double(), ref), (name, (got.cpu().double() - ref).abs().max().item())
+
+
+@pytest.mark.parametrize('dt', [torch.float16, torch.bfloat16])
+def test_half_wgrad_partials_cancel(dt):
+    """d/d kernel where the split-K partials are large and cancel: 512 pixels are two splits of 256 (at least 256 pixels
+    per CTA), and the upstream gradient is positive on the first 256 pixels and negative on the others, so each partial is
+    about +-256 while their sum is a few units.  The partials must meet in FP32: one rounded to T on the way costs up to
+    half an ulp_T(256), far above the bar's allowance of 2 * 512 * 2^-24 * 512 = 0.03 here."""
+    B, C, h, w, I = 1, 64, 16, 32, 16
+    gen = torch.Generator().manual_seed(23)
+    feat = (torch.rand(B, C, h, w, generator=gen) + 0.5).to(dt).to(DEV)
+    kern = (torch.rand(B, I, C, generator=gen) * 0.1).to(dt).to(DEV)
+    sign = torch.where(torch.arange(h * w) < h * w // 2, 1.0, -1.0).view(1, 1, h, w)
+    gout = (sign * (torch.rand(B, I, h, w, generator=gen) + 0.5)).to(dt).to(DEV)
+    _, gf, gk = _grads(feat, kern, gout)
+    refs, mags = _refs(feat, kern, gout), _refs(feat.abs(), kern.abs(), gout.abs())
+    assert float(refs[2].abs().max()) < 0.25 * float(mags[2].min())      # the precondition: the partials cancel
+    check_elementwise(f'{dt} cancelling partials d/d kernel', gk, refs[2], mags[2], h * w, dt)
+    check_elementwise(f'{dt} cancelling partials d/d feat', gf, refs[1], mags[1], I, dt)
 
 
 @pytest.mark.parametrize('dt', [torch.float16, torch.bfloat16])
