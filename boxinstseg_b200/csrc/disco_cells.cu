@@ -1,6 +1,7 @@
-// DiscoBox's dynamic kernels of the covered grid cells, packed for ONE dense dynamic convolution per network
+// The dynamic kernels of some grid cells of every level, packed for ONE dense dynamic convolution per operand
 //     replaces the gather kernel_preds[l][b].view(C, -1)[:, grid_order] of discobox_head.py:1180-1189 for every (level, image),
-//     whose per-(level, image) F.conv2d (:1214-1227) all read the same operand s_ins_pred[b].
+//     whose per-(level, image) F.conv2d (:1214-1227) all read the same operand s_ins_pred[b], and the positive cells of
+//     BoxSOLOv2's levels of one size (box_solov2_head.py:204-216 indexed as :317-320).
 //
 //     pack:   packed[b, r, c] = grid_l[b, c, cell] for the r-th row of image b (levels in order, each level's cells in the
 //             order given: the reference's loop order, repeats included); rows past an image's total are zero.  A pure gather

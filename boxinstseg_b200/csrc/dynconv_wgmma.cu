@@ -20,15 +20,15 @@
 //   warps 0-7: two consumer warpgroups, 64 pixels of a 128-pixel tile each (ld.shared -> wgmma -> global stores)
 //   warp 8   : TMA producer (B once, then a ring of 16 KB A stages)
 // synchronised with mbarriers only (full/empty per stage).
-// Each pipeline loop is written once: dynconv_tf32_body (TF32 pixel streaming) and dynconv_wgrad_body (split-K weight
-// gradient, TF32 or 16-bit) are driven by a job object per kernel that says where its operands and results are.  The
-// host path of each product (forward, backward) is one template over the operand dtype.
+// Each pipeline loop is written once: dynconv_tf32_kernel (TF32 pixel streaming), dynconv_h_kernel (16-bit pixel
+// streaming) and dynconv_wgrad_body (split-K weight gradient, TF32 or 16-bit, driven by a job object per kernel that
+// says where its operands and results are).  The host path of each product (forward, backward) is one template over the
+// operand dtype.
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 
 #include <algorithm>
-#include <cstring>
 #include <type_traits>
 
 #include "common.cuh"
@@ -205,87 +205,6 @@ __device__ __forceinline__ float lds_box(const uint8_t* box, int k, int p) {
   return *reinterpret_cast<const float*>(box + k * 128 + ((((p >> 2) ^ (k & 7))) << 4) + (p & 3) * 4);
 }
 
-// The pixel-streaming loop of the positive-cell forward and d/d operand kernels (dynconv_tf32_kernel writes it out; see
-// there).  `job` says where its operands and results are:
-//   job.C, job.P, job.I  : channels (the reduction), pixels, kernels of the job's problem
-//   job.kmap, job.krow<BN>(): B = rows [krow, krow + BN) of the 2-D kernel map, K-blocks of 32 channels, resident
-//   job.load_a(bar, dst, pixel, kb): the [32 channels][32 pixels] box of K-block kb at `pixel`
-//   job.kvalid(kb)       : channels of K-block kb that hold data; the box's other rows are read as 0
-//   job.template store<BN>(acc, mt, box, p0, p1, c4): the accumulator rows of a warp (see DenseOut::store)
-// The job is built from `args` (the kernel's parameters) by Job's constructor.
-template <int BN, class Job, class... Args>
-__device__ __forceinline__ void dynconv_tf32_body(const Args&... args) {
-  extern __shared__ uint8_t smem_raw[];
-  SmemLayout& S = *reinterpret_cast<SmemLayout*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const Job job(args...);
-  const int kblocks = (job.C + BLOCK_K - 1) / BLOCK_K;   // channels beyond C are zero-filled by the 3-D tensor map
-  const int tiles_m = (job.P + BLOCK_M - 1) / BLOCK_M;
-
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < STAGES; ++s) { mbar_init(&S.full[s], 1); mbar_init(&S.empty[s], CONSUMER_WARPS); }
-    mbar_init(&S.b_full, 1);
-    fence_mbarrier_init();
-  }
-  __syncthreads();
-  if (warp == CONSUMER_WARPS) {
-    // ===================== TMA producer =====================
-    if (lane == 0) {
-      mbar_expect_tx(&S.b_full, (uint32_t)kblocks * BN * BLOCK_K * 4);
-      for (int kb = 0; kb < kblocks; ++kb)
-        tma_load_2d(job.kmap, &S.b_full, S.b[kb], kb * BLOCK_K, job.template krow<BN>());
-      int stage = 0, phase = 0;
-      for (int mt = blockIdx.x; mt < tiles_m; mt += gridDim.x) {
-        for (int kb = 0; kb < kblocks; ++kb) {
-          mbar_wait(&S.empty[stage], phase ^ 1);
-          mbar_expect_tx(&S.full[stage], A_STAGE_BYTES);
-#pragma unroll
-          for (int g = 0; g < BLOCK_M / 32; ++g)
-            job.load_a(&S.full[stage], S.a[stage] + g * BOX_BYTES, mt * BLOCK_M + g * 32, kb);
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-      }
-    }
-  } else {
-    // ===================== consumers: ld.shared A -> wgmma -> global =====================
-    const int wg = warp >> 2, w = warp & 3, r = lane >> 2, c4 = lane & 3;
-    const int box = 2 * wg + (w >> 1);             // the 32-pixel box of this warp's 16 rows
-    const int p0 = a_pixel(r, 2 * (w & 1)), p1 = a_pixel(r, 2 * (w & 1) + 1);
-    mbar_wait(&S.b_full, 0);
-    int stage = 0, phase = 0;
-    for (int mt = blockIdx.x; mt < tiles_m; mt += gridDim.x) {
-      float acc[BN / 2];
-#pragma unroll
-      for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
-      for (int kb = 0; kb < kblocks; ++kb) {
-        mbar_wait(&S.full[stage], phase);
-        const uint8_t* abox = S.a[stage] + box * BOX_BYTES;
-        const int kv = job.kvalid(kb);
-        uint32_t a[BLOCK_K / MMA_K][4];
-#pragma unroll
-        for (int k4 = 0; k4 < BLOCK_K / MMA_K; ++k4) {
-          const int k = k4 * MMA_K + c4;
-          a[k4][0] = k < kv ? to_tf32(lds_box(abox, k, p0)) : 0u;
-          a[k4][1] = k < kv ? to_tf32(lds_box(abox, k, p1)) : 0u;
-          a[k4][2] = k + 4 < kv ? to_tf32(lds_box(abox, k + 4, p0)) : 0u;
-          a[k4][3] = k + 4 < kv ? to_tf32(lds_box(abox, k + 4, p1)) : 0u;
-        }
-        const uint32_t b_base = smem_u32(S.b[kb]);
-        wgmma_fence();
-#pragma unroll
-        for (int k4 = 0; k4 < BLOCK_K / MMA_K; ++k4) wgmma_rs<BN>(acc, a[k4], make_desc(b_base + k4 * (MMA_K * 4)));
-        wgmma_commit();
-        wgmma_wait_all();
-        fence_acc(acc);
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&S.empty[stage]);
-        if (++stage == STAGES) { stage = 0; phase ^= 1; }
-      }
-      job.template store<BN>(acc, mt, box, p0, p1, c4);
-    }
-  }
-}
-
 // the epilogue of a [B,I,P] output (image b, kernel chunk `chunk`), as dynconv_tf32_kernel stores it
 struct DenseOut {
   float* out;
@@ -313,9 +232,9 @@ struct DenseOut {
 
 // grid: (ctas_per_group, B * n_chunks).  CTA (x, g): image b = g / n_chunks, kernel chunk g % n_chunks of BN kernels,
 // pixel tiles x, x + gridDim.x, ...
-// The loop is dynconv_tf32_body's, written out: run on dynconv_tf32_body through a job object, this kernel compiles to
-// different address arithmetic and fragment-load order, and at BN = 32 it measured 1.3-2 % slower (H100 80GB HBM3,
-// 700 W power limit, I = 16 at 200 x 256 pixels).
+// The loop is written out rather than driven by a job object as dynconv_wgrad_body is: through a job object this kernel
+// compiles to different address arithmetic and fragment-load order, and at BN = 32 it measured 1.3-2 % slower (H100 80GB
+// HBM3, 700 W power limit, I = 16 at 200 x 256 pixels).
 template <int BN>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 dynconv_tf32_kernel(const __grid_constant__ CUtensorMap tm_feat, const __grid_constant__ CUtensorMap tm_kern,
@@ -589,472 +508,6 @@ inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 
 
 using namespace bxs;
 
-
-// =====================================================================================================================
-// Positive-cell dynamic convolution (BoxSOLOv2's forward + boolean indexing, box_solov2_head.py:204-216, 317-320):
-// level l convolves the positive cells of its kernel grid [B,C,S_l,S_l] with operand op(l) [B,C,P_op], and its result
-// [n_l, P_op] holds the rows of image 0, then image 1, ..., cells ascending.  A problem is (operand o, image b); its
-// kernels are the positive cells of every level of o (levels of one operand are consecutive), level by level.
-//   forward   : pack (gather the problems' kernels K-major from the raw grids) + dynconv_tf32_body over the table
-//   d/d operand: pack K^T per problem, each level's kernels zero-padded to 32, + dynconv_tf32_body with the roles swapped
-//               (A = the level's output gradient rows, B = K^T)
-//   d/d kernel: dynconv_wgrad_body per (level, image) segment + an ordered reduce into the raw [B,C,S,S] layout
-// =====================================================================================================================
-namespace bxs {
-namespace {
-
-constexpr int CELLS_MAX_LEVELS = 8;
-constexpr int CELLS_MAX_OPS = 4;
-constexpr int CELLS_MAX_IMAGES = 16;
-constexpr int CELLS_MAX_PROBLEMS = CELLS_MAX_OPS * CELLS_MAX_IMAGES;
-constexpr int CELLS_MAX_SEGS = CELLS_MAX_LEVELS * CELLS_MAX_IMAGES;
-
-// The problem table, passed by value (about 3 KB of kernel parameters)
-struct CellsPlan {
-  CUtensorMap a[CELLS_MAX_LEVELS];        // A maps: operands (forward) or level output gradients (backward)
-  CUtensorMap b[CELLS_MAX_OPS];           // B maps: packed kernels in b[0] (forward, d/d operand) or operands (d/d kernel)
-  float* out[CELLS_MAX_LEVELS];           // forward: level outputs; d/d operand: operand gradients; d/d kernel: grids
-  const float* kern[CELLS_MAX_LEVELS];    // raw kernel grids [B,C,S_l,S_l]
-  const int32_t* cells;                   // [sum n_l] level-major, image-major, cells ascending
-  int S2[CELLS_MAX_LEVELS];
-  int lo[CELLS_MAX_OPS + 1];              // operand o owns levels [lo[o], lo[o+1])
-  int P[CELLS_MAX_OPS];
-  int start[CELLS_MAX_SEGS + 1];          // segment (l, b) = rows [start[l B + b], start[l B + b + 1]) of `cells`
-  int pbase[CELLS_MAX_PROBLEMS + 1];      // problem (o, b) = packed kernel rows [pbase[o B + b], pbase[o B + b + 1])
-  int chunk0[CELLS_MAX_SEGS + 1];         // first grid row of each problem (forward, d/d operand) or segment (d/d kernel)
-  int n_levels, n_ops, B, C, KP, splits;
-  __host__ __device__ int cnt(int l, int b) const { return start[l * B + b + 1] - start[l * B + b]; }
-  __host__ __device__ int level_row(int l, int b) const { return start[l * B + b] - start[l * B]; }   // in level l's output
-  __host__ __device__ int op_of(int l) const {
-    int o = 0;
-    while (o + 1 < n_ops && lo[o + 1] <= l) ++o;
-    return o;
-  }
-};
-
-__device__ __forceinline__ int find_chunk(const int* chunk0, int n, int y) {
-  int i = 0;
-  while (i + 1 < n && chunk0[i + 1] <= y) ++i;
-  return i;
-}
-
-__device__ __forceinline__ float cell_kernel(const CellsPlan& pl, int l, int b, int i, int c) {
-  const int cell = __ldg(pl.cells + pl.start[l * pl.B + b] + i);
-  if (cell < 0 || cell >= pl.S2[l]) return 0.f;          // outside the grid: a zero kernel, never a stray read
-  return __ldg(pl.kern[l] + ((int64_t)b * pl.C + c) * pl.S2[l] + cell);
-}
-
-// kpack[row, c], rows in problem order (the forward's K-major B operand)
-__global__ void cells_pack_kernel(const __grid_constant__ CellsPlan pl, float* __restrict__ kpack, int64_t total) {
-  const int np = pl.n_ops * pl.B;
-  for (int64_t idx = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; idx < total; idx += (int64_t)gridDim.x * blockDim.x) {
-    const int row = (int)(idx / pl.C), c = (int)(idx % pl.C);
-    const int p = find_chunk(pl.pbase, np, row);
-    const int o = p / pl.B, b = p % pl.B;
-    int i = row - pl.pbase[p], l = pl.lo[o];
-    while (l + 1 < pl.lo[o + 1] && i >= pl.cnt(l, b)) i -= pl.cnt(l++, b);
-    kpack[idx] = cell_kernel(pl, l, b, i, c);
-  }
-}
-
-// kT[p, c, k] (k < KP): problem p's kernels K^T, each level's kernels zero-padded to a multiple of 32
-__global__ void cells_pack_t_kernel(const __grid_constant__ CellsPlan pl, float* __restrict__ kt, int64_t total) {
-  for (int64_t idx = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; idx < total; idx += (int64_t)gridDim.x * blockDim.x) {
-    int k = (int)(idx % pl.KP);
-    const int c = (int)((idx / pl.KP) % pl.C), p = (int)(idx / ((int64_t)pl.KP * pl.C));
-    const int o = p / pl.B, b = p % pl.B;
-    float v = 0.f;
-    for (int l = pl.lo[o]; l < pl.lo[o + 1]; ++l) {
-      const int n = pl.cnt(l, b), n32 = (n + 31) & ~31;
-      if (k < n32) {
-        if (k < n) v = cell_kernel(pl, l, b, k, c);
-        break;
-      }
-      k -= n32;
-    }
-    kt[idx] = v;
-  }
-}
-
-// forward: problem (o, b), kernel chunk `chunk`
-struct CellsFwdJob {
-  const CellsPlan* pl;
-  const CUtensorMap* kmap;
-  int o, b, chunk, C, P, I, kbase;
-  __device__ __forceinline__ CellsFwdJob(const CellsPlan& p) : pl(&p), kmap(&p.b[0]) {
-    const int np = p.n_ops * p.B, q = find_chunk(p.chunk0, np, blockIdx.y);
-    o = q / p.B, b = q % p.B, chunk = blockIdx.y - p.chunk0[q];
-    C = p.C, P = p.P[o], kbase = p.pbase[q], I = p.pbase[q + 1] - kbase;
-  }
-  template <int BN>
-  __device__ __forceinline__ int krow() const { return kbase + chunk * BN; }
-  __device__ __forceinline__ void load_a(uint64_t* bar, void* dst, int x, int kb) const {
-    tma_load_3d(&pl->a[o], bar, dst, x, kb * BLOCK_K, b);
-  }
-  __device__ __forceinline__ int kvalid(int) const { return BLOCK_K; }
-  // kernel n of the problem -> its row of its level's output
-  __device__ __forceinline__ float* row(int n) const {
-    int l = pl->lo[o];
-    while (l + 1 < pl->lo[o + 1] && n >= pl->cnt(l, b)) n -= pl->cnt(l++, b);
-    return pl->out[l] + (int64_t)(pl->level_row(l, b) + n) * P;
-  }
-  template <int BN>
-  __device__ __forceinline__ void store(const float (&acc)[BN / 2], int mt, int box, int p0, int p1, int c4) const {
-    const int pix = mt * BLOCK_M + box * 32;
-    const bool in0 = pix + p0 < P, in1 = pix + p1 < P;
-#pragma unroll
-    for (int j = 0; j < BN / 8; ++j) {
-      const int n = chunk * BN + 8 * j + 2 * c4;
-      if (n < I) {
-        float* dst = row(n) + pix;
-        if (in0) dst[p0] = acc[4 * j];
-        if (in1) dst[p1] = acc[4 * j + 2];
-      }
-      if (n + 1 < I) {
-        float* dst = row(n + 1) + pix;
-        if (in0) dst[p0] = acc[4 * j + 1];
-        if (in1) dst[p1] = acc[4 * j + 3];
-      }
-    }
-  }
-};
-
-// d/d operand: problem (o, b), channel chunk `chunk`; reduction over the problem's padded kernels
-struct CellsDgradJob {
-  const CellsPlan* pl;
-  const CUtensorMap* kmap;
-  int o, b, chunk, C, P, I, q;
-  __device__ __forceinline__ CellsDgradJob(const CellsPlan& p, int n_chunks) : pl(&p), kmap(&p.b[0]) {
-    q = blockIdx.y / n_chunks, chunk = blockIdx.y % n_chunks;
-    o = q / p.B, b = q % p.B, P = p.P[o], I = p.C;
-    C = 0;
-    for (int l = p.lo[o]; l < p.lo[o + 1]; ++l) C += (p.cnt(l, b) + 31) & ~31;
-  }
-  template <int BN>
-  __device__ __forceinline__ int krow() const { return q * I + chunk * BN; }
-  // K-block kb = 32 gradient rows of one level, the k-th block of its (level, image) segment
-  __device__ __forceinline__ int segment(int& kb) const {
-    int l = pl->lo[o];
-    for (;; ++l) {
-      const int nk = (pl->cnt(l, b) + 31) >> 5;
-      if (kb < nk || l + 1 == pl->lo[o + 1]) return l;
-      kb -= nk;
-    }
-  }
-  __device__ __forceinline__ void load_a(uint64_t* bar, void* dst, int x, int kb) const {
-    const int l = segment(kb);
-    tma_load_3d(&pl->a[l], bar, dst, x, pl->level_row(l, b) + kb * BLOCK_K, 0);
-  }
-  // rows past the segment belong to the next image (or lie outside the map): read as 0, so that nothing of another
-  // image's gradient, not even an Inf or NaN, reaches this one
-  __device__ __forceinline__ int kvalid(int kb) const {
-    const int l = segment(kb);
-    return min(BLOCK_K, pl->cnt(l, b) - kb * BLOCK_K);
-  }
-  template <int BN>
-  __device__ __forceinline__ void store(const float (&acc)[BN / 2], int mt, int box, int p0, int p1, int c4) const {
-    DenseOut{pl->out[o], P, I, b, chunk}.template store<BN>(acc, mt, box, p0, p1, c4);   // g_operand[o] [B,C,P]
-  }
-};
-
-// d/d kernel: segment (l, b), row chunk `chunk` of 128 kernels, split `split` of the pixels
-struct CellsWgJob {
-  const CellsPlan* pl;
-  float* partial;
-  int l, o, b, chunk, split, C, I, kb0, kb1;
-  __device__ __forceinline__ CellsWgJob(const CellsPlan& p, float* partial_) : pl(&p), partial(partial_) {
-    const int s = find_chunk(p.chunk0, p.n_levels * p.B, blockIdx.y);
-    l = s / p.B, b = s % p.B, chunk = blockIdx.y - p.chunk0[s], split = blockIdx.x;
-    o = p.op_of(l);
-    C = p.C, I = p.cnt(l, b);
-    const int kb_total = (p.P[o] + BLOCK_K - 1) / BLOCK_K, kb_per = (kb_total + p.splits - 1) / p.splits;
-    kb0 = split * kb_per, kb1 = min(kb0 + kb_per, kb_total);
-  }
-  __device__ __forceinline__ void load_g(uint64_t* bar, void* dst, int kb) const {
-    tma_load_3d(&pl->a[l], bar, dst, kb * BLOCK_K, pl->level_row(l, b) + chunk * 128, 0);   // rows past I: dropped
-  }
-  __device__ __forceinline__ void load_f(uint64_t* bar, void* dst, int kb) const {
-    tma_load_3d(&pl->b[o], bar, dst, kb * BLOCK_K, 0, b);
-  }
-  // partial[(grid row, split)] = [128 rows][C]
-  template <int BN>
-  __device__ __forceinline__ void store(const float (&acc)[BN / 2], int wg, int w, int r, int c4) const {
-    const int row0 = wg * 64 + w * 16 + r;
-    float* dst = partial + ((int64_t)blockIdx.y * pl->splits + split) * 128 * C;
-#pragma unroll
-    for (int i = 0; i < BN / 2; i += 2) {
-      const int row = row0 + ((i & 2) ? 8 : 0), n = 8 * (i >> 2) + 2 * c4;
-      if (chunk * 128 + row < I && n < C)
-        *reinterpret_cast<float2*>(dst + (int64_t)row * C + n) = make_float2(acc[i], acc[i + 1]);
-    }
-  }
-};
-
-template <int BN>
-__global__ void __launch_bounds__(NUM_THREADS, 1) dynconv_cells_kernel(const __grid_constant__ CellsPlan pl) {
-  dynconv_tf32_body<BN, CellsFwdJob>(pl);
-}
-
-template <int BN>
-__global__ void __launch_bounds__(NUM_THREADS, 1) dynconv_cells_dgrad_kernel(const __grid_constant__ CellsPlan pl,
-                                                                             int n_chunks) {
-  dynconv_tf32_body<BN, CellsDgradJob>(pl, n_chunks);
-}
-
-template <int BN>
-__global__ void __launch_bounds__(NUM_THREADS, 1) dynconv_cells_wgrad_kernel(const __grid_constant__ CellsPlan pl,
-                                                                             float* __restrict__ partial) {
-  const CellsWgJob job(pl, partial);
-  dynconv_wgrad_body<BN, Tf32Mma>(job);
-}
-
-// d kernel_pred[l][b, c, cell] = the split-ordered sum of the partials of the positive cell's row, 0 for other cells.
-// One thread per (level, image, cell); the row of a positive cell is found by bisection (cells ascending per segment).
-__global__ void dynconv_cells_wgrad_reduce(const __grid_constant__ CellsPlan pl, const float* __restrict__ partial,
-                                           int64_t total) {
-  for (int64_t idx = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; idx < total; idx += (int64_t)gridDim.x * blockDim.x) {
-    int64_t rem = idx;
-    int l = 0;
-    while (rem >= (int64_t)pl.B * pl.S2[l]) rem -= (int64_t)pl.B * pl.S2[l++];
-    const int b = (int)(rem / pl.S2[l]), cell = (int)(rem % pl.S2[l]);
-    const int32_t* seg = pl.cells + pl.start[l * pl.B + b];
-    int lo = 0, hi = pl.cnt(l, b);
-    while (lo < hi) {
-      const int mid = (lo + hi) >> 1;
-      if (__ldg(seg + mid) < cell) lo = mid + 1; else hi = mid;
-    }
-    float* dst = pl.out[l] + (int64_t)b * pl.C * pl.S2[l] + cell;
-    if (lo < pl.cnt(l, b) && __ldg(seg + lo) == cell) {
-      const int g = pl.chunk0[l * pl.B + b] + lo / 128, r = lo % 128;
-      const float* src = partial + ((int64_t)g * pl.splits * 128 + r) * pl.C;
-      for (int c = 0; c < pl.C; ++c) {
-        float acc = 0.f;
-        for (int s = 0; s < pl.splits; ++s) acc += src[(int64_t)s * 128 * pl.C + c];      // split order: deterministic
-        dst[(int64_t)c * pl.S2[l]] = acc;
-      }
-    } else {
-      for (int c = 0; c < pl.C; ++c) dst[(int64_t)c * pl.S2[l]] = 0.f;
-    }
-  }
-}
-
-// Validates the host arrays and fills the sizes of the table (no device pointers, no maps).  BXS_OK or an error code.
-int cells_plan(CellsPlan& pl, const int64_t* op_size, const int64_t* grid, const int64_t* level_op, const int64_t* counts,
-               int64_t n_levels, int64_t n_ops, int64_t B, int64_t C) {
-  if (!op_size || !grid || !level_op || !counts || n_levels <= 0 || n_ops <= 0 || B <= 0 || C <= 0)
-    return BXS_ERR_INVALID_ARG;
-  if (n_levels > CELLS_MAX_LEVELS || n_ops > CELLS_MAX_OPS || B > CELLS_MAX_IMAGES || C % BLOCK_K ||
-      C > BLOCK_K * MAX_KBLOCKS)
-    return BXS_ERR_UNSUPPORTED;
-  memset(&pl, 0, sizeof(pl));
-  pl.n_levels = (int)n_levels, pl.n_ops = (int)n_ops, pl.B = (int)B, pl.C = (int)C;
-  for (int o = 0; o < n_ops; ++o) {
-    if (op_size[o] <= 0) return BXS_ERR_INVALID_ARG;
-    if (op_size[o] % 4 || op_size[o] >= (int64_t(1) << 31)) return BXS_ERR_UNSUPPORTED;
-    pl.P[o] = (int)op_size[o];
-  }
-  int64_t total = 0;
-  for (int l = 0; l < n_levels; ++l) {
-    // operands in level order, each owning consecutive levels
-    if (l == 0 ? level_op[0] != 0 : (level_op[l] != level_op[l - 1] && level_op[l] != level_op[l - 1] + 1))
-      return BXS_ERR_INVALID_ARG;
-    if (grid[l] <= 0) return BXS_ERR_INVALID_ARG;
-    if (grid[l] * grid[l] * B * C >= (int64_t(1) << 31)) return BXS_ERR_UNSUPPORTED;
-    pl.S2[l] = (int)(grid[l] * grid[l]);
-    if (l == 0 || level_op[l] != level_op[l - 1]) pl.lo[level_op[l]] = l;
-    for (int b = 0; b < B; ++b) {
-      const int64_t n = counts[l * B + b];
-      if (n < 0 || n > grid[l] * grid[l]) return BXS_ERR_INVALID_ARG;
-      pl.start[l * B + b] = (int)total;
-      total += n;
-    }
-  }
-  if (level_op[n_levels - 1] != n_ops - 1) return BXS_ERR_INVALID_ARG;
-  if (total * C >= (int64_t(1) << 31)) return BXS_ERR_UNSUPPORTED;
-  pl.start[n_levels * B] = (int)total;
-  pl.lo[n_ops] = (int)n_levels;
-  int rows = 0;
-  for (int o = 0; o < n_ops; ++o)
-    for (int b = 0; b < B; ++b) {
-      pl.pbase[o * B + b] = rows;
-      for (int l = pl.lo[o]; l < pl.lo[o + 1]; ++l) rows += pl.cnt(l, b);
-    }
-  pl.pbase[n_ops * B] = rows;
-  return BXS_OK;
-}
-
-// widest padded kernel count of a problem (the reduction of d/d operand)
-int cells_kp(const CellsPlan& pl) {
-  int kp = 0;
-  for (int o = 0; o < pl.n_ops; ++o)
-    for (int b = 0; b < pl.B; ++b) {
-      int k = 0;
-      for (int l = pl.lo[o]; l < pl.lo[o + 1]; ++l) k += (pl.cnt(l, b) + 31) & ~31;
-      kp = std::max(kp, k);
-    }
-  return kp;
-}
-
-int cells_wgrad_splits(CellsPlan& pl) {
-  int chunks = 0, kb_min = 1 << 30;
-  for (int l = 0; l < pl.n_levels; ++l)
-    for (int b = 0; b < pl.B; ++b) {
-      pl.chunk0[l * pl.B + b] = chunks;
-      chunks += (pl.cnt(l, b) + 127) / 128;
-    }
-  pl.chunk0[pl.n_levels * pl.B] = chunks;
-  for (int o = 0; o < pl.n_ops; ++o) kb_min = std::min<int>(kb_min, (int)ceil_div(pl.P[o], BLOCK_K));
-  pl.splits = (int)std::max<int64_t>(1, std::min<int64_t>((2 * (int64_t)sm_count()) / std::max(chunks, 1),
-                                                          std::max(1, kb_min / (256 / BLOCK_K))));
-  return chunks;
-}
-}  // namespace
-}  // namespace bxs
-
-extern "C" int64_t bxs_dynconv1x1_cells_forward_workspace_bytes(const int64_t* counts_host, int64_t n_levels, int64_t B,
-                                                                int64_t C) {
-  if (!counts_host || n_levels <= 0 || B <= 0 || C <= 0) return 0;
-  int64_t total = 0;
-  for (int64_t i = 0; i < n_levels * B; ++i) total += std::max<int64_t>(0, counts_host[i]);
-  return total ? 4 * total * C + 1024 : 0;
-}
-
-extern "C" int bxs_dynconv1x1_cells_forward(const float* const* operands_host, const int64_t* op_size_host,
-                                            const float* const* kernels_host, const int64_t* grid_host,
-                                            const int64_t* level_op_host, const int64_t* counts_host, const int32_t* cells,
-                                            float* const* out_host, void* workspace, int64_t n_levels, int64_t n_ops,
-                                            int64_t B, int64_t C, bxs_stream_t stream) {
-  CellsPlan pl;
-  int rc = cells_plan(pl, op_size_host, grid_host, level_op_host, counts_host, n_levels, n_ops, B, C);
-  if (rc != BXS_OK) return rc;
-  const int total = pl.start[n_levels * B];
-  if (total == 0) return BXS_OK;
-  if (!operands_host || !kernels_host || !out_host || !cells || !workspace) return BXS_ERR_INVALID_ARG;
-  for (int o = 0; o < n_ops; ++o) {
-    if (!operands_host[o]) return BXS_ERR_INVALID_ARG;
-    if (!aligned16(operands_host[o])) return BXS_ERR_UNSUPPORTED;
-  }
-  for (int l = 0; l < n_levels; ++l) {
-    if (!kernels_host[l] || (!out_host[l] && pl.start[(l + 1) * B] > pl.start[l * B])) return BXS_ERR_INVALID_ARG;
-    pl.kern[l] = kernels_host[l];
-    pl.out[l] = out_host[l];
-  }
-  pl.cells = cells;
-  const int bn = forward_bn([&] {
-    int m = 0;
-    for (int q = 0; q < n_ops * B; ++q) m = std::max(m, pl.pbase[q + 1] - pl.pbase[q]);
-    return m;
-  }());
-  int groups = 0, tiles = 0;
-  for (int q = 0; q < n_ops * B; ++q) {
-    pl.chunk0[q] = groups;
-    groups += (int)ceil_div(pl.pbase[q + 1] - pl.pbase[q], bn);
-  }
-  pl.chunk0[n_ops * B] = groups;
-  if (groups > 65535) return BXS_ERR_UNSUPPORTED;
-  float* kpack = align1k<float>(workspace);
-  for (int o = 0; o < n_ops; ++o) {
-    tiles = std::max(tiles, (int)ceil_div(pl.P[o], BLOCK_M));
-    if (!make_map(&pl.a[o], 3, operands_host[o], B, C, pl.P[o], BLOCK_K)) return BXS_ERR_LAUNCH;
-  }
-  if (!make_map(&pl.b[0], 2, kpack, 1, total, C, bn)) return BXS_ERR_LAUNCH;
-  cudaStream_t st = as_stream(stream);
-  cells_pack_kernel<<<stride_grid((int64_t)total * C), 256, 0, st>>>(pl, kpack, (int64_t)total * C);
-  if ((rc = check_launch()) != BXS_OK) return rc;
-  const dim3 grid = persistent_grid(groups, tiles);
-  auto go = [&](auto kernel) { return launch(kernel, grid, sizeof(SmemLayout) + 1024, st, pl); };
-  return bn == 32 ? go(dynconv_cells_kernel<32>) : bn == 64 ? go(dynconv_cells_kernel<64>) : go(dynconv_cells_kernel<128>);
-}
-
-extern "C" int64_t bxs_dynconv1x1_cells_backward_workspace_bytes(const int64_t* op_size_host, const int64_t* grid_host,
-                                                                 const int64_t* level_op_host, const int64_t* counts_host,
-                                                                 int64_t n_levels, int64_t n_ops, int64_t B, int64_t C) {
-  CellsPlan pl;
-  if (cells_plan(pl, op_size_host, grid_host, level_op_host, counts_host, n_levels, n_ops, B, C) != BXS_OK) return 0;
-  const int chunks = cells_wgrad_splits(pl);
-  return 4 * (int64_t)n_ops * B * C * cells_kp(pl) + 1024 + 4 * (int64_t)chunks * pl.splits * 128 * C + 1024;
-}
-
-extern "C" int bxs_dynconv1x1_cells_backward(const float* const* operands_host, const int64_t* op_size_host,
-                                             const float* const* kernels_host, const int64_t* grid_host,
-                                             const int64_t* level_op_host, const int64_t* counts_host,
-                                             const int32_t* cells, const float* const* g_out_host,
-                                             float* const* g_operands_host, float* const* g_kernels_host, void* workspace,
-                                             int64_t n_levels, int64_t n_ops, int64_t B, int64_t C, bxs_stream_t stream) {
-  CellsPlan pl;
-  int rc = cells_plan(pl, op_size_host, grid_host, level_op_host, counts_host, n_levels, n_ops, B, C);
-  if (rc != BXS_OK) return rc;
-  if (!operands_host || !kernels_host || !g_out_host || (!g_operands_host && !g_kernels_host) || !workspace ||
-      (pl.start[n_levels * B] && !cells))
-    return BXS_ERR_INVALID_ARG;
-  pl.KP = cells_kp(pl);
-  if (g_operands_host && pl.KP > 256) return BXS_ERR_UNSUPPORTED;
-  for (int o = 0; o < n_ops; ++o) {
-    if (!operands_host[o] || (g_operands_host && !g_operands_host[o])) return BXS_ERR_INVALID_ARG;
-    if (!aligned16(operands_host[o])) return BXS_ERR_UNSUPPORTED;
-  }
-  for (int l = 0; l < n_levels; ++l) {
-    const bool rows = pl.start[(l + 1) * B] > pl.start[l * B];
-    if (!kernels_host[l] || (rows && !g_out_host[l]) || (g_kernels_host && !g_kernels_host[l])) return BXS_ERR_INVALID_ARG;
-    if (rows && !aligned16(g_out_host[l])) return BXS_ERR_UNSUPPORTED;
-    pl.kern[l] = kernels_host[l];
-  }
-  pl.cells = cells;
-  cudaStream_t st = as_stream(stream);
-  const int chunks = cells_wgrad_splits(pl);         // fills chunk0 / splits of the d/d kernel table
-  float* kt = align1k<float>(workspace);
-  float* partial = align1k<float>(kt + (int64_t)n_ops * B * C * pl.KP);
-  if (g_operands_host) {
-    CellsPlan d = pl;
-    for (int o = 0; o < n_ops; ++o) d.out[o] = g_operands_host[o];
-    if (d.KP == 0) {                                   // no positive cell at all: zero gradients
-      for (int o = 0; o < n_ops; ++o)
-        if (cudaMemsetAsync(d.out[o], 0, sizeof(float) * B * C * d.P[o], st) != cudaSuccess) return check_launch();
-    } else {
-      for (int l = 0; l < n_levels; ++l) {
-        const int n = d.start[(l + 1) * B] - d.start[l * B];
-        if (n && !make_map(&d.a[l], 3, g_out_host[l], 1, n, d.P[d.op_of(l)], BLOCK_K)) return BXS_ERR_LAUNCH;
-      }
-      const int bn = forward_bn(C), n_chunks = (int)ceil_div(C, bn);
-      if (!make_map(&d.b[0], 2, kt, 1, (int64_t)n_ops * B * C, d.KP, bn)) return BXS_ERR_LAUNCH;
-      const int64_t total = (int64_t)n_ops * B * C * d.KP;
-      cells_pack_t_kernel<<<stride_grid(total), 256, 0, st>>>(d, kt, total);
-      if ((rc = check_launch()) != BXS_OK) return rc;
-      int tiles = 0;
-      for (int o = 0; o < n_ops; ++o) tiles = std::max(tiles, (int)ceil_div(d.P[o], BLOCK_M));
-      const dim3 grid = persistent_grid(n_ops * (int)B * n_chunks, tiles);
-      auto go = [&](auto kernel) { return launch(kernel, grid, sizeof(SmemLayout) + 1024, st, d, n_chunks); };
-      rc = bn == 32 ? go(dynconv_cells_dgrad_kernel<32>) : bn == 64 ? go(dynconv_cells_dgrad_kernel<64>)
-                                                                     : go(dynconv_cells_dgrad_kernel<128>);
-      if (rc != BXS_OK) return rc;
-    }
-  }
-  if (g_kernels_host) {
-    CellsPlan w = pl;
-    for (int l = 0; l < n_levels; ++l) w.out[l] = g_kernels_host[l];
-    if (chunks) {
-      for (int l = 0; l < n_levels; ++l) {
-        const int n = w.start[(l + 1) * B] - w.start[l * B];
-        if (n && !make_map(&w.a[l], 3, g_out_host[l], 1, n, w.P[w.op_of(l)], 128)) return BXS_ERR_LAUNCH;
-      }
-      for (int o = 0; o < n_ops; ++o)
-        if (!make_map(&w.b[o], 3, operands_host[o], B, C, w.P[o], (int)C)) return BXS_ERR_LAUNCH;
-      const dim3 grid(w.splits, chunks);
-      auto go = [&](auto kernel) { return launch(kernel, grid, sizeof(WgSmem) + 1024, st, w, partial); };
-      rc = C <= 32    ? go(dynconv_cells_wgrad_kernel<32>)
-           : C <= 64  ? go(dynconv_cells_wgrad_kernel<64>)
-           : C <= 128 ? go(dynconv_cells_wgrad_kernel<128>)
-                      : go(dynconv_cells_wgrad_kernel<256>);
-      if (rc != BXS_OK) return rc;
-    }
-    int64_t total = 0;
-    for (int l = 0; l < n_levels; ++l) total += B * (int64_t)w.S2[l];
-    dynconv_cells_wgrad_reduce<<<stride_grid(total), 256, 0, st>>>(w, partial, total);
-    if ((rc = check_launch()) != BXS_OK) return rc;
-  }
-  return BXS_OK;
-}
-
 // =====================================================================================================================
 // 16-bit operands (FP16 or BF16, chosen at compile time), FP32 accumulation in registers: the same three products for
 // callers that run in mixed precision (the reference's DiscoBox configs train under autocast), at half the bytes.
@@ -1326,7 +779,7 @@ struct Kernels<float> {
   template <int BN> static constexpr auto fwd = dynconv_tf32_kernel<BN>;
   template <int BN> static constexpr auto wgrad = dynconv_wgrad_kernel<BN>;
   static constexpr size_t fwd_smem = sizeof(SmemLayout) + 1024;
-  static constexpr int kmap_rank = 2;                 // dynconv_tf32_body loads B with 2-D TMA
+  static constexpr int kmap_rank = 2;                 // dynconv_tf32_kernel loads B with 2-D TMA
 };
 
 // out[b, i, p] = sum_c kern[b, i, c] * feat3[b, c, p] for c < C; rows c >= feat_rows of feat3 read as zeros

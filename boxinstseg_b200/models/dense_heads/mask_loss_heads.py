@@ -171,9 +171,10 @@ class BoxSOLOv2Head(nn.Module):
     def loss(self, ins_preds, cate_preds, levelset_feats, gt_bbox_list, gt_label_list, gt_mask_list, img, img_metas, cfg,
              gt_bboxes_ignore=None):
         """dict(loss_boxpro, loss_levelset, loss_cate) as the reference computes them.  ``ins_preds``: ``forward``'s
-        ``SoloInsPreds`` (only the positive cells are convolved, ``solo_cells_conv``: one launch for every level and image)
-        or the reference's dense per-level [B,S*S,h,w] tensors (their positive rows are gathered).  ``gt_mask_list``: per
-        image uint8 [G,H,W] tensors, or anything with mmdet's ``to_tensor(dtype, device)`` (BitmapMasks).
+        ``SoloInsPreds`` (only the positive cells are convolved, ``solo_cells_conv``: one pack, convolution and row gather
+        per run of levels of one size) or the reference's dense per-level [B,S*S,h,w] tensors (their positive rows are
+        gathered).  ``gt_mask_list``: per image uint8 [G,H,W] tensors, or anything with mmdet's
+        ``to_tensor(dtype, device)`` (BitmapMasks).
         The grid targets are built on the device (``solo_grid_targets``), the image and level-set targets stay per image (the
         trees are shared by its instances), ``loss_cate`` is ``sigmoid_focal_loss_levels`` on the [B,C,S,S] maps as they lie.
         ONE read back to the host: the positive count of every (level, image).
@@ -264,8 +265,9 @@ class BoxSOLOv2Head(nn.Module):
     def dynamic_conv(self, feature_pred, kernel_pred, out_size=None, cells=None):
         """feature_pred [B,C,h,w], kernel_pred [B,C,S,S] -> [B,S*S,h',w'].  ``cells`` (list of per-image ascending index
         tensors) restricts the convolution to the positive grid cells the loss will index (:317-320), which is
-        what the training loss needs, and returns the per-image list of [n_b,h',w'] rows (``solo_cells_conv``: one launch,
-        the resize applied to feature_pred); without it all S*S cells are computed as the reference does."""
+        what the training loss needs, and returns the per-image list of [n_b,h',w'] rows (``solo_cells_conv``: one pack,
+        convolution and row gather, the resize applied to feature_pred); without it all S*S cells are computed as the
+        reference does."""
         if cells is not None:
             size = tuple(out_size) if out_size is not None else tuple(feature_pred.shape[-2:])
             rows = solo_cells_conv(feature_pred, [kernel_pred], [cells], [size])[0]

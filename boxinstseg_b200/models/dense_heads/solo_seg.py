@@ -16,14 +16,12 @@ import types
 import torch
 
 from ...ops import solo_seg as S
-from ...ops.dynconv import _DiscoPack, dynconv1x1
+from ...ops.dynconv import PACK_MAX_ROWS, _CellPack, dynconv1x1, row_chunks
 
 try:                                            # pragma: no cover - mmdet is absent in this image
     from mmdet.core import InstanceData
 except ImportError:
     InstanceData = None
-
-DISCO_MAX_ROWS = 2048                           # rows per image of one bxs_disco_cells_pack call
 
 
 def cfg_get(cfg, key):
@@ -93,8 +91,8 @@ class Candidates:
 
 def _disco_sources(cands, kernel_preds, seg_pred):
     """DiscoBox's candidate convolution: every distinct cell once, packed per image (``bxs_disco_cells_pack``, at most
-    DISCO_MAX_ROWS rows per image and call) and convolved by ``dynconv1x1`` under the caller's autocast.  Returns the row
-    sources (one [B*I_pad, h, w] logit tensor per chunk) and the source row id of every distinct row."""
+    PACK_MAX_ROWS rows per image and call: ``row_chunks``) and convolved by ``dynconv1x1`` under the caller's autocast.
+    Returns the row sources (one [B*I_pad, h, w] logit tensor per chunk) and the source row id of every distinct row."""
     B, n_lv = cands.B, len(kernel_preds)
     dev = seg_pred.device
     h, w = seg_pred.shape[-2:]
@@ -102,32 +100,22 @@ def _disco_sources(cands, kernel_preds, seg_pred):
     for l in range(n_lv):
         for b in range(B):
             seg_start.append(seg_start[-1] + cands.seg_counts[l][b])
-    totals = [sum(cands.seg_counts[l][b] for l in range(n_lv)) for b in range(B)]
-    n_chunks = max(1, -(-max(totals) // DISCO_MAX_ROWS))
-    if n_chunks > S.MAX_SOURCES:
-        raise NotImplementedError(f'DiscoBoxSOLOv2Head.get_seg: more than {S.MAX_SOURCES * DISCO_MAX_ROWS} distinct '
+    chunks = row_chunks(cands.seg_counts)
+    if len(chunks) > S.MAX_SOURCES:
+        raise NotImplementedError(f'DiscoBoxSOLOv2Head.get_seg: more than {S.MAX_SOURCES * PACK_MAX_ROWS} distinct '
                                   'candidate cells in one image')
     dt = kernel_preds[0].dtype if kernel_preds[0].dtype in (torch.float32, torch.float16, torch.bfloat16) else torch.float32
     grids = [k.detach().to(dt).contiguous() for k in kernel_preds]
     cells = cands.row_cell.to(torch.int32)
-    sources, ids, src_start = [], [], 0
+    sources, src_start = [], 0
     pieces = []                                   # (distinct-row start, length, source id base) of every sub-range
-    for k in range(n_chunks):
-        lo, hi = k * DISCO_MAX_ROWS, (k + 1) * DISCO_MAX_ROWS
-        counts, cell_parts, q = [], [], [0] * B
-        i_pad = max(min(t, hi) - lo for t in totals)
-        for l in range(n_lv):
-            for b in range(B):
-                n = cands.seg_counts[l][b]
-                a, e = max(q[b], lo), min(q[b] + n, hi)
-                take = max(0, e - a)
-                counts.append(take)
-                if take:
-                    r0 = seg_start[l * B + b] + (a - q[b])
-                    cell_parts.append(cells[r0:r0 + take])
-                    pieces.append((r0, take, src_start + b * i_pad + (a - lo)))
-                q[b] += n
-        packed = _DiscoPack.apply(counts, i_pad, torch.cat(cell_parts), *grids)
+    for i_pad, counts, parts in chunks:
+        cell_parts = []
+        for l, b, j, n, r in parts:
+            r0 = seg_start[l * B + b] + j
+            cell_parts.append(cells[r0:r0 + n])
+            pieces.append((r0, n, src_start + b * i_pad + r))
+        packed = _CellPack.apply(counts, i_pad, torch.cat(cell_parts), *grids)
         logits = dynconv1x1(seg_pred.detach(), packed)                                      # [B, i_pad, h, w]
         sources.append(logits.reshape(B * i_pad, h, w))
         src_start += B * i_pad

@@ -134,132 +134,13 @@ def _ptrs(tensors):
     return (ctypes.c_void_p * len(tensors))(*[None if t is None else t.data_ptr() for t in tensors])
 
 
-class _SoloCells(torch.autograd.Function):
-    """Levels -> positive rows on bxs_dynconv1x1_cells_*.  Inputs: the plan (host lists), the device cell list, then the
-    operands and the raw kernel grids."""
-
-    @staticmethod
-    def forward(ctx, plan, cells, *tensors):
-        level_op, counts = plan
-        n_ops = len(tensors) - len(level_op)
-        ops, kerns = tensors[:n_ops], tensors[n_ops:]
-        B, C = ops[0].shape[:2]
-        outs = [ops[o].new_empty((sum(n), ops[o].shape[2], ops[o].shape[3])) for o, n in zip(level_op, counts)]
-        ctx.save_for_backward(cells, *tensors)
-        ctx.plan = plan
-        args = (_i64([o.shape[2] * o.shape[3] for o in ops]), _ptrs(kerns), _i64([k.shape[-1] for k in kerns]),
-                _i64(level_op), _i64([c for n in counts for c in n]))
-        ctx.args = args
-        flat = args[-1]
-        with torch.cuda.device(ops[0].device):
-            ws = torch.empty(L.lib().bxs_dynconv1x1_cells_forward_workspace_bytes(flat, len(kerns), B, C), dtype=torch.uint8,
-                             device=ops[0].device)
-            L.check(L.lib().bxs_dynconv1x1_cells_forward(_ptrs(ops), args[0], args[1], args[2], args[3], flat, L.ptr(cells),
-                                                         _ptrs(outs), L.ptr(ws), len(kerns), n_ops, B, C, L.stream()),
-                    'dynconv1x1_cells_forward')
-        return tuple(outs)
-
-    @staticmethod
-    def backward(ctx, *g_outs):
-        cells, *tensors = ctx.saved_tensors
-        level_op, counts = ctx.plan
-        n_ops = len(tensors) - len(level_op)
-        ops, kerns = tensors[:n_ops], tensors[n_ops:]
-        B, C = ops[0].shape[:2]
-        need_op = any(ctx.needs_input_grad[2:2 + n_ops])
-        need_k = any(ctx.needs_input_grad[2 + n_ops:])
-        g = [torch.zeros((sum(n),) + ops[o].shape[2:], device=ops[0].device) if t is None else L.dense_aligned(t.float())
-             for t, o, n in zip(g_outs, level_op, counts)]
-        g_ops = [torch.empty_like(o) for o in ops] if need_op else None
-        g_k = [torch.empty_like(k) for k in kerns] if need_k else None
-        sizes, kp, grid, lop, flat = ctx.args
-        lib = L.lib()
-        with torch.cuda.device(ops[0].device):
-            ws = torch.empty(lib.bxs_dynconv1x1_cells_backward_workspace_bytes(sizes, grid, lop, flat, len(kerns), n_ops, B, C),
-                             dtype=torch.uint8, device=ops[0].device)
-            call = lambda gop, gk: lib.bxs_dynconv1x1_cells_backward(      # noqa: E731
-                _ptrs(ops), sizes, kp, grid, lop, flat, L.ptr(cells), _ptrs(g), gop, gk, L.ptr(ws), len(kerns), n_ops, B, C,
-                L.stream())
-            if need_op and _cells_widest_problem(level_op, counts) > 256:
-                # more than 256 kernels in a problem: d/d operand through cuBLAS, as dynconv1x1 does beyond 256 kernels
-                g_ops = _cells_operand_grad_mm(ops, kerns, cells, g, level_op, counts)
-                rc = call(None, _ptrs(g_k)) if need_k else 0
-            else:
-                rc = call(_ptrs(g_ops) if need_op else None, _ptrs(g_k) if need_k else None)
-            L.check(rc, 'dynconv1x1_cells_backward')
-        return (None, None, *(g_ops if need_op else [None] * n_ops), *(g_k if need_k else [None] * len(kerns)))
-
-
-def _cells_widest_problem(level_op, counts):
-    """Kernels of the widest (operand, image) problem, each level's count padded to 32: what the d/d operand kernel reduces
-    over (cells_kp in csrc/dynconv_wgmma.cu), and what limits it to 256."""
-    widest = 0
-    for o in set(level_op):
-        per_image = zip(*[n for n, lo in zip(counts, level_op) if lo == o])
-        widest = max([widest] + [sum((c + 31) & ~31 for c in image) for image in per_image])
-    return widest
-
-
-def _cells_operand_grad_mm(ops, kerns, cells, g, level_op, counts):
-    g_ops = [torch.zeros_like(o) for o in ops]
-    start = 0
-    for l, (o, n) in enumerate(zip(level_op, counts)):
-        C = kerns[l].shape[1]
-        row = 0
-        for b, nb in enumerate(n):
-            if nb:
-                k = kerns[l][b].reshape(C, -1)[:, cells[start:start + nb].long()]
-                g_ops[o][b] += (k @ g[l][row:row + nb].flatten(1)).view_as(g_ops[o][b])
-            start, row = start + nb, row + nb
-    return g_ops
-
-
-CELLS_MAX_IMAGES = 16      # images of one bxs_dynconv1x1_cells_* or bxs_disco_cells_* call (their problem tables)
-
-
-def _image_groups(B):
-    """[b0, b1) ranges of at most CELLS_MAX_IMAGES images covering the batch in order."""
-    return [(b0, min(b0 + CELLS_MAX_IMAGES, B)) for b0 in range(0, max(B, 1), CELLS_MAX_IMAGES)]
-
-
-def solo_cells_conv(feature_pred, kernel_preds, cells, out_sizes):
-    """The positive rows of BoxSOLOv2's per-level dynamic convolution (box_solov2_head.py:204-216, indexed as :317-320).
-
-    feature_pred [B,C,h,w]; kernel_preds: per level the raw grid [B,C,S,S] (as ``solo_kernel`` produces it); cells: per level
-    a list of B int tensors, the ascending positive cells (gy*S + gx) of each image; out_sizes: per level (h_l, w_l).
-    Returns per level [n_l, h_l, w_l] = interpolate(conv2d(feature_pred, cells), (h_l, w_l), bilinear)[positives], images
-    in order: the reference's rows.  The resize is applied to the operand instead of the result (both are linear and
-    per channel): levels of feature_pred's own size convolve it directly, every other size convolves one
-    ``bilinear_resize`` of it, shared by the consecutive levels of that size.  All levels and images run in one launch
-    (TF32 operands, FP32 accumulation); a batch of more than 16 images runs one launch per group of 16 and concatenates
-    each level's rows in image order.  Other dtypes are promoted to float32.  Differentiable with respect to
-    feature_pred and kernel_preds; gradients are deterministic.  C % 32 == 0, C <= 256, h_l*w_l % 4 == 0."""
-    f = L.dense_aligned(feature_pred.float())
-    L.require_cuda(f)
-    sizes = [(int(s[0]), int(s[1])) for s in out_sizes]
-    level_op, op_sizes = [], []
-    for s in sizes:
-        if not op_sizes or op_sizes[-1] != s:
-            op_sizes.append(s)
-        level_op.append(len(op_sizes) - 1)
-    ops = [f if s == tuple(f.shape[-2:]) else bilinear_resize(f, s) for s in op_sizes]
-    kerns = [k.contiguous().float() for k in kernel_preds]
-    groups = []
-    for b0, b1 in _image_groups(f.shape[0]):
-        counts = [[int(c.numel()) for c in lvl[b0:b1]] for lvl in cells]
-        flat = [c.reshape(-1) for lvl in cells for c in lvl[b0:b1]]
-        flat = torch.cat(flat).to(device=f.device, dtype=torch.int32) if flat else f.new_zeros(0, dtype=torch.int32)
-        whole = b1 - b0 == f.shape[0]
-        groups.append(_SoloCells.apply((level_op, counts), flat, *[t if whole else t[b0:b1] for t in ops + kerns]))
-    if len(groups) == 1:
-        return list(groups[0])
-    return [torch.cat(rows, 0) for rows in zip(*groups)]        # the level rows are image-major: groups in image order
-
-
+PACK_MAX_IMAGES = 16       # images of one bxs_disco_cells_pack call (its problem table)
+PACK_MAX_ROWS = 2048       # rows per image of one bxs_disco_cells_pack call (the unpack's row links in shared memory)
+PACK_MAX_GRID = 64         # S of a grid the pack takes (the unpack's list heads in shared memory)
 _PACK_DTYPE = {torch.float32: 0, torch.float16: 1, torch.bfloat16: 2}
 
 
-class _DiscoPack(torch.autograd.Function):
+class _CellPack(torch.autograd.Function):
     """Raw kernel grids -> packed [B,I_pad,C] rows (bxs_disco_cells_pack); backward: bxs_disco_cells_unpack_grad."""
 
     @staticmethod
@@ -288,48 +169,128 @@ class _DiscoPack(torch.autograd.Function):
         return (None, None, None, *g_grids)
 
 
+_DiscoPack = _CellPack          # its name while DiscoBox was its only user
+
+
+def _image_groups(B):
+    """[b0, b1) ranges of at most PACK_MAX_IMAGES images covering the batch in order."""
+    return [(b0, min(b0 + PACK_MAX_IMAGES, B)) for b0 in range(0, max(B, 1), PACK_MAX_IMAGES)]
+
+
+def row_chunks(seg_counts):
+    """Splits the rows of a pack into calls of at most PACK_MAX_ROWS rows per image.  seg_counts[l][b]: the rows of
+    segment (level l, image b); image b's rows are those of its segments (0, b), (1, b), ... in turn.  Returns one
+    (I_pad, counts, pieces) per call: I_pad its largest row count of an image, counts[l * B + b] the rows of segment (l, b)
+    it takes, and per segment part it takes, level-major then image-major, (l, b, j, n, r): rows j .. j + n of segment
+    (l, b) are its rows r .. r + n of image b."""
+    n_lv, B = len(seg_counts), len(seg_counts[0])
+    totals = [sum(seg_counts[l][b] for l in range(n_lv)) for b in range(B)]
+    chunks = []
+    for lo in range(0, max(max(totals), 1), PACK_MAX_ROWS):
+        hi = lo + PACK_MAX_ROWS
+        counts, pieces, q = [], [], [0] * B
+        for l in range(n_lv):
+            for b in range(B):
+                a, e = max(q[b], lo), min(q[b] + seg_counts[l][b], hi)
+                counts.append(max(0, e - a))
+                if e > a:
+                    pieces.append((l, b, a - q[b], e - a, a - lo))
+                q[b] += seg_counts[l][b]
+        chunks.append((max(min(t, hi) - lo for t in totals), counts, pieces))
+    return chunks
+
+
+def cells_conv(operand, grids, cells):
+    """The dynamic convolution of some grid cells of every level with one operand.
+
+    operand [B,C,h,w]; grids: per level the raw kernel grid [B,C,S,S] (S <= 64), all of one dtype (float32, float16 or
+    bfloat16); cells: per level a list of B int tensors, the cells (gy*S + gx) of each image in any order, repeats allowed.
+    Returns per level [n_l,h,w]: the rows of image 0, then image 1, ..., each image's in the order of its cells.
+    The kernels of all levels of image b are packed, in the grids' dtype, into the rows of one [B,I_pad,C] operand
+    (``bxs_disco_cells_pack``: one call per group of at most 16 images and chunk of at most 2048 rows per image, the chunks
+    side by side; I_pad the largest per-image total of the batch, zero rows past an image's own), convolved by one
+    ``dynconv1x1`` call under its dtype and autocast rules, and the level rows are taken out of the [B,I_pad,h,w] result by
+    one ``index_select``.  Differentiable with respect to operand and grids; d/d grids sums repeated cells in row order
+    (``bxs_disco_cells_unpack_grad``) and is 0 at every cell not named, bit-identical from run to run.  The counts are the
+    cell tensors' shapes: nothing is read back and nothing is copied to the device but the cells."""
+    big = [g.shape[-1] for g in grids if g.shape[-1] > PACK_MAX_GRID]
+    if big:
+        raise NotImplementedError(f'cells_conv: kernel grids of at most {PACK_MAX_GRID} x {PACK_MAX_GRID} cells, got '
+                                  f'{big[0]} x {big[0]}')
+    grids = [L.dense_aligned(g) for g in grids]
+    L.require_cuda(*grids)
+    B, dev = operand.shape[0], operand.device
+    seg_counts = [[int(c.numel()) for c in lvl] for lvl in cells]
+    packs, pieces, col = [], [], 0
+    for I_pad, counts, parts in row_chunks(seg_counts):
+        group_packs = []
+        for b0, b1 in _image_groups(B):
+            flat = [cells[l][b].reshape(-1)[j:j + n] for l, b, j, n, _ in parts if b0 <= b < b1]
+            flat = torch.cat(flat).to(dev, torch.int32) if flat else torch.zeros(0, dtype=torch.int32, device=dev)
+            g_counts = [counts[l * B + b] for l in range(len(grids)) for b in range(b0, b1)]
+            whole = b1 - b0 == B
+            group_packs.append(_CellPack.apply(g_counts, I_pad, flat, *[g if whole else g[b0:b1] for g in grids]))
+        packs.append(group_packs[0] if len(group_packs) == 1 else torch.cat(group_packs, 0))
+        pieces += [(l, b, j, n, col + r) for l, b, j, n, r in parts]
+        col += I_pad
+    packed = packs[0] if len(packs) == 1 else torch.cat(packs, 1)                       # [B,I_pad,C]
+    rows = dynconv1x1(operand, packed)                                                # [B,I_pad,h,w]
+    pieces.sort()                                                                     # level, image, row of the segment
+    index = [torch.arange(b * col + r, b * col + r + n, device=dev) for _, b, _, n, r in pieces]
+    index = torch.cat(index) if index else torch.zeros(0, dtype=torch.int64, device=dev)
+    return list(rows.reshape((-1,) + rows.shape[2:]).index_select(0, index).split([sum(n) for n in seg_counts]))
+
+
+def solo_cells_conv(feature_pred, kernel_preds, cells, out_sizes):
+    """The positive rows of BoxSOLOv2's per-level dynamic convolution (box_solov2_head.py:204-216, indexed as :317-320).
+
+    feature_pred [B,C,h,w]; kernel_preds: per level the raw grid [B,C,S,S] (as ``solo_kernel`` produces it); cells: per level
+    a list of B int tensors, the ascending positive cells (gy*S + gx) of each image; out_sizes: per level (h_l, w_l).
+    Returns per level [n_l, h_l, w_l] = interpolate(conv2d(feature_pred, cells), (h_l, w_l), bilinear)[positives], images
+    in order: the reference's rows.  The resize is applied to the operand instead of the result (both are linear and
+    per channel): levels of feature_pred's own size convolve it directly, every other size convolves one
+    ``bilinear_resize`` of it, and each run of consecutive levels of one size is one ``cells_conv`` call, so each operand is
+    read once per image for all its levels.  TF32 operands and FP32 accumulation whatever the autocast state: other dtypes
+    are promoted to float32.  Differentiable with respect to feature_pred and kernel_preds; gradients are deterministic.
+    C % 32 == 0, C <= 256, h_l*w_l % 4 == 0; a grid larger than 64 x 64 cells raises NotImplementedError."""
+    sizes = [(int(s[0]), int(s[1])) for s in out_sizes]
+    rows, l0 = [], 0
+    with torch.autocast('cuda', enabled=False):
+        f = L.dense_aligned(feature_pred.float())
+        L.require_cuda(f)
+        for l1 in range(1, len(sizes) + 1):
+            if l1 == len(sizes) or sizes[l1] != sizes[l0]:
+                op = f if sizes[l0] == tuple(f.shape[-2:]) else bilinear_resize(f, sizes[l0])
+                rows += cells_conv(op, [k.float() for k in kernel_preds[l0:l1]], cells[l0:l1])
+                l0 = l1
+    return rows
+
+
 def disco_cells_conv(ins_pred, kernel_preds_raw, grid_orders):
-    """Every (level, image) dynamic convolution of DiscoBox (discobox_head.py:1180-1246) in ONE ``dynconv1x1`` call.
+    """Every (level, image) dynamic convolution of DiscoBox (discobox_head.py:1180-1246) in ONE ``cells_conv`` call.
 
     ins_pred [B,C,h,w]; kernel_preds_raw: per level the raw grid [B,C,S,S]; grid_orders: per level a list of B int tensors,
     the covered cells (gy*S + gx) of each image in the target builder's order, repeats included.  Every level convolves the
-    same ``ins_pred[b]``, so the kernels of all levels of image b are packed, in the grids' dtype, into one [B,I_pad,C]
-    operand (``bxs_disco_cells_pack``, one call per group of at most 16 images; I_pad the largest per-image total of the
-    whole batch, zero rows past an image's own) and convolved by ``dynconv1x1`` under its dtype and autocast rules.
-    Returns (per level [n_l,h,w] or None for a level without cells, per level the int64 image of each row or None): the
-    rows the reference concatenates.  Differentiable with respect to ins_pred and kernel_preds_raw; d/d kernel_preds_raw
-    sums repeated cells in row order (``bxs_disco_cells_unpack_grad``), bit-identical from run to run.  The
-    per-(level, image) counts are the cell tensors' shapes: nothing is read back."""
-    B = ins_pred.shape[0]
-    n_lv = len(kernel_preds_raw)
-    counts = [int(grid_orders[l][b].numel()) for l in range(n_lv) for b in range(B)]
-    totals = [sum(counts[l * B + b] for l in range(n_lv)) for b in range(B)]
-    I_pad = max(totals)
-    dev = ins_pred.device
-    if I_pad == 0:
+    same ``ins_pred[b]``, so the kernels of all levels are packed in the grids' dtype (float32 for any other) and convolved
+    by ``dynconv1x1`` under its dtype and autocast rules.  Returns (per level [n_l,h,w] or None for a level without cells,
+    per level the int64 image of each row or None): the rows the reference concatenates.  Differentiable with respect to
+    ins_pred and kernel_preds_raw; d/d kernel_preds_raw sums repeated cells in row order, bit-identical from run to run.
+    The per-(level, image) counts are the cell tensors' shapes: nothing is read back."""
+    B, n_lv = ins_pred.shape[0], len(kernel_preds_raw)
+    counts = [[int(grid_orders[l][b].numel()) for b in range(B)] for l in range(n_lv)]
+    if not any(map(any, counts)):
         return [None] * n_lv, [None] * n_lv
     dt = kernel_preds_raw[0].dtype if kernel_preds_raw[0].dtype in _PACK_DTYPE else torch.float32
-    grids = [L.dense_aligned(k.to(dt)) for k in kernel_preds_raw]
-    L.require_cuda(*grids)
-    packs = []
-    for b0, b1 in _image_groups(B):
-        cells = torch.cat([grid_orders[l][b].reshape(-1) for l in range(n_lv) for b in range(b0, b1)]).to(dev, torch.int32)
-        g_counts = [counts[l * B + b] for l in range(n_lv) for b in range(b0, b1)]
-        whole = b1 - b0 == B
-        packs.append(_DiscoPack.apply(g_counts, I_pad, cells, *[g if whole else g[b0:b1] for g in grids]))
-    packed = packs[0] if len(packs) == 1 else torch.cat(packs, 0)                      # [B,I_pad,C]
-    rows = dynconv1x1(ins_pred, packed)                                              # [B,I_pad,h,w]
+    rows = cells_conv(ins_pred, [k.to(dt) for k in kernel_preds_raw], grid_orders)
     preds, img_inds = [], []
-    row0 = [0] * B
-    for l in range(n_lv):
-        n = counts[l * B:(l + 1) * B]
+    for r, n in zip(rows, counts):
         if not sum(n):
             preds.append(None)
             img_inds.append(None)
             continue
-        preds.append(torch.cat([rows[b, row0[b]:row0[b] + n[b]] for b in range(B) if n[b]], 0))
-        img_inds.append(torch.cat([torch.full((n[b],), b, dtype=torch.int64, device=dev) for b in range(B) if n[b]]))
-        row0 = [r + c for r, c in zip(row0, n)]
+        preds.append(r)
+        img_inds.append(torch.cat([torch.full((c,), b, dtype=torch.int64, device=ins_pred.device) for b, c in enumerate(n)
+                                   if c]))
     return preds, img_inds
 
 

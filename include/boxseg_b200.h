@@ -345,44 +345,11 @@ int64_t bxs_dynconv1x1_backward_workspace_bytes(int64_t B, int64_t C, int64_t P,
 int bxs_dynconv1x1_backward(const float* feat, const float* kernels, const float* g_out, float* g_feat, float* g_kernels,
                             void* workspace, int64_t B, int64_t C, int64_t P, int64_t I, bxs_stream_t stream);
 
-/* a2  the dynamic convolution of the POSITIVE grid cells only, all levels and images in one launch
- *     replaces F.interpolate(F.conv2d(feature_pred, kernel_pred[l] cells, groups=B), (2h_l, 2w_l))[positives]
- *     (box_solov2_head.py:204-216 followed by the boolean indexing of :317-320).
- * Level l (n_levels) convolves operand level_op_host[l] (operands [B,C,op_size_host[o]] float32, e.g. feature_pred and
- * its bilinear resizes to the levels' output sizes; the levels of one operand are consecutive, level_op_host runs
- * 0, ..., n_ops-1 without gaps) with the positive cells of its raw kernel grid kernels_host[l] [B,C,S_l,S_l]
- * (S_l = grid_host[l]).  counts_host [n_levels*B]: positives of (level, image).  cells i32 [sum counts] on the device:
- * the cell index (gy*S_l + gx) of every positive, level-major, then image-major, ascending within a (level, image).
- * out_host[l] -> [n_l, op_size] with the rows in that order: exactly the rows the reference's boolean indexing keeps.
- * A problem is (operand, image): each operand is read once per image for all its levels.  The kernels are gathered
- * from the raw grids by a pack launch (K-major, in the workspace); then one TMA + wgmma launch (TF32, FP32 accumulate).
- * Backward: g_out_host[l] [n_l, op_size] ->
- *   g_operands_host[o] [B,C,op_size] (the roles-swapped product per problem; NULL: not needed) and
- *   g_kernels_host[l] [B,C,S_l,S_l] (split-K + an ordered reduce: positive cells get their gradient, every other cell 0;
- *   NULL: not needed).  Deterministic, no atomics.  Both need cells ascending within each (level, image).
- * A cell outside [0, S_l^2) acts as a zero kernel.  The *_host arrays are HOST arrays, copied into kernel parameters.
- * Limits: n_levels <= 8, n_ops <= 4, B <= 16, C % 32 == 0, C <= 256, op_size % 4 == 0, 16-byte aligned operands and
- * output gradients; d/d operand also needs sum over a problem's levels of round_up(count, 32) <= 256.
- * BXS_ERR_UNSUPPORTED outside them, BXS_ERR_INVALID_ARG for NULL pointers the shapes need, non-positive sizes, a count
- * outside [0, S_l^2] or a level_op_host that is not as described.  All checks run before any device call. */
-int64_t bxs_dynconv1x1_cells_forward_workspace_bytes(const int64_t* counts_host, int64_t n_levels, int64_t B, int64_t C);
-int bxs_dynconv1x1_cells_forward(const float* const* operands_host, const int64_t* op_size_host,
-                                 const float* const* kernels_host, const int64_t* grid_host, const int64_t* level_op_host,
-                                 const int64_t* counts_host, const int32_t* cells, float* const* out_host, void* workspace,
-                                 int64_t n_levels, int64_t n_ops, int64_t B, int64_t C, bxs_stream_t stream);
-int64_t bxs_dynconv1x1_cells_backward_workspace_bytes(const int64_t* op_size_host, const int64_t* grid_host,
-                                                      const int64_t* level_op_host, const int64_t* counts_host,
-                                                      int64_t n_levels, int64_t n_ops, int64_t B, int64_t C);
-int bxs_dynconv1x1_cells_backward(const float* const* operands_host, const int64_t* op_size_host,
-                                  const float* const* kernels_host, const int64_t* grid_host, const int64_t* level_op_host,
-                                  const int64_t* counts_host, const int32_t* cells, const float* const* g_out_host,
-                                  float* const* g_operands_host, float* const* g_kernels_host, void* workspace,
-                                  int64_t n_levels, int64_t n_ops, int64_t B, int64_t C, bxs_stream_t stream);
-
-/* a3  DiscoBox's dynamic kernels of the covered cells, packed for one dense convolution per network
- *     replaces the gather kernel_preds[l][b].view(C, -1)[:, grid_order] (discobox_head.py:1180-1189) of every (level, image):
- *     all levels of image b convolve the same s_ins_pred[b], so bxs_dynconv1x1_forward / _half_forward on the packed
- *     [B,I_pad,C] operand computes every (level, image) convolution of :1214-1227 in one call.
+/* a2 / a3  the dynamic kernels of some grid cells of every level, packed for one dense convolution per operand
+ *     replaces the gather kernel_preds[l][b].view(C, -1)[:, grid_order] (discobox_head.py:1180-1189) of every (level, image)
+ *     and BoxSOLOv2's positive cells (box_solov2_head.py:204-216 indexed as :317-320): the levels of image b that convolve
+ *     the same operand (DiscoBox's s_ins_pred[b], or one size of BoxSOLOv2's feature_pred[b]) share its rows, so
+ *     bxs_dynconv1x1_forward / _half_forward on the packed [B,I_pad,C] operand computes all their convolutions in one call.
  * grids_host[l] [B,C,S_l,S_l] (S_l = grid_host[l]) of the element type dtype (0 float32, 1 float16, 2 bfloat16);
  * counts_host [n_levels*B]: rows of (level, image); cells i32 [n_cells] on the device: the cell (gy*S_l + gx) of every row,
  * level-major, then image-major, each (level, image) in the order given (repeats allowed: DiscoBox appends a cell once per

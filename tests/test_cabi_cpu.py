@@ -42,7 +42,7 @@ def test_every_declared_symbol_is_exported_and_bound(lib):
 @pytest.mark.parametrize('name, argtypes, restype', [
     ('bxs_boxinst_targets_forward', [c_p] * 13 + [c_i64] * 3 + [c_int] * 3 + [c_f, c_p], c_int),
     ('bxs_corr_retrieve', [c_p] * 19 + [c_i64] * 8 + [c_f] * 6 + [c_int] * 2 + [c_p], c_int),
-    ('bxs_dynconv1x1_cells_forward', [c_p] * 9 + [c_i64] * 4 + [c_p], c_int),            # const float* const*
+    ('bxs_sigmoid_focal_loss_cells_forward', [c_p] * 7 + [c_i64] * 3 + [c_f] * 3 + [c_p], c_int),   # const float* const*
     ('bxs_lsap_workspace_bytes', [c_p, c_p, c_i64], c_i64),
     ('bxs_version', [], c_int),
     ('bxs_last_error', [], ctypes.c_char_p),

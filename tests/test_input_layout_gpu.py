@@ -588,12 +588,11 @@ def test_pairwise_ext_refuses_strided_like_the_reference(kind):
     assert torch.equal(pairwise_nlog(x, 3, 2), out)
 
 
-def test_solo_cells_backward_routes_by_count_not_by_status():
-    """d/d operand goes through cuBLAS exactly when a problem holds more than 256 kernels (counted on the host); an
-    operand or upstream gradient the kernel cannot take as it is gets an aligned copy instead of being mistaken for that."""
+def test_solo_cells_backward_routes_by_kernels_per_image():
+    """d/d operand goes through cuBLAS exactly when an image holds more than 256 kernels of one operand (``dynconv1x1``
+    decides from the shapes); an operand or upstream gradient the kernel cannot take as it is gets an aligned copy instead
+    of being mistaken for that."""
     from boxinstseg_b200.ops import dynconv
-    assert dynconv._cells_widest_problem([0, 0, 1], [[3, 40], [30, 1], [256, 0]]) == 256
-    assert dynconv._cells_widest_problem([0, 0], [[200, 1], [33, 1]]) == 224 + 64
     g = _gen(31)
     feat, k = _randn(g, 1, 32, 8, 8).to(DEV), _randn(g, 1, 32, 18, 18).to(DEV)
     cells = [[torch.arange(300)]]

@@ -1,6 +1,6 @@
-"""GPU parity of the positive-cell dynamic convolution (``ops.dynconv.solo_cells_conv``, bxs_dynconv1x1_cells_*) against
-the reference's lines in float64: ``F.interpolate(F.conv2d(feature_pred, kernel cells, groups=B), (h_l, w_l))`` indexed by
-the positive cells (box_solov2_head.py:204-216, 317-320).  The op resizes the operand instead of the result.
+"""GPU parity of the positive-cell dynamic convolution (``ops.dynconv.solo_cells_conv``: the cell pack and ``dynconv1x1``)
+against the reference's lines in float64: ``F.interpolate(F.conv2d(feature_pred, kernel cells, groups=B), (h_l, w_l))``
+indexed by the positive cells (box_solov2_head.py:204-216, 317-320).  The op resizes the operand instead of the result.
 
 Every case runs twice:
   * random data, judged element-wise (``scaled_err``, tests/helpers.py) against the float64 reference.  The op's
@@ -33,7 +33,7 @@ def _sizes(h, w):
 
 
 def _sizes8(h, w):
-    """8 levels over 4 operands: the cells table's limits (consecutive levels of one size share an operand)."""
+    """8 levels over 4 operands (consecutive levels of one size share an operand)."""
     f, half, quarter = (h, w), (h // 2, w // 2), (h // 4, w // 4)
     return [f, f, half, half, quarter, quarter, f, f]
 
@@ -168,7 +168,7 @@ def test_cells_config_d_shapes(h, w):
 
 @pytest.mark.parametrize('B', [1, 8, 16, 17, 33])
 def test_cells_batch_sizes(B):
-    """8 levels over 4 operands with random counts; 16 images fill one launch's table, 17 and 33 take two and three."""
+    """8 levels over 4 operands with random counts; 16 images fill one pack call's table, 17 and 33 take two and three."""
     gen = torch.Generator().manual_seed(B)
     h, w = 64, 80
     grids = (40, 36, 24, 16, 12, 12, 40, 36)
@@ -182,8 +182,8 @@ def test_cells_batch_sizes(B):
 # per level (8 levels, operands: levels 0-1 full size, 2-3 half, 4-5 quarter, 6-7 full again), per image (3: the middle one
 # without any positive); per (level, image) segment and per (operand, image) problem the kernel counts 0, 1, 31, 32, 33,
 # 127, 128 and 129 -- the edges of the 32-row K-blocks of d/d operand, the 128-row chunks of d/d kernel and the forward's
-# kernel chunks.  'native': the widest problem pads to exactly 256 kernels (operand 0, image 2: 128 + 128), the largest the
-# d/d operand kernel takes; 'fallback': operand 0, image 0 pads to 160 + 128 > 256, d/d operand through cuBLAS.
+# kernel chunks.  'native': the widest problem holds exactly 256 kernels (operand 0, image 2: 128 + 128), the most the
+# d/d operand kernel takes; 'fallback': operand 0, image 0 holds 129 + 128 > 256, d/d operand through cuBLAS.
 EDGE_GRIDS = (12, 16, 12, 12, 12, 12, 16, 12)
 EDGE_COUNTS = {
     'native': [[31, 0, 128], [1, 0, 128], [33, 0, 127], [0, 0, 0], [32, 0, 129], [0, 0, 1], [127, 0, 33], [0, 0, 31]],
@@ -195,11 +195,10 @@ EDGE_MAPS = {'native': (44, 48), 'fallback': (56, 72)}
 
 @pytest.mark.parametrize('table', ['native', 'fallback'])
 @pytest.mark.parametrize('C', [32, 96, 160, 224, 256])
-def test_cells_envelope_edges(C, table):
-    from boxinstseg_b200.ops.dynconv import _cells_widest_problem
+def test_cells_envelope_edges_per_image(C, table):
     counts = EDGE_COUNTS[table]
     level_op = [0, 0, 1, 1, 2, 2, 3, 3]
-    widest = _cells_widest_problem(level_op, counts)
+    widest = max(sum(n[b] for n, lo in zip(counts, level_op) if lo == o) for o in range(4) for b in range(3))
     assert widest == 256 if table == 'native' else widest > 256
     gen = torch.Generator().manual_seed(C)
     h, w = EDGE_MAPS[table]
@@ -224,6 +223,24 @@ def test_cells_every_cell_positive():
     _check(2, 256, h, w, grids, [(h, w), (h // 2, w // 2)], cells, seed=7)
     counts = [[129, 200], [0, 0]]                 # native d/d operand with 129..200 kernels per problem, C = 64
     _check(2, 64, h, w, grids, [(h, w), (h // 2, w // 2)], _cells(2, grids, gen, counts), seed=8)
+
+
+def test_cells_rows_beyond_one_pack():
+    """every cell of a 40x40 and a 36x36 level of one operand on image 0: 2896 rows, more than the 2048 of one pack call,
+    so they take two and level 1's rows of that image straddle them; image 1's 1600 rows fit the first."""
+    gen = torch.Generator().manual_seed(9)
+    grids, h, w = (40, 36), 32, 40
+    counts = [[1600, 700], [1296, 900]]
+    _check(2, 64, h, w, grids, [(h, w), (h, w)], _cells(2, grids, gen, counts), seed=9)
+
+
+def test_cells_grid_beyond_64_raises():
+    """the pack takes grids of at most 64 x 64 cells: a larger one is an error, never wrong rows."""
+    from boxinstseg_b200.ops.dynconv import solo_cells_conv
+    f = torch.randn(1, 32, 8, 8, device=DEV)
+    k = torch.randn(1, 32, 65, 65, device=DEV)
+    with pytest.raises(NotImplementedError, match='64 x 64'):
+        solo_cells_conv(f, [k], [[torch.arange(3, device=DEV)]], [(8, 8)])
 
 
 def test_cells_no_positive_at_all():
@@ -267,33 +284,3 @@ def test_dynamic_conv_cells_matches_dense():
     rows = head.dynamic_conv(feat, kp, out_size=(20, 24), cells=cells)
     for b in range(2):
         _elementwise(f'rows of image {b} against the dense path', rows[b], dense[b, cells[b]], TOL_OUT)
-
-
-def test_cells_c_abi_limits():
-    import ctypes
-    from boxinstseg_b200 import _lib as L
-    i64 = lambda v: (ctypes.c_int64 * len(v))(*v)    # noqa: E731
-    lib = L.lib()
-    f = torch.zeros(1, 32, 4, 4, device=DEV)
-    ptrs = (ctypes.c_void_p * 9)(*([f.data_ptr()] * 9))
-    cells = torch.zeros(1, dtype=torch.int32, device=DEV)
-    ws = torch.empty(1 << 20, dtype=torch.uint8, device=DEV)
-    # nine levels: beyond the limit
-    rc = lib.bxs_dynconv1x1_cells_forward(ptrs, i64([16]), ptrs, i64([2] * 9), i64([0] * 9), i64([0] * 9), L.ptr(cells),
-                                          ptrs, L.ptr(ws), 9, 1, 1, 32, L.stream())
-    assert rc == -3
-    # C not a multiple of 32
-    rc = lib.bxs_dynconv1x1_cells_forward(ptrs, i64([16]), ptrs, i64([2]), i64([0]), i64([1]), L.ptr(cells), ptrs,
-                                          L.ptr(ws), 1, 1, 1, 48, L.stream())
-    assert rc == -3
-    # a level_op that skips an operand; a count above S^2
-    rc = lib.bxs_dynconv1x1_cells_forward(ptrs, i64([16, 16]), ptrs, i64([2, 2]), i64([0, 2]), i64([1, 1]), L.ptr(cells),
-                                          ptrs, L.ptr(ws), 2, 2, 1, 32, L.stream())
-    assert rc == -1
-    rc = lib.bxs_dynconv1x1_cells_forward(ptrs, i64([16]), ptrs, i64([2]), i64([0]), i64([5]), L.ptr(cells), ptrs,
-                                          L.ptr(ws), 1, 1, 1, 32, L.stream())
-    assert rc == -1
-    # the first level must take operand 0
-    rc = lib.bxs_dynconv1x1_cells_forward(ptrs, i64([16]), ptrs, i64([2]), i64([1]), i64([1]), L.ptr(cells), ptrs,
-                                          L.ptr(ws), 1, 1, 1, 32, L.stream())
-    assert rc == -1
