@@ -1,2 +1,3 @@
 from .condinst import LogVars, mask_branch_step, parse_losses  # noqa: F401
-from .solo import BoxLevelSet, DiscoBoxSOLOv2, format_results  # noqa: F401  (registers the classes)
+from .discobox import DiscoBoxSOLOv2, forward_train, momentum_update  # noqa: F401  (registers the class)
+from .solo import BoxLevelSet, format_results  # noqa: F401  (registers the class)

@@ -59,8 +59,3 @@ class _FormatResults:
 @register(HEADS, partial=True)
 class BoxLevelSet(_FormatResults):
     """mmdet/models/detectors/boxlevelset.py: the reference's detector with ``format_results`` on one host wait."""
-
-
-@register(HEADS, partial=True)
-class DiscoBoxSOLOv2(_FormatResults):
-    """mmdet/models/detectors/discobox.py: the reference's detector with ``format_results`` on one host wait."""

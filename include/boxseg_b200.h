@@ -803,6 +803,32 @@ int64_t bxs_mask_rle_strings_workspace_bytes(int64_t n, int64_t R);
 int bxs_mask_rle_strings(const uint32_t* counts, const int64_t* offsets, int64_t n, int64_t R, void* workspace,
                          uint8_t* chars, int64_t* char_offsets, bxs_stream_t stream);
 
+/* ---------------------------------------------------------------------------------------
+ * f3  teacher momentum update             replaces SingleStageWSInsTeacherDetector.momentum_update's arithmetic
+ *     (mmdet/models/detectors/single_stage_ts.py:118-131: `cur * (1. - m) + self * m` per state-dict entry, then
+ *     load_state_dict's copy_ into the teacher).
+ * A table of n entries: entry k updates count_host[k] elements of the type dtype_host[k] (a bxs_ema_dtype_t) in place,
+ * t <- fl(fl(s * a) + fl(t * b)), with t the teacher region teacher_host[k] and s the student region student_host[k]
+ * (device pointers, dense), and a = ab_host[0] = 1 - m, b = ab_host[1] = m (HOST doubles, computed as Python does).
+ * Roundings are torch's, without fused multiply-add: float32 in float32 with a and b cast to float; float16 / bfloat16
+ * with each product and the sum computed in float and rounded to the dtype (nearest even); float64 in double; integer
+ * and bool entries promoted to float32 (nearest), combined in float32, then converted back as torch's copy_ does
+ * (toward zero; uint8 through int64; bool as != 0).
+ * The *_host arrays are HOST arrays, copied into the kernel parameters (no H2D copy: the call can be captured in a CUDA
+ * graph).  One launch per 1024 entries; entries of 64 KB chunks, 16-byte accesses where both regions are 16-byte aligned.
+ * No atomics, no host synchronisation; n == 0 and zero-count entries do no work.  A student region may alias its own
+ * teacher region element for element.  BXS_ERR_INVALID_ARG: a negative n or count, an unknown dtype, a NULL ab_host, a
+ * NULL region with a count above 0, two teacher regions that overlap, or a student region that overlaps a teacher region
+ * other than exactly its own.  BXS_ERR_UNSUPPORTED: one entry of 2^31 or more 64 KB chunks.  All checks run before any
+ * device call.
+ * --------------------------------------------------------------------------------------- */
+typedef enum {
+  BXS_EMA_F32 = 0, BXS_EMA_F16 = 1, BXS_EMA_BF16 = 2, BXS_EMA_F64 = 3, BXS_EMA_I64 = 4,
+  BXS_EMA_I32 = 5, BXS_EMA_I16 = 6, BXS_EMA_I8 = 7, BXS_EMA_U8 = 8, BXS_EMA_BOOL = 9
+} bxs_ema_dtype_t;
+int bxs_momentum_update(void* const* teacher_host, const void* const* student_host, const int64_t* count_host,
+                        const int32_t* dtype_host, int64_t n, const double* ab_host, bxs_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
