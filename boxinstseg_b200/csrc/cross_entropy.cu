@@ -3,8 +3,10 @@
 //     with mmdet's CrossEntropyLoss(use_sigmoid=False, reduction='mean', class_weight=w) (cross_entropy_loss.py, utils.py:
 //     weight_reduce_loss), once per decoder layer.
 //
-//     One warp owns one query row: a max-subtracted logsumexp over the K scores, the row's loss w[y] (lse - x_y) and its
-//     gradient w[y] (softmax - onehot(y)) * loss_weight / (avg_factor + FLT_EPSILON), written in the same pass.  avg_factor
+//     One warp owns one query row: with m the row maximum, d_k = x_k - m and ls = log sum_k exp(d_k), the row's loss
+//     w[y] (ls - d_y) and its gradient w[y] (exp(d_k - ls) - [k == y]) * loss_weight / (avg_factor + FLT_EPSILON), written
+//     in the same pass.  Every term stays relative to m, as in F.cross_entropy's log_softmax: adding m back (lse = m + ls)
+//     before subtracting would round the loss and the softmax to ulp(m), far coarser than a confident row's loss.  avg_factor
 //     = sum_i w[y_i] depends on the labels only: every CTA re-reads its layer's B*Q labels in one fixed order, so it is known
 //     on the device before the first gradient is written.  Each CTA leaves one FP32 partial; a second launch (one CTA per
 //     layer) sums them in a fixed order.  No atomics: loss and gradient are bit-identical from run to run.
@@ -74,14 +76,14 @@ __global__ void __launch_bounds__(CE_NT) ce_layers_kernel(const CeTable tab, con
     float s = 0.f;
     for (int64_t k = lane; k < K; k += kWarp) s += expf(xr[k] - m);
     s = warp_sum(s);
-    const float lse = m + logf(s);
+    const float ls = logf(s);                                  // log-sum-exp relative to the row maximum
     const int64_t y = lab[row];
     const float w = label_weight(y, K, cw);
-    if (lane == 0 && w != 0.f) acc += w * (lse - xr[y]);
+    if (lane == 0 && w != 0.f) acc += w * (ls - (xr[y] - m));
     if (g) {
       float* gr = g + row * K;
       const float ws = w * scale;
-      for (int64_t k = lane; k < K; k += kWarp) gr[k] = ws * (expf(xr[k] - lse) - (k == y ? 1.f : 0.f));
+      for (int64_t k = lane; k < K; k += kWarp) gr[k] = ws * (expf((xr[k] - m) - ls) - (k == y ? 1.f : 0.f));
     }
   }
   if (lane == 0) s_row[warp] = acc;
