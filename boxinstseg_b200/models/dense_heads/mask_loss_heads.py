@@ -121,10 +121,21 @@ class BoxSOLOv2Head(nn.Module):
         is a ``SoloInsPreds`` -- feature_pred, the raw kernel grids and the output sizes -- instead of the dense
         [B,S*S,h,w] predictions, which ``loss`` never needs (it convolves the positive cells only).  ``eval=True``: the
         reference's outputs, the sigmoid of the dense convolution (wgmma) and the local-max-masked category scores."""
+        kernel_pred, cate_pred, featmap_sizes, feature_pred = self._towers(feats, eval, 'forward')
+        levelset_feats = self.levelset_bottom(feature_pred)
+        if eval:
+            return [torch.sigmoid(self.dynamic_conv(feature_pred, k)) for k in kernel_pred], list(cate_pred), levelset_feats
+        ins_pred = SoloInsPreds(SoloLevelPred(feature_pred, k, (2 * s[0], 2 * s[1])) for k, s in zip(kernel_pred, featmap_sizes))
+        return ins_pred, list(cate_pred), levelset_feats
+
+    # box_solov2_head.py:181-202, the lines forward and simple_test share
+    def _towers(self, feats, eval, caller):
+        """(kernel_pred, cate_pred, featmap_sizes, feature_pred): the per-level raw kernel grids and category outputs of
+        ``forward_single`` and the mask features, everything ``forward`` computes before the dynamic convolution."""
         missing = [n for n in _SOLO_TOWERS if not hasattr(self, n)]
         if missing:
-            raise RuntimeError('BoxSOLOv2Head.forward needs the modules the reference constructor builds (mmdet installed); '
-                               f'this head has no {", ".join(missing)}')
+            raise RuntimeError(f'BoxSOLOv2Head.{caller} needs the modules the reference constructor builds (mmdet '
+                               f'installed); this head has no {", ".join(missing)}')
         feats = [feat.float() for feat in feats]
         new_feats = self.split_feats(feats)
         featmap_sizes = [featmap.size()[-2:] for featmap in new_feats]
@@ -134,12 +145,24 @@ class BoxSOLOv2Head(nn.Module):
         for i in range(1, 3):
             feature_add_all_level = feature_add_all_level + self.feature_convs[i](feats[i])
         feature_add_all_level = feature_add_all_level + self.feature_convs[3](torch.cat([feats[3], coord_feat], 1))
-        feature_pred = self.solo_mask(feature_add_all_level)
-        levelset_feats = self.levelset_bottom(feature_pred)
-        if eval:
-            return [torch.sigmoid(self.dynamic_conv(feature_pred, k)) for k in kernel_pred], list(cate_pred), levelset_feats
-        ins_pred = SoloInsPreds(SoloLevelPred(feature_pred, k, (2 * s[0], 2 * s[1])) for k, s in zip(kernel_pred, featmap_sizes))
-        return ins_pred, list(cate_pred), levelset_feats
+        return kernel_pred, cate_pred, featmap_sizes, self.solo_mask(feature_add_all_level)
+
+    def simple_test(self, feats, img_metas, rescale=False, cfg=None):
+        """``get_seg(*forward(feats, eval=True), img_metas, cfg, rescale)`` without the dense predictions: the towers run as
+        ``forward(eval=True)`` runs them (``levelset_bottom``, which ``get_seg`` never reads, is skipped), and only the
+        distinct cells whose category score passes ``score_thr`` are convolved, each once (``solo_seg.candidate_sources``).
+        Masks, labels and scores equal that expression's bit for bit, in float32, under float16 and under bfloat16 autocast.
+        ``cfg``: the test config (``score_thr``, ``mask_thr``, ``nms_pre``, ``max_per_img``, ``kernel``, ``sigma``,
+        ``filter_thr``); ``None`` reads ``self.test_cfg``.  ``rescale`` is accepted and, as in ``get_seg``, not used: the
+        masks are pasted at each image's ``ori_shape``.  Two host reads per call: the candidate counts and the kept counts."""
+        from .solo_seg import box_solov2_cells_get_seg
+        if cfg is None:
+            cfg = getattr(self, 'test_cfg', None)
+            if cfg is None:
+                raise ValueError('BoxSOLOv2Head.simple_test needs a test config: pass cfg or set the head\'s test_cfg')
+        with torch.no_grad():
+            kernel_pred, cate_pred, _, feature_pred = self._towers(feats, True, 'simple_test')
+            return box_solov2_cells_get_seg(list(cate_pred), list(kernel_pred), feature_pred, self.strides, img_metas, cfg)
 
     # box_solov2_head.py:219-224
     @staticmethod

@@ -3,8 +3,8 @@
 
   1. candidates ``cate > score_thr`` of every image; the distinct candidate rows (level, image, cell) -- a cell above the
      threshold for several classes is one row;
-  2. the rows' packed masks, areas and masked sums (``bxs_solo_mask_stats``; BoxSOLOv2 reads its per-level predictions in
-     place, DiscoBox convolves each distinct cell once);
+  2. the rows' packed masks, areas and masked sums (``bxs_solo_mask_stats``; BoxSOLOv2's ``get_seg`` reads its per-level
+     predictions in place, its ``simple_test`` and DiscoBox convolve each distinct cell once: ``candidate_sources``);
   3. the stride filter and mask scores per candidate, one stable descending sort per image with invalid slots at -inf,
      Matrix NMS for every image in one call (``bxs_matrix_nms``), a second stable sort;
   4. per image, the fused paste of the kept masks (``bxs_solo_paste_masks``).
@@ -16,7 +16,7 @@ import types
 import torch
 
 from ...ops import solo_seg as S
-from ...ops.dynconv import PACK_MAX_ROWS, _CellPack, dynconv1x1, row_chunks
+from ...ops.dynconv import PACK_MAX_ROWS, _CellPack, _image_groups, dynconv1x1, row_chunks
 
 try:                                            # pragma: no cover - mmdet is absent in this image
     from mmdet.core import InstanceData
@@ -89,34 +89,44 @@ class Candidates:
         self.cand_stride = stride_of[p]
 
 
-def _disco_sources(cands, kernel_preds, seg_pred):
-    """DiscoBox's candidate convolution: every distinct cell once, packed per image (``bxs_disco_cells_pack``, at most
-    PACK_MAX_ROWS rows per image and call: ``row_chunks``) and convolved by ``dynconv1x1`` under the caller's autocast.
-    Returns the row sources (one [B*I_pad, h, w] logit tensor per chunk) and the source row id of every distinct row."""
-    B, n_lv = cands.B, len(kernel_preds)
-    dev = seg_pred.device
-    h, w = seg_pred.shape[-2:]
+def candidate_sources(cands, kernel_grids, operand):
+    """The candidate convolution of both SOLOv2 heads: every distinct candidate cell once.
+
+    kernel_grids: per level the raw kernel grid [B,E,S,S] (S <= 64); operand [B,E,h,w].  The distinct cells' kernels are
+    packed per image (``bxs_disco_cells_pack``, in the grids' dtype, float32 for any other), one call per group of at most
+    PACK_MAX_IMAGES images and chunk of at most PACK_MAX_ROWS rows per image (``row_chunks``), and each chunk is convolved
+    by one ``dynconv1x1`` call under the caller's autocast.  Returns the row sources (one [B*I_pad, h, w] logit tensor per
+    chunk, read in place by the stats and paste kernels) and the source row id of every distinct row.  ``dynconv1x1``
+    gives each output element the same accumulation whatever the number of kernel rows, so a row equals the dense
+    convolution's row of that cell bit for bit."""
+    B, n_lv = cands.B, len(kernel_grids)
+    dev = operand.device
+    h, w = operand.shape[-2:]
     seg_start = [0]
     for l in range(n_lv):
         for b in range(B):
             seg_start.append(seg_start[-1] + cands.seg_counts[l][b])
     chunks = row_chunks(cands.seg_counts)
     if len(chunks) > S.MAX_SOURCES:
-        raise NotImplementedError(f'DiscoBoxSOLOv2Head.get_seg: more than {S.MAX_SOURCES * PACK_MAX_ROWS} distinct '
-                                  'candidate cells in one image')
-    dt = kernel_preds[0].dtype if kernel_preds[0].dtype in (torch.float32, torch.float16, torch.bfloat16) else torch.float32
-    grids = [k.detach().to(dt).contiguous() for k in kernel_preds]
+        raise NotImplementedError(f'SOLOv2 get_seg: more than {S.MAX_SOURCES * PACK_MAX_ROWS} distinct candidate cells '
+                                  'in one image')
+    dt = kernel_grids[0].dtype if kernel_grids[0].dtype in (torch.float32, torch.float16, torch.bfloat16) else torch.float32
+    grids = [k.detach().to(dt).contiguous() for k in kernel_grids]
     cells = cands.row_cell.to(torch.int32)
     sources, src_start = [], 0
     pieces = []                                   # (distinct-row start, length, source id base) of every sub-range
     for i_pad, counts, parts in chunks:
-        cell_parts = []
-        for l, b, j, n, r in parts:
-            r0 = seg_start[l * B + b] + j
-            cell_parts.append(cells[r0:r0 + n])
-            pieces.append((r0, n, src_start + b * i_pad + r))
-        packed = _CellPack.apply(counts, i_pad, torch.cat(cell_parts), *grids)
-        logits = dynconv1x1(seg_pred.detach(), packed)                                      # [B, i_pad, h, w]
+        group_packs = []
+        for b0, b1 in _image_groups(B):
+            cell_parts = [cells[seg_start[l * B + b] + j:seg_start[l * B + b] + j + n]
+                          for l, b, j, n, _ in parts if b0 <= b < b1]
+            flat = torch.cat(cell_parts) if cell_parts else torch.zeros(0, dtype=torch.int32, device=dev)
+            g_counts = [counts[l * B + b] for l in range(n_lv) for b in range(b0, b1)]
+            whole = b1 - b0 == B
+            group_packs.append(_CellPack.apply(g_counts, i_pad, flat, *[g if whole else g[b0:b1] for g in grids]))
+        packed = group_packs[0] if len(group_packs) == 1 else torch.cat(group_packs, 0)     # [B, i_pad, E]
+        pieces += [(seg_start[l * B + b] + j, n, src_start + b * i_pad + r) for l, b, j, n, r in parts]
+        logits = dynconv1x1(operand.detach(), packed)                                     # [B, i_pad, h, w]
         sources.append(logits.reshape(B * i_pad, h, w))
         src_start += B * i_pad
     pieces.sort()
@@ -190,6 +200,22 @@ def box_solov2_get_seg(seg_preds, cate_preds, strides, img_metas, cfg):
     return get_seg(cate_preds, grids, strides, img_metas, cfg, sources_of)
 
 
+def box_solov2_cells_get_seg(cate_preds, kernel_preds, feature_pred, strides, img_metas, cfg):
+    """BoxSOLOv2Head without its dense predictions: the distinct candidate cells of ``kernel_preds`` (per level the raw
+    grid [B,E,S,S]) convolved with ``feature_pred`` [B,E,h,w] once each (``candidate_sources``), under the caller's
+    autocast.  Bit for bit ``box_solov2_get_seg`` of ``forward(eval=True)``'s sigmoid rows: float32 and float16 logits go
+    to the stats and paste kernels, which apply torch's sigmoid for the dtype; bfloat16 logits, which those kernels do not
+    take, are turned into float32 probabilities as ``box_solov2_get_seg`` turns the dense bfloat16 rows."""
+    grids = [int(c.shape[1]) for c in cate_preds]
+
+    def sources_of(cands):
+        tensors, ids = candidate_sources(cands, kernel_preds, feature_pred)
+        if tensors[0].dtype not in S._DTYPE:
+            return [torch.sigmoid(t).float() for t in tensors], ids, False, False
+        return tensors, ids, True, False
+    return get_seg(cate_preds, grids, strides, img_metas, cfg, sources_of)
+
+
 def discobox_get_seg(cate_preds, kernel_preds, seg_pred, strides, img_metas, cfg, autocast=True):
     """DiscoBoxSOLOv2Head: the distinct candidate cells of ``kernel_preds`` (per level [B,E,S,S]) convolved with
     ``seg_pred`` [B,E,h,w] once each.  ``autocast``: under float16 autocast, as the reference's ``@autocast()`` runs
@@ -198,7 +224,7 @@ def discobox_get_seg(cate_preds, kernel_preds, seg_pred, strides, img_metas, cfg
     grids = [int(c.shape[1]) for c in cate_preds]
 
     def sources_of(cands):
-        tensors, ids = _disco_sources(cands, kernel_preds, seg_pred)
+        tensors, ids = candidate_sources(cands, kernel_preds, seg_pred)
         return tensors, ids, True, autocast
     with torch.autocast('cuda', dtype=torch.float16, enabled=autocast):
         return get_seg(cate_preds, grids, strides, img_metas, cfg, sources_of)

@@ -1,6 +1,8 @@
 """``format_results`` of the SOLOv2-family detectors -- ``SingleStageBoxInsDetector`` (mmdet/models/detectors/
 single_stage_boxseg.py:75-90, BoxLevelSet) and ``SingleStageWSInsDetector`` (single_stage_ts.py:88-103, DiscoBoxSOLOv2),
-whose two copies are the same function -- with one host wait per image instead of up to nine per detection.
+whose two copies are the same function -- with one host wait per image instead of up to nine per detection; and
+BoxLevelSet's ``simple_test`` (single_stage_boxseg.py:64-73) on ``BoxSOLOv2Head.simple_test``, which convolves only the
+candidate grid cells instead of all of them.
 
 Per image: one ``bxs_mask_extents`` call gives every mask's area and box; the masks and one packed float64 table of labels,
 scores, areas and boxes are copied to pinned host memory without blocking, and one event wait ends the device work.  The
@@ -11,6 +13,7 @@ import torch
 
 from ...ops import solo_seg as S
 from ..builder import HEADS, register
+from ..dense_heads.mask_loss_heads import BoxSOLOv2Head
 
 _BOX = [3, 4, 5, 6, 1]          # columns of the packed table that make a bbox row: x0, y0, x1, y1, score
 
@@ -58,4 +61,18 @@ class _FormatResults:
 
 @register(HEADS, partial=True)
 class BoxLevelSet(_FormatResults):
-    """mmdet/models/detectors/boxlevelset.py: the reference's detector with ``format_results`` on one host wait."""
+    """mmdet/models/detectors/boxlevelset.py: the reference's detector with ``format_results`` on one host wait and
+    ``simple_test`` on the candidate cells."""
+
+    def simple_test(self, img, img_meta, rescale=False):
+        """The reference's ``simple_test``: per image ``format_results`` of the head's results.  With this package's
+        ``BoxSOLOv2Head`` the results come from ``bbox_head.simple_test`` -- bit for bit those of ``get_seg`` on
+        ``bbox_head(x, eval=True)``, without the dense [B, S^2, h, w] predictions of every level; any other head runs the
+        reference's lines."""
+        x = self.extract_feat(img)
+        if isinstance(self.bbox_head, BoxSOLOv2Head):
+            results_list = self.bbox_head.simple_test(x, img_meta, rescale=rescale, cfg=self.test_cfg)
+        else:
+            outs = self.bbox_head(x, eval=True)
+            results_list = self.bbox_head.get_seg(*(tuple(outs) + (img_meta, self.test_cfg, rescale)))
+        return [self.format_results(results) for results in results_list]
