@@ -7,6 +7,7 @@ sm_90a kernels of libboxseg_b200:
   forward      -> ops.condinst.dynamic_mask_head   (a1: rel-coords + 3 dynamic 1x1 convs + aligned x2)
   get_targets  -> ops.boxinst.boxinst_targets      (a5: no host round trip, no per-GT Python loop)
   loss         -> ops.boxinst.boxinst_mask_loss    (a6+a7+a8 fused; no [N,8,H,W] tensors)
+                  ops.condinst.dice_mask_loss      (boxinst_enabled=False: the masks sampled in place, no [N,h,w] target)
 There is no CPU fallback: a missing extension raises.
 """
 import torch
@@ -162,12 +163,8 @@ class CondInstMaskHead(nn.Module):
             losses['loss_prj'] = prj
             losses['loss_pairwise'] = pair
         else:
-            _, bitmasks, _ = self.get_targets(gt_bboxes, gt_masks, imgs, img_metas)
-            gt = torch.cat(bitmasks, dim=0)[gt_inds].unsqueeze(1).to(mask_logits.dtype)
-            s = mask_logits.sigmoid().flatten(1)
-            t = gt.flatten(1)
-            dice = 1. - 2 * (s * t).sum(1) / ((s * s).sum(1) + (t * t).sum(1) + 1e-5)
-            losses['loss_mask'] = dice.mean()
+            from ...ops.condinst import dice_mask_loss
+            losses['loss_mask'] = dice_mask_loss(mask_logits, gt_masks, gt_inds, self.out_stride)
         return losses
 
     def _unfused_boxinst_loss(self, mask_logits, targets, gt_inds):

@@ -775,6 +775,47 @@ int bxs_condinst_paste_masks(const float* logits, int64_t n, int64_t h, int64_t 
                              int64_t H_out, int64_t W_out, int rescale, uint8_t* out, bxs_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------
+ * Mask-supervised CondInst   replaces the dice loss of CondInstMaskHead.loss with boxinst_enabled=False
+ *     (condinst_head.py:117-131 dice_coefficient, :1298-1341) and CondInstSegmHead.get_targets (:950-968).
+ * Mask table: B <= 64 images; mask_host[b] (a HOST array of device pointers) is image b's uint8 [G_b, H, W] masks (the
+ *   bytes of a uint8 or bool tensor), read in place at the element strides mask_strides_host[3b .. 3b+2] (any layout, no
+ *   alignment needed); gt_off_host i64 [B+1] (HOST) holds the images' first global ground-truth index, gt_off_host[0] = 0
+ *   and G_b = gt_off_host[b+1] - gt_off_host[b] >= 0.  H and W are shared by every image.
+ * bxs_condinst_dice_forward: logits f32 [N, h, w] (dense, 4-byte aligned), gt_inds i32 [N] (global ground-truth indices)
+ *   -> sums f32 [N,3] = per instance (I, S, T) = (sum sigmoid(x) t, sum sigmoid(x)^2, sum t^2) with t(y, x) = the byte
+ *   mask[gt][start + y*stride, start + x*stride] as a float (the reference's m[:, start::s, start::s].to(float)), and
+ *   loss f32 [1] = mean_i(1 - 2 I_i / (S_i + T_i + 1e-5)), each term in float32 in the reference's operation order.  The
+ *   sums accumulate in double per CTA, then in a fixed order.  A gt_inds entry outside [0, sum G_b) gives T = NaN (and a
+ *   NaN loss) instead of a fault.  workspace: bxs_condinst_dice_workspace_bytes(N, h, w) bytes.  Two launches.
+ * bxs_condinst_dice_backward: the same logits, gt_inds and table, the forward's sums and the upstream gradient g_loss (a
+ *   device scalar) -> g_logits f32 [N, h, w] = d loss / d logits.  One launch, one more read of the logits and targets.
+ * N == 0 is a no-op for both.  start + (h-1)*stride < H and start + (w-1)*stride < W.
+ * bxs_condinst_semantic_targets: labels_host[b] (HOST array of device pointers) i64 [G_b] -> areas i64 [sum G_b] = the
+ *   sum of each mask's byte values (a byte of 255 counts 255, as torch.sum), and targets i64 [B, oh, ow], oh =
+ *   |range(stride/2, H, stride)|, ow likewise: at the sampled pixel (stride/2 + stride*i, stride/2 + stride*j) the label
+ *   of the first ground truth of least weight, a ground truth weighing its area where its mask is non-zero and 1e8
+ *   elsewhere; num_classes where that least weight is 1e8 or the image has no ground truth.  A memset and two launches
+ *   (the area sum adds int64 partials with integer atomics: the same result in any order).
+ * No host synchronisation, no float atomics: deterministic.  BXS_ERR_INVALID_ARG: a NULL pointer the call needs, a
+ * negative count or stride, a non-positive size or stride, gt_off_host[0] != 0, a sampled pixel outside [H, W].
+ * BXS_ERR_UNSUPPORTED: more than 64 images, N > 65535, h*w near INT32_MAX, more than 65535 ground truths for the semantic
+ * targets.  All checks run before any device call.
+ * --------------------------------------------------------------------------------------- */
+int64_t bxs_condinst_dice_workspace_bytes(int64_t N, int64_t h, int64_t w);
+int bxs_condinst_dice_forward(const float* logits, const int32_t* gt_inds, int64_t N, int64_t h, int64_t w,
+                              const uint8_t* const* mask_host, const int64_t* mask_strides_host, const int64_t* gt_off_host,
+                              int64_t B, int64_t H, int64_t W, int64_t start, int64_t stride, float* sums, float* loss,
+                              void* workspace, bxs_stream_t stream);
+int bxs_condinst_dice_backward(const float* logits, const int32_t* gt_inds, int64_t N, int64_t h, int64_t w,
+                               const uint8_t* const* mask_host, const int64_t* mask_strides_host, const int64_t* gt_off_host,
+                               int64_t B, int64_t H, int64_t W, int64_t start, int64_t stride, const float* sums,
+                               const float* g_loss, float* g_logits, bxs_stream_t stream);
+int bxs_condinst_semantic_targets(const uint8_t* const* mask_host, const int64_t* mask_strides_host,
+                                  const int64_t* const* labels_host, const int64_t* gt_off_host, int64_t B, int64_t H,
+                                  int64_t W, int64_t stride, int64_t num_classes, int64_t* areas, int64_t* targets,
+                                  bxs_stream_t stream);
+
+/* ---------------------------------------------------------------------------------------
  * COCO RLE of instance masks   replaces pycocotools' mask.encode in mmdet's encode_mask_results (mmdet/core/mask/utils.py:
  *     38-65): rleEncode + rleToString of maskApi.c, byte for byte.
  * masks: n masks u8 [n, H, W] (the bytes of a bool or uint8 tensor, dense, row-major).  Walked in column-major order
