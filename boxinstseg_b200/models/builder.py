@@ -53,6 +53,7 @@ except Exception:                               # noqa: BLE001
     MODELS = Registry('models')
     HEADS = LOSSES = MODELS                      # builder.py:9-15 -- one shared registry
     MATCH_COST = Registry('Match Cost')
+    PIPELINES = Registry('pipeline')             # mmdet/datasets/builder.py; filled by `import boxinstseg_b200.datasets`
 
 
 def register(registry, partial=False, **kw):

@@ -870,6 +870,26 @@ typedef enum {
 int bxs_momentum_update(void* const* teacher_host, const void* const* student_host, const int64_t* count_host,
                         const int32_t* dtype_host, int64_t n, const double* ab_host, bxs_stream_t stream);
 
+/* ---------------------------------------------------------------------------------------
+ * box masks                              replaces the dense host array of GenerateBoxMask
+ *     (mmdet/datasets/pipelines/loading.py:647-668) and BitmapMasks.to_tensor's host-to-device copy
+ *     (mmdet/core/mask/structures.py:507-509) for masks that are rectangles.
+ * B images; sizes_host i64 [B, 3] = (G_b, H_b, W_b); rects_host i32 [sum G_b, 4] = (y0, x0, y1, x1), image-major, with
+ *   0 <= y0 <= y1 <= H_b and 0 <= x0 <= x1 <= W_b (an empty rectangle has y0 == y1 or x0 == x1); out_host[b] (a HOST
+ *   array of device pointers) is image b's dense [G_b, H_b, W_b] output of elem_bytes-byte elements, aligned to
+ *   elem_bytes -> out[g, y, x] = (y0_g <= y < y1_g && x0_g <= x < x1_g) ? one_bits : 0, one_bits being the bit pattern
+ *   of 1 in the output type (1 for uint8 / bool / int16 / int32, 0x3C00 float16, 0x3F80 bfloat16, 0x3F800000 float32).
+ * Every *_host array is a HOST array, copied into the kernel parameters (no host-to-device copy: the call can be
+ *   captured in a CUDA graph).  One launch per 64 images or 1792 rectangles.  Write-only: 16-byte stores on each row's
+ *   16-byte aligned part, no reads, no atomics, no host synchronisation.  Images with G_b * H_b * W_b == 0 do no work
+ *   (their out_host entry and, with G_b == 0, rects_host may be NULL).  BXS_ERR_INVALID_ARG: a negative B or size, a NULL
+ *   array the call needs, elem_bytes not 1, 2 or 4, one_bits outside [0, 2^(8 elem_bytes)), an output not aligned to
+ *   elem_bytes, a rectangle outside the order above.  BXS_ERR_UNSUPPORTED: H_b * W_b > 2^31 - 1.  All checks run
+ *   before any device call.
+ * --------------------------------------------------------------------------------------- */
+int bxs_box_masks_rasterize(void* const* out_host, const int32_t* rects_host, const int64_t* sizes_host, int64_t B,
+                            int elem_bytes, int64_t one_bits, bxs_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
